@@ -106,7 +106,7 @@ struct ConvertArgs {
                                        // (fused gather)
     uint32_t unit_tris;                // triangles per work unit (<= 32), chosen by the host for balance
     uint32_t n_units;
-    unsigned long long* trace;         // M2S_TRACE builds only: 16 globaltimer stamps per raster warp
+    unsigned long long* trace;         // M2S_TRACE builds only: 16 per-phase sums per raster warp (TraceSlot)
     // multi-GPU fused gather (world <= 1: off).  peer_out[p] / peer_xch[p] are rank p's final buffer and
     // exchange block mapped into this process (NVLink peer memory); every rank's fragment kernel stores its
     // records into ALL final buffers at its global offset.  xch block: [kMaxPeers][4] u64 =

@@ -116,15 +116,21 @@ __device__ __forceinline__ void tma_store_1d(void* dst_gmem, const void* src_sme
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// M2S_TRACE builds: per-warp SUMS over all the warp's units, 16 slots per raster warp (scripts/trace_raster.py).
+// Phases are clock64() deltas (SM cycles: the globaltimer ticks too coarsely for one unit); TR_PHASE adds the cycles
+// since the previous mark to its slot.  Fire-and-forget atomics: the trace adds no wait to the chain it measures.
+enum TraceSlot {
+    kTrLoadWait, kTrSetup, kTrWalkScan, kTrLarger, kTrReserve, kTrList, kTrShade, kTrUnitEnd, kTrTail,
+    kTrUnits, kTrDirectUnits, kTrGroups, kTrCycles, kTrNanos, kTrEntry
+};
 #ifdef M2S_TRACE
 __device__ __forceinline__ unsigned long long gtime() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
-#define STAMP(a, slot) do { if ((a).trace && lane == 0) (a).trace[((size_t)blockIdx.x * (blockDim.x >> 5) + warp) * 16 + (slot)] = gtime(); } while (0)
-#define STAMPV(a, slot, v) do { if ((a).trace && lane == 0) (a).trace[((size_t)blockIdx.x * (blockDim.x >> 5) + warp) * 16 + (slot)] = (v); } while (0)
-#define TNOW() gtime()
+#define TR_SLOT(s) (((size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * 16 + (s))
+#define TR_PHASE(a, s) do { const long long n_ = clock64(); if ((a).trace && (threadIdx.x & 31) == 0) atomicAdd((a).trace + TR_SLOT(s), (unsigned long long)(n_ - tr_prev_)); tr_prev_ = n_; } while (0)
+#define TR_ADD(a, s, v) do { if ((a).trace && (threadIdx.x & 31) == 0) atomicAdd((a).trace + TR_SLOT(s), (unsigned long long)(v)); } while (0)
 #else
-#define STAMPV(a, slot, v) do { } while (0)
-#define TNOW() 0ull
-#define STAMP(a, slot) do { } while (0)
+#define TR_PHASE(a, s) do { } while (0)
+#define TR_ADD(a, s, v) do { } while (0)
 #endif
 __device__ __forceinline__ void st_release_sys(unsigned long long* p, unsigned long long v) {
     asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
@@ -787,7 +793,11 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     WarpBlock<RK>& wb = *reinterpret_cast<WarpBlock<RK>*>(smem + (size_t)warp * sizeof(WarpBlock<RK>));
     const unsigned char* tri_bytes = reinterpret_cast<const unsigned char*>(a.tris);
-    STAMP(a, 11);
+#ifdef M2S_TRACE
+    long long tr_prev_ = clock64();
+    const long long tr_c0_ = tr_prev_;
+    const unsigned long long tr_ns0_ = gtime();
+#endif
 
 #ifdef M2S_EARLY_TRIGGER
     // PDL early trigger: one fragment-kernel CTA per SM becomes resident beside this CTA (37 KB of shared memory are
@@ -848,20 +858,28 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
     uint32_t phase = 0;
     Stash st;
     st.n_it = 0; st.cur_nb = 0; st.cur_total = 0; st.frags = 0; st.slots = 0; st.seen = 0;
-    STAMP(a, 0);
+    TR_PHASE(a, kTrEntry);
 
     while (unit < a.n_units) {
         const uint32_t t0 = unit * a.unit_tris;
         const uint32_t ntri = min(a.unit_tris, a.tri_count - t0);
         uint32_t next = 0xffffffffu;
+        // launches with a direct path and fewer than three units per warp: the next unit is claimed only once this unit's
+        // work is known (after its shading for a direct unit).  A direct unit shades anything from 0 to 16 groups of 32
+        // fragments; claimed up front, every warp would get its two units whatever they weigh, and the kernel would end with
+        // the warps that drew heavy ones.  Claimed late, a warp that is still shading leaves the remaining units to the
+        // warps that are done.  The late claim costs one exposed atomic round trip per unit: with more units per warp the
+        // weights average out and the claim stays up front.
+        const bool claim_late = kDirectOK && multi_round && a.world <= 1 && a.n_units < 3 * nwarps_total;
         if (lane == 0) {
-            if (a.n_units > nwarps_total) next = nwarps_total + atomicAdd(SCHED(a, 0), 1u);  // needed only after the set-up
+            if (a.n_units > nwarps_total && !claim_late) next = nwarps_total + atomicAdd(SCHED(a, 0), 1u);  // needed only after the set-up
             tma_store_wait_read();  // the previous unit's record store has finished reading wb.rec
         }
         mbar_wait(&wb.bar, phase);
         phase ^= 1;
         __syncwarp();
-        STAMP(a, 1);
+        TR_PHASE(a, kTrLoadWait);
+        TR_ADD(a, kTrUnits, 1);
 
         // ---- per-triangle stage: one lane per triangle ----
         uint32_t cnt = 0;
@@ -871,7 +889,7 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         Rec& myrec = wb.rec[lane];
         if ((uint32_t)lane < ntri) cnt = setup_triangle<RK>(wb.tri + lane * 9, a.tri_first + t0 + lane, a, tabs, ts, myrec);
         __syncwarp();
-        STAMP(a, 2);
+        TR_PHASE(a, kTrSetup);
         next = __shfl_sync(0xffffffffu, next, 0);
 
         // ---- small triangles: lane-per-triangle lock-step walk of the candidate box -> coverage mask ----
@@ -908,7 +926,6 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
                 else { f0 += a0; f1 += a1; f2 += a2; }
             }
         }
-        STAMP(a, 3);
         const uint32_t nh = (uint32_t)__popcll(hits);
         uint32_t incl_scan = nh;  // inclusive warp scan
 #pragma unroll
@@ -930,12 +947,17 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
             myrec.box = cnt ? ((unsigned)ts.w | ((unsigned)ts.h << 13) | (ts.incl << 26) | (small ? kBoxSmall : 0u)) : 0u;
         }
         __syncwarp();
-        STAMP(a, 4);
+        TR_PHASE(a, kTrWalkScan);
         // DIRECT path (REF96 / PACKED56, single GPU): when the unit's small triangles emit at most M2S_DIRECT_MAX fragments
         // this warp shades them itself, straight from the records in its shared-memory slice — no work item, no record
         // round trip through L2, no second kernel on the critical path.  The triangle staging area (dead since the set-up)
         // is the warp's output stage then, so the next unit's triangles start flying in after the shading instead of now.
         const bool direct = kDirectOK && multi_round && a.world <= 1 && total_small != 0 && total_small <= (uint32_t)M2S_DIRECT_MAX;
+        auto claim = [&]() {   // the next unit, claimed once this one's work is known
+            if (lane == 0) next = nwarps_total + atomicAdd(SCHED(a, 0), 1u);
+            next = __shfl_sync(0xffffffffu, next, 0);
+        };
+        if (claim_late && !direct) claim();
         if (!direct && lane == 0 && next < a.n_units) issue_load(next);
 
         // ---- all other triangles: the warp counts one triangle at a time, one lane per pixel row; the tall triangles of
@@ -981,12 +1003,14 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
             stash_unit_item<RK>(a, wb, unit, st, total_small, ntri, hits, (uint32_t)w, incl_scan - nh, lane);
             stash_flush<RK>(a, wb, unit, st, lane);
         }
-        STAMP(a, 5);
+        TR_PHASE(a, kTrLarger);
         if constexpr (kDirectOK) {
             if (direct) {
                 constexpr int kStride = Cfg<RK>::kStride;   // layout == raster kind for REF96 / PACKED56
                 static_assert(32 * kStride <= kUnitTris * kTriBytes, "the output stage lives in the triangle staging area");
                 const unsigned long long dfirst = stash_flush<RK>(a, wb, unit, st, lane, total_small);   // the stash area is free after this
+                TR_PHASE(a, kTrReserve);
+                TR_ADD(a, kTrDirectUnits, 1);
                 // every lane lists the covered pixels of its triangle at their place in the unit: slot | column << 5 | row << 11
                 unsigned short* list = reinterpret_cast<unsigned short*>(wb.pend);
                 {
@@ -1001,13 +1025,14 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
                     }
                 }
                 __syncwarp();
-                STAMP(a, 8);
-                STAMPV(a, 10, total_small);
+                TR_PHASE(a, kTrList);
                 direct_run<RK>(a, wb, total_small, dfirst, t0, base_prev, room, lane);
-                STAMP(a, 9);
+                TR_PHASE(a, kTrShade);
+                TR_ADD(a, kTrGroups, (total_small + 31) / 32);
                 // the stage was written through the generic proxy: every writer fences before the TMA engine writes there again
                 fence_proxy_async();
                 __syncwarp();
+                if (claim_late) claim();
                 if (lane == 0 && next < a.n_units) issue_load(next);
             }
         }
@@ -1024,9 +1049,8 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
             }
         }
         unit = next;
-        STAMP(a, 6);
+        TR_PHASE(a, kTrUnitEnd);
     }
-    STAMP(a, 7);
     // ---- help: tickets on the CTA's queue until no warp of the CTA can post any more ----
     if (lane == 0) atomicSub_block(&cq.active, 1u);
     for (;;) {
@@ -1056,12 +1080,9 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         stash_close_item<RK>(a, wb, eu, st, lane);
         stash_flush<RK>(a, wb, eu, st, lane);
     }
-    STAMP(a, 12);
     if (lane == 0) tma_store_wait_all();  // record stores are complete (not just read) before the kernel ends
-    STAMP(a, 13);
     // ---- last CTA out publishes the counts and re-arms the scheduler for the next launch ---------
     __syncthreads();
-    STAMP(a, 14);
     if (warp == 0) {
         uint32_t last = 0;
         unsigned long long tot = 0;
@@ -1096,6 +1117,11 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
             }
         }
     }
+#ifdef M2S_TRACE
+    TR_PHASE(a, kTrTail);
+    TR_ADD(a, kTrCycles, clock64() - tr_c0_);   // with kTrNanos: the SM clock the cycles convert at
+    TR_ADD(a, kTrNanos, gtime() - tr_ns0_);
+#endif
 }
 
 // A warp's staged records (shared memory) -> one contiguous span of global memory at byte offset `boff` of `dstbase`

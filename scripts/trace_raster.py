@@ -1,4 +1,8 @@
-"""Timeline of the raster kernel's warps (needs a -DM2S_TRACE build selected with M2S_LIB)."""
+"""Per-phase account of the raster kernel's warps (needs a -DM2S_TRACE build selected with M2S_LIB).
+
+Every raster warp sums the SM cycles (clock64) it spends in each phase over ALL its units; the kernel also records each
+warp's cycles and globaltimer nanoseconds from entry to exit, which give the SM clock the cycles convert at.
+usage: trace_raster.py [packed56|ref96] [density] [helmet|dh|quad]"""
 import os, sys, ctypes as C
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
@@ -10,28 +14,34 @@ which = sys.argv[3] if len(sys.argv) > 3 else "helmet"
 ctx = Context(0)
 scene = {"helmet": lambda: synth.helmet_standin(2048), "quad": synth.unit_quad, "dh": lambda: synth.damaged_helmet_standin(2048)}[which]()
 ds = ctx.upload(scene)
-nw = 132 * 16
+nw = torch.cuda.get_device_properties(0).multi_processor_count * 16
 tr = torch.zeros(nw * 16, dtype=torch.int64, device="cuda")
 _lib.lib().m2s_debug_set_trace(C.c_void_p(tr.data_ptr()))
+flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
 out = None
 for i in range(5):
-    tr.zero_()
+    flush.zero_(); tr.zero_(); torch.cuda.synchronize()   # cold L2, as in bench.py
     out = ctx.convert(ds, R, layout, flags=_abi.FLAG_UNCAPPED, capacity=6 * R * R, out=out.data if out else None)
 t = tr.cpu().numpy().reshape(nw, 16).astype(np.float64)
-t0 = t[:, 11][t[:, 11] > 0].min() if (t[:, 11] > 0).any() else t[:, 0][t[:, 0] > 0].min()
-names = ["start", "tma_done", "setup_done", "walk_done", "scan_done", "flush_done", "unit_end", "units_done", "list_done", "direct_done", "-", "kernel_entry", "help_done", "stores_done", "cta_synced"]
-if os.environ.get("TRACE_SETUP"):
-    names += ["s:prim_loaded", "s:quat_done", "s:scale_done", "s:raster_done"]
-print(f"{which} R={R} layout={layout}: device_ms={out.device_ms:.4f} total={out.total}")
-for k, n in enumerate(names):
-    v = t[:, k]; v = v[v > 0]
-    if len(v):
-        r = (v - t0) / 1e3
-        print(f"{n:12s} n={len(v):5d}  min {r.min():7.2f}  p50 {np.median(r):7.2f}  p90 {np.percentile(r, 90):7.2f}  max {r.max():7.2f} us")
-d = (t[:, 9] - t[:, 8]) / 1e3; n = t[:, 10]; m = (t[:, 9] > 0)
-if m.any():
-    print("direct shading per warp: us p50 %.2f p90 %.2f max %.2f; fragments p50 %d max %d; us per 32-fragment group p50 %.2f" % (np.median(d[m]), np.percentile(d[m], 90), d[m].max(), np.median(n[m]), n[m].max(), np.median(d[m] / np.maximum(1, np.ceil(n[m] / 32)))))
-sys.exit(0)
-it = t[:, 12]
-print("drain items/warp: mean %.1f max %d; per-item us: load %.2f setup %.2f raster+flush %.2f" % (
-    it.mean(), it.max(), t[:, 13].sum() / max(it.sum(), 1) / 1e3, t[:, 14].sum() / max(it.sum(), 1) / 1e3, t[:, 15].sum() / max(it.sum(), 1) / 1e3))
+_lib.lib().m2s_debug_set_trace(None)
+# slots: enum TraceSlot in m2s_kernels.cu
+PHASES = ["triangle-load wait", "set-up", "walk + scan", "larger tris + flush", "reservation wait", "listing",
+          "direct shading", "unit end (stores)", "tail (help, last CTA)"]
+UNITS, DUNITS, GROUPS, CYC, NS, ENTRY = 9, 10, 11, 12, 13, 14
+live = t[:, CYC] > 0
+t = t[live]
+mhz = t[:, CYC].sum() / t[:, NS].sum() * 1e3
+print(f"{which} R={R} layout={layout}: device_ms={out.device_ms:.4f} total={out.total} warps={len(t)} SM clock {mhz:.0f} MHz (clock64 / globaltimer)")
+print(f"units/warp p50 {np.median(t[:, UNITS]):.0f} max {t[:, UNITS].max():.0f}; direct units/warp p50 {np.median(t[:, DUNITS]):.0f}; "
+      f"32-fragment groups/warp p50 {np.median(t[:, GROUPS]):.1f} max {t[:, GROUPS].max():.0f}")
+us = lambda c: c / mhz
+print(f"{'phase (per-warp sum)':24s} {'p50 us':>8s} {'p90 us':>8s} {'mean us':>8s}")
+for k, n in enumerate(PHASES + ["entry (tables)"]):
+    v = us(t[:, ENTRY if n == "entry (tables)" else k])
+    print(f"{n:24s} {np.median(v):8.2f} {np.percentile(v, 90):8.2f} {v.mean():8.2f}")
+v = us(t[:, CYC])
+print(f"{'warp entry -> exit':24s} {np.median(v):8.2f} {np.percentile(v, 90):8.2f} {v.mean():8.2f}")
+g = t[:, GROUPS] > 0
+if g.any():
+    pg = us(t[g, 6]) / t[g, GROUPS]
+    print(f"direct shading per 32-fragment group: p50 {np.median(pg):.3f} us  p90 {np.percentile(pg, 90):.3f} us")
