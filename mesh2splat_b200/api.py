@@ -153,6 +153,20 @@ class Context:
         return ConvertOutput(out, keys, int(res.total), int(res.written), int(res.cap), float(res.device_ms), layout,
                              st == _abi.M2S_E_CAPACITY)
 
+    def convert_plan(self, dscene: DeviceScene, resolution: int, layout: int = _abi.LAYOUT_REF96, capacity: int = 0,
+                     max_gaussians: int = 0, flags: int = 0, first_triangle: int = 0,
+                     triangle_count: int = 0) -> _abi.m2s_convert_plan:
+        """The launch plan convert() makes for the same arguments (m2s_debug_convert_plan): grid, work units, item
+        sizes, effective cap and the raster kernel's route (multi_round, direct_ok, claim_late)."""
+        L = lib()
+        fn = L.m2s_debug_convert_plan
+        fn.restype = C.c_int
+        fn.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(_abi.m2s_params), C.c_uint64, C.POINTER(_abi.m2s_convert_plan)]
+        p = _abi.make_params(resolution, layout, 0.65, max_gaussians, flags, first_triangle, triangle_count)
+        plan = _abi.m2s_convert_plan()
+        check(fn(self.handle, dscene.handle, C.byref(p), capacity, C.byref(plan)))
+        return plan
+
     def convert_enqueue(self, dscene: DeviceScene, params: _abi.m2s_params, out, capacity: int, keys=None,
                         total=None, stream: int = 0) -> None:
         """Enqueue only (no synchronisation); out/keys/total are torch device tensors."""
@@ -161,13 +175,16 @@ class Context:
                                         total.data_ptr() if total is not None else None, stream or None))
 
     def prepass(self, records, count: int, layout: int, world_to_view, view_to_clip, model_to_world, resolution, near_far,
-                std_dev: float, render_mode: int = 0):
+                std_dev: float, render_mode: int = 0, quads=None, depths=None):
         """GaussiansPrepass::execute on device-resident records (a torch uint8 tensor, e.g. ConvertOutput.data): returns
-        (quads [m, 24] float32, depths [m] float32) as numpy arrays, in atomic arrival order (m2s_prepass)."""
+        (quads [m, 24] float32, depths [m] float32) as numpy arrays, in atomic arrival order (m2s_prepass).
+        quads / depths: optional caller-owned device tensors of at least count * 96 bytes / count floats."""
         import torch
         dev = records.device
-        quads = torch.empty(max(1, count) * _abi.QUAD_BYTES, dtype=torch.uint8, device=dev)
-        depths = torch.empty(max(1, count), dtype=torch.float32, device=dev)
+        if quads is None:
+            quads = torch.empty(max(1, count) * _abi.QUAD_BYTES, dtype=torch.uint8, device=dev)
+        if depths is None:
+            depths = torch.empty(max(1, count), dtype=torch.float32, device=dev)
         p = _abi.make_prepass_params(world_to_view, view_to_clip, model_to_world, resolution, near_far, std_dev, render_mode, layout)
         valid = C.c_uint32(0)
         check(lib().m2s_prepass(self.handle, records.data_ptr(), count, C.byref(p), quads.data_ptr(), depths.data_ptr(), C.byref(valid)))
@@ -182,8 +199,9 @@ class Context:
 
     def convert_host(self, scene: _abi.Scene, resolution: int, layout: int = _abi.LAYOUT_REF96,
                      gaussian_std: float = 0.65, max_gaussians: int = 0, flags: int = 0, capacity: int | None = None,
-                     want_keys: bool = False, out: np.ndarray | None = None, c_scene=None):
-        """Host buffers in, host buffers out (m2s_convert_host). Returns (records, keys, result)."""
+                     want_keys: bool = False, out: np.ndarray | None = None, c_scene=None, keys: np.ndarray | None = None):
+        """Host buffers in, host buffers out (m2s_convert_host). Returns (records, keys, result).
+        out / keys: optional caller-owned host arrays (uint8, >= capacity * stride bytes / uint64, >= capacity)."""
         stride = _abi.STRIDES[layout]
         if capacity is None:
             if max_gaussians:
@@ -194,7 +212,8 @@ class Context:
                 capacity = _abi.reference_capacity(resolution, len(scene.primitives))
         if out is None:
             out = np.empty(max(1, capacity) * stride, np.uint8)
-        keys = np.empty(max(1, capacity), np.uint64) if want_keys else None
+        if want_keys and keys is None:
+            keys = np.empty(max(1, capacity), np.uint64)
         cs, keep = c_scene if c_scene is not None else scene.c_struct()
         p = _abi.make_params(resolution, layout, gaussian_std, max_gaussians, flags)
         res = _abi.m2s_result()

@@ -571,6 +571,75 @@ static uint64_t effective_cap(const m2s_dscene* s, const m2s_params* p, uint64_t
     return std::min(cap, out_capacity);
 }
 
+// The launch plan of one conversion: what the two kernels are launched with and which route the raster kernel takes.
+// One function computes it for the launch and for m2s_debug_convert_plan, so the route a test reads is the route the
+// kernel runs.  Every field is a u64 (the ctypes mirror is _abi.m2s_convert_plan).
+struct ConvertPlan {
+    uint64_t grid, raster_warps;      // raster CTAs, and their warps
+    uint64_t unit_tris, n_units;      // work units of the triangle range
+    uint64_t item_max, flush_frags;   // fragment work-item sizes
+    uint64_t queue_cap;               // work-item queue slots
+    uint64_t cap;                     // records stored (the effective cap)
+    uint64_t multi_round;             // n_units > raster_warps: the warps take several units each
+    uint64_t direct_ok;               // the raster kernel shades light units itself (PACKED56, multi-round, one GPU)
+    uint64_t claim_late;              // ... and claims a warp's next unit once its current one is done (< 3 units per warp)
+    uint64_t direct_max;              // M2S_DIRECT_MAX: the heaviest unit (small-triangle fragments) the direct path takes
+};
+
+static void convert_plan(const m2s_ctx* ctx, const m2s_dscene* s, const m2s_params* p, uint64_t out_capacity, uint32_t world,
+                         ConvertPlan* pl) {
+    const uint64_t first = std::min<uint64_t>(p->first_triangle, s->ntri);
+    uint64_t count = p->triangle_count;
+    if (count == 0 || first + count > s->ntri) count = s->ntri - first;
+    const int klayout = (int)p->layout;
+    pl->cap = effective_cap(s, p, out_capacity);
+    pl->grid = (uint64_t)ctx->sm_count * ctx->blocks_per_sm[klayout];
+    pl->raster_warps = pl->grid * convert_warps_per_cta(klayout);
+    // work-unit size: as large as 32 triangles, but small enough that every warp of the grid gets the
+    // same number of units (a 70 k-triangle mesh is only ~1 unit of 32 per resident warp)
+    const uint64_t warps = pl->raster_warps;
+    const uint64_t rounds = std::max<uint64_t>(1, (count + warps * kUnitTris - 1) / (warps * kUnitTris));
+    pl->unit_tris = std::min<uint64_t>(std::max<uint64_t>((count + warps * rounds - 1) / (warps * rounds), 1), kUnitTris);
+    pl->n_units = (count + pl->unit_tris - 1) / pl->unit_tris;
+    // work-item granularity: ~8 items per SM at the expected output (O(2 R^2) fragments) so that small conversions
+    // still spread over the GPU, at most 2048 fragments; an oversized row block (<= 32 rows x R pixels) takes at most
+    // kMaxSplit queue slots
+    uint32_t item_max = (uint32_t)std::min<uint64_t>(kItemMaxFrags, (2ull * p->resolution * p->resolution) / ((uint64_t)ctx->sm_count * 8));
+    item_max = std::max<uint32_t>({item_max, 64u, (32u * p->resolution + kMaxSplit - 1) / kMaxSplit});
+    item_max = std::min<uint32_t>((item_max + 31u) & ~31u, kItemMaxFrags);
+    pl->item_max = item_max;
+    pl->flush_frags = std::max<uint32_t>(32u, item_max / 2);
+    // item queue: a warp stops taking slots once it has seen the counter pass the cap, so live items cover disjoint
+    // output ranges below it: per unit one item of small triangles and one end-of-unit item, cap/32 items closed by
+    // 32 non-empty blocks, cap/flush closed by their fragment count, cap/item_max pieces of oversized blocks; plus
+    // ONE reservation per raster warp that may straddle the cap (< 2 kMaxSplit + kStashItems slots).  The queue
+    // cannot overflow.
+    pl->queue_cap = std::min<uint64_t>(2 * pl->n_units + pl->cap / 32 + pl->cap / pl->flush_frags + pl->cap / pl->item_max +
+                                       warps * (2ull * kMaxSplit + kStashItems) + 64, (1u << 24) - 1);
+    pl->multi_round = pl->n_units > warps;
+#ifndef M2S_EXP_NODIRECT
+    pl->direct_ok = klayout == M2S_LAYOUT_PACKED56 && pl->multi_round && world <= 1;
+#else
+    pl->direct_ok = 0;
+#endif
+    // the late claim evens out the weights of the direct units when each warp gets only two of them; with more units
+    // per warp they average out anyway and the claim's exposed atomic round trip is not worth it (DESIGN §4)
+    pl->claim_late = pl->direct_ok && pl->n_units < 3 * warps;
+    pl->direct_max = M2S_DIRECT_MAX;
+}
+
+// Test and tuning aid (not part of m2s.h): the plan m2s_convert would launch with for these arguments.  `plan` receives
+// the fields of ConvertPlan in order.
+extern "C" __attribute__((visibility("default"))) m2s_status m2s_debug_convert_plan(m2s_ctx* ctx, const m2s_dscene* s, const m2s_params* p,
+                                                                                  uint64_t out_capacity, uint64_t* plan) {
+    if (!ctx || !s || !p || !plan) { set_error("m2s_debug_convert_plan: NULL argument"); return M2S_E_INVALID; }
+    if (p->resolution < 1 || p->resolution > 4096 || p->layout > M2S_LAYOUT_PLY_COMPRESSED) { set_error("m2s_debug_convert_plan: bad params"); return M2S_E_INVALID; }
+    ConvertPlan pl;
+    convert_plan(ctx, s, p, out_capacity, 1u, &pl);
+    std::memcpy(plan, &pl, sizeof(pl));
+    return M2S_OK;
+}
+
 static m2s_status convert_enqueue_impl(m2s_ctx* ctx, const m2s_dscene* s, const m2s_params* p, void* d_out, uint64_t out_capacity,
                                        uint64_t* d_keys, uint64_t* d_total, void* stream_, const m2s_peers* peers,
                                        const unsigned long long* prev_totals = nullptr, uint32_t nprev = 0,
@@ -591,39 +660,15 @@ static m2s_status convert_enqueue_impl(m2s_ctx* ctx, const m2s_dscene* s, const 
     if (count == 0 || first + count > s->ntri) count = s->ntri - first;
     CUDA_TRY(cudaSetDevice(ctx->device));
     cudaStream_t stream = stream_ ? (cudaStream_t)stream_ : ctx->stream;
-    const uint64_t cap = effective_cap(s, p, out_capacity);
     const int klayout = (int)p->layout;  // every layout, the .ply rows included, is written by the fragment kernel itself
     void* kout = d_out;
     if (reinterpret_cast<uintptr_t>(kout) & 15u) { set_error("m2s_convert: the output buffer must be 16-byte aligned"); return M2S_E_INVALID; }
-    const int grid = ctx->sm_count * ctx->blocks_per_sm[klayout];
-    // work-unit size: as large as 32 triangles, but small enough that every warp of the grid gets the
-    // same number of units (a 70 k-triangle mesh is only ~1 unit of 32 per resident warp)
-    uint64_t unit_tris, n_units;
-    {
-        const uint64_t warps = (uint64_t)grid * convert_warps_per_cta(klayout);
-        const uint64_t rounds = std::max<uint64_t>(1, (count + warps * kUnitTris - 1) / (warps * kUnitTris));
-        unit_tris = (count + warps * rounds - 1) / (warps * rounds);
-        unit_tris = std::min<uint64_t>(std::max<uint64_t>(unit_tris, 1), kUnitTris);
-        n_units = (count + unit_tris - 1) / unit_tris;
-    }
-    // work-item granularity: ~8 items per SM at the expected output (O(2 R^2) fragments) so that small conversions
-    // still spread over the GPU, at most 2048 fragments; an oversized row block (<= 32 rows x R pixels) takes at most
-    // kMaxSplit queue slots
-    uint32_t item_max = (uint32_t)std::min<uint64_t>(kItemMaxFrags, (2ull * p->resolution * p->resolution) / ((uint64_t)ctx->sm_count * 8));
-    item_max = std::max<uint32_t>({item_max, 64u, (32u * p->resolution + kMaxSplit - 1) / kMaxSplit});
-    item_max = std::min<uint32_t>((item_max + 31u) & ~31u, kItemMaxFrags);
-    const uint32_t flush_frags = std::max<uint32_t>(32u, item_max / 2);
-    // item queue: a warp stops taking slots once it has seen the counter pass the cap, so live items cover disjoint
-    // output ranges below it: per unit one item of small triangles and one end-of-unit item, cap/32 items closed by
-    // 32 non-empty blocks, cap/flush closed by their fragment count, cap/item_max pieces of oversized blocks; plus
-    // ONE reservation per raster warp that may straddle the cap (< 2 kMaxSplit + kStashItems slots).  The queue
-    // cannot overflow.
-    const uint64_t raster_warps = (uint64_t)grid * convert_warps_per_cta(klayout);
-    const uint64_t queue_cap = std::min<uint64_t>(2 * n_units + cap / 32 + cap / flush_frags + cap / item_max +
-                                                  raster_warps * (2ull * kMaxSplit + kStashItems) + 64, (1u << 24) - 1);
+    ConvertPlan pl;
+    convert_plan(ctx, s, p, out_capacity, (peers && peers->world > 1) ? peers->world : 1u, &pl);
+    const uint64_t cap = pl.cap;
     {   // scratch between the two kernels (grown on demand, kept by the context)
         m2s_status st = grow(ctx, &ctx->d_trifrag, &ctx->trifrag_bytes, std::max<uint64_t>(count, 1) * tri_frag_bytes(klayout), stream);
-        if (st == M2S_OK) st = grow(ctx, &ctx->d_items, &ctx->items_bytes, queue_cap * sizeof(FragItem), stream);
+        if (st == M2S_OK) st = grow(ctx, &ctx->d_items, &ctx->items_bytes, pl.queue_cap * sizeof(FragItem), stream);
         if (st != M2S_OK) return st;
     }
     if (ctx->dirty) {
@@ -646,9 +691,9 @@ static m2s_status convert_enqueue_impl(m2s_ctx* ctx, const m2s_dscene* s, const 
     a.log_sz = logf(1e-7f * a.mult);
     a.tri_frag = (unsigned char*)ctx->d_trifrag;
     a.items = (FragItem*)ctx->d_items;
-    a.queue_cap = (uint32_t)queue_cap;
-    a.item_max_frags = item_max;
-    a.flush_frags = flush_frags;
+    a.queue_cap = (uint32_t)pl.queue_cap;
+    a.item_max_frags = (uint32_t)pl.item_max;
+    a.flush_frags = (uint32_t)pl.flush_frags;
     a.n_items_out = ctx->d_nitems;
     a.out = (uint8_t*)kout;
     a.cap = cap;
@@ -661,8 +706,10 @@ static m2s_status convert_enqueue_impl(m2s_ctx* ctx, const m2s_dscene* s, const 
     a.host_total = host_total;
     a.host_tag = host_tag;
     a.sched = ctx->d_sched;
-    a.unit_tris = (uint32_t)unit_tris;
-    a.n_units = (uint32_t)n_units;
+    a.unit_tris = (uint32_t)pl.unit_tris;
+    a.n_units = (uint32_t)pl.n_units;
+    a.direct_ok = (uint32_t)pl.direct_ok;
+    a.claim_late = (uint32_t)pl.claim_late;
     a.trace = g_trace;
     if (peers && peers->world > 1) {
         a.world = peers->world; a.rank = peers->rank;
@@ -672,7 +719,7 @@ static m2s_status convert_enqueue_impl(m2s_ctx* ctx, const m2s_dscene* s, const 
         a.status = ctx->d_status;
     }
     const int fgrid = ctx->sm_count * ctx->frag_blocks_per_sm[klayout];
-    cudaError_t e = convert_launch(klayout, a, grid, fgrid, stream, mid);
+    cudaError_t e = convert_launch(klayout, a, (int)pl.grid, fgrid, stream, mid);
     if (e != cudaSuccess) { ctx->dirty = true; set_error(std::string("convert launch: ") + cudaGetErrorString(e)); return M2S_E_CUDA; }
     if (peers && peers->world > 1)
         CUDA_TRY(gather_wait_launch((const unsigned long long*)peers->xch[peers->rank], peers->world, a.epoch, out_capacity,

@@ -18,6 +18,9 @@ constexpr uint32_t kDeferBlocks = 4;      // row blocks per help-queue entry
 constexpr uint32_t kMaxSplit = 64;       // queue slots one oversized row block can take (item_max_frags >= R / 2)
 constexpr unsigned long long kFragMask = (1ull << 40) - 1;  // ConvertArgs::counter: fragments | queue slots << 40
 constexpr float kGuard = 8192.0f;        // window-coordinate guard band (|xw| beyond -> triangle dropped)
+#ifndef M2S_DIRECT_MAX
+#define M2S_DIRECT_MAX 512   // a unit whose small triangles emit at most this many fragments is shaded by the raster kernel itself (<= 1024)
+#endif
 
 // ---- raster_kernel -> fragment_kernel interface (context-owned scratch, L2-resident at the sizes of interest) ----
 // The raster kernel only COUNTS: per triangle it leaves a record (TriRec, m2s_kernels.cu) holding the exact edge
@@ -106,6 +109,8 @@ struct ConvertArgs {
                                        // (fused gather)
     uint32_t unit_tris;                // triangles per work unit (<= 32), chosen by the host for balance
     uint32_t n_units;
+    uint32_t direct_ok;                // the raster kernel may shade light units itself (ConvertPlan::direct_ok)
+    uint32_t claim_late;               // ... and claims its next unit once the current one is done (ConvertPlan::claim_late)
     unsigned long long* trace;         // M2S_TRACE builds only: 16 per-phase sums per raster warp (TraceSlot)
     // multi-GPU fused gather (world <= 1: off).  peer_out[p] / peer_xch[p] are rank p's final buffer and
     // exchange block mapped into this process (NVLink peer memory); every rank's fragment kernel stores its

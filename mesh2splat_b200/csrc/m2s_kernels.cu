@@ -772,9 +772,6 @@ template <int STRIDE>
 __device__ __forceinline__ void copy_span(uint8_t* dstbase, unsigned long long boff, const unsigned char* stage, uint32_t nbytes, int lane);
 template <int STRIDE>
 __device__ __forceinline__ uint32_t stage_shift(unsigned long long record_index);
-#ifndef M2S_DIRECT_MAX
-#define M2S_DIRECT_MAX 512   // a unit whose small triangles emit at most this many fragments is shaded by the raster kernel itself (<= 1024)
-#endif
 // DIRECT path: the fragments of a light unit's small triangles, listed in the unit's shared-memory slice, are shaded
 // by the warp that rasterised them, in groups of 32 (direct_run).  Used when the warps have several units each
 // (n_units > resident warps: on an H100 (132 SMs x 16 warps x 32 triangles) meshes of > 67 k triangles, where most units emit a handful of fragments and a work item
@@ -854,7 +851,6 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
 #else
     constexpr bool kDirectOK = false;
 #endif
-    const bool multi_round = a.n_units > nwarps_total;   // the warps take several units each
     uint32_t phase = 0;
     Stash st;
     st.n_it = 0; st.cur_nb = 0; st.cur_total = 0; st.frags = 0; st.slots = 0; st.seen = 0;
@@ -869,8 +865,8 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         // fragments; claimed up front, every warp would get its two units whatever they weigh, and the kernel would end with
         // the warps that drew heavy ones.  Claimed late, a warp that is still shading leaves the remaining units to the
         // warps that are done.  The late claim costs one exposed atomic round trip per unit: with more units per warp the
-        // weights average out and the claim stays up front.
-        const bool claim_late = kDirectOK && multi_round && a.world <= 1 && a.n_units < 3 * nwarps_total;
+        // weights average out and the claim stays up front.  The host decides (ConvertPlan::claim_late).
+        const bool claim_late = kDirectOK && a.claim_late != 0;
         if (lane == 0) {
             if (a.n_units > nwarps_total && !claim_late) next = nwarps_total + atomicAdd(SCHED(a, 0), 1u);  // needed only after the set-up
             tma_store_wait_read();  // the previous unit's record store has finished reading wb.rec
@@ -952,7 +948,7 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         // this warp shades them itself, straight from the records in its shared-memory slice — no work item, no record
         // round trip through L2, no second kernel on the critical path.  The triangle staging area (dead since the set-up)
         // is the warp's output stage then, so the next unit's triangles start flying in after the shading instead of now.
-        const bool direct = kDirectOK && multi_round && a.world <= 1 && total_small != 0 && total_small <= (uint32_t)M2S_DIRECT_MAX;
+        const bool direct = kDirectOK && a.direct_ok != 0 && total_small != 0 && total_small <= (uint32_t)M2S_DIRECT_MAX;
         auto claim = [&]() {   // the next unit, claimed once this one's work is known
             if (lane == 0) next = nwarps_total + atomicAdd(SCHED(a, 0), 1u);
             next = __shfl_sync(0xffffffffu, next, 0);

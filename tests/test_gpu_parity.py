@@ -35,25 +35,42 @@ def check(ctx, scene, R, layout=LAYOUT_REF96, **kw):
 
 # ---- KATs (SURVEY 8c) ------------------------------------------------------------------------------
 def test_unit_quad_kat(gpu_ctx):
+    """The unit quad at R = 64: 4096 = 2080 + 2016 records, one per pixel centre (the diagonal's belong to triangle 0)."""
+    _unit_quad_kat(gpu_ctx, 64)
+
+
+@pytest.mark.parametrize("R", [1, 2, 3])
+def test_unit_quad_kat_smallest_grids(gpu_ctx, R):
+    """The same KAT at the smallest resolutions: at R = 1 the single centre lies on the diagonal and belongs to
+    triangle 0."""
+    _unit_quad_kat(gpu_ctx, R)
+
+
+def _unit_quad_kat(gpu_ctx, R):
+    """R^2 records, one per pixel centre; the R of them on the diagonal belong to triangle 0 (left edge)."""
     s = synth.unit_quad()
-    out = check(gpu_ctx, s, 64)
-    assert out.total == 4096 and out.written == 4096 and not out.overflow
+    out = check(gpu_ctx, s, R)
+    n = R * R
+    assert out.total == n and out.written == n and not out.overflow
     rec, keys = out.numpy(), out.keys_numpy()
     tri = (keys >> np.uint64(24)).astype(np.int64)
-    assert np.bincount(tri).tolist() == [2080, 2016]  # diagonal centres belong to triangle 0 (left edge)
+    n0, n1 = R * (R + 1) // 2, R * (R - 1) // 2
+    assert np.bincount(tri, minlength=2).tolist() == [n0, n1]  # diagonal centres belong to triangle 0 (left edge)
     px = (keys & np.uint64(0xfff)).astype(np.float32)
     py = ((keys >> np.uint64(12)) & np.uint64(0xfff)).astype(np.float32)
-    np.testing.assert_allclose(rec["position"][:, 0], (px + 0.5) / 64, atol=1e-6)
-    np.testing.assert_allclose(rec["position"][:, 1], (py + 0.5) / 64, atol=1e-6)
+    assert len(np.unique(keys & np.uint64(0xffffff))) == n and px.max() < R and py.max() < R
+    np.testing.assert_allclose(rec["position"][:, 0], (px + 0.5) / R, atol=1e-6)
+    np.testing.assert_allclose(rec["position"][:, 1], (py + 0.5) / R, atol=1e-6)
     assert np.all(rec["position"][:, 2] == 0)
-    np.testing.assert_allclose(rec["scale"], np.tile(np.array([1, 1, 1e-7, 0], np.float32), (4096, 1)), rtol=1e-6)
+    if R == 64:
+        np.testing.assert_allclose(rec["scale"], np.tile(np.array([1, 1, 1e-7, 0], np.float32), (n, 1)), rtol=1e-6)
     q0 = np.array([0, 0.9238795, 0.38268343, 0], np.float32)
     q1 = np.array([0.9238795, 0, 0, 0.38268343], np.float32)
-    np.testing.assert_allclose(rec["rotation"][tri == 0], np.tile(q0, (2080, 1)), atol=1e-6)
-    np.testing.assert_allclose(rec["rotation"][tri == 1], np.tile(q1, (2016, 1)), atol=1e-6)
+    np.testing.assert_allclose(rec["rotation"][tri == 0], np.tile(q0, (n0, 1)), atol=1e-6)
+    np.testing.assert_allclose(rec["rotation"][tri == 1], np.tile(q1, (n1, 1)), atol=1e-6)
     assert np.all(rec["color"] == 1.0)
-    np.testing.assert_allclose(rec["pbr"], np.tile(np.array([0.1, 0.5, 0, 1], np.float32), (4096, 1)))
-    np.testing.assert_allclose(rec["normal"], np.tile(np.array([0, 0, 1, 0], np.float32), (4096, 1)), atol=1e-6)
+    np.testing.assert_allclose(rec["pbr"], np.tile(np.array([0.1, 0.5, 0, 1], np.float32), (n, 1)))
+    np.testing.assert_allclose(rec["normal"], np.tile(np.array([0, 0, 1, 0], np.float32), (n, 1)), atol=1e-6)
 
 
 def test_unit_quad_textured(gpu_ctx):
@@ -250,12 +267,20 @@ def test_convert_host_pipelined_chunks(gpu_ctx, layout):
 
 def test_convert_host_pipelined_chunks_through_the_direct_path(gpu_ctx):
     """A mesh big enough that every chunk of the host pipeline is a launch in which the warps take several units each
-    (4 chunks of 90 000 triangles): the raster kernel shades the small triangles itself (direct path) and appends after
-    the earlier chunks' records.  Same multiset of records and keys as one device-resident conversion, bit for bit."""
+    (4 chunks of 90 000 triangles; asserted from the launch plan of each chunk's range): the raster kernel shades the
+    small triangles itself (direct path) and appends after the earlier chunks' records.  Same multiset of records and
+    keys as one device-resident conversion, bit for bit."""
     tri = synth.displaced_sphere(600, 300, seed=4, amplitude=0.05)   # 360 000 triangles
     s = Scene(tri, [Primitive(0, len(tri), (1.0, 0.8, 0.9, 1.0), 0, -1, -1)], synth.make_material_textures(256, 8)[:1])
     s.compute_bboxes()
     R = 300
+    ds = gpu_ctx.upload(s)
+    per = -(-s.triangle_count // 4)
+    for c in range(4):
+        p = gpu_ctx.convert_plan(ds, R, LAYOUT_PACKED56, capacity=6 * R * R, flags=FLAG_UNCAPPED, first_triangle=c * per,
+                                 triangle_count=min(per, s.triangle_count - c * per))
+        assert p.multi_round and p.direct_ok, c
+    ds.free()
     rec, keys, res = gpu_ctx.convert_host(s, R, LAYOUT_PACKED56, flags=FLAG_UNCAPPED, want_keys=True)
     ds = gpu_ctx.upload(s)
     whole = gpu_ctx.convert(ds, R, LAYOUT_PACKED56, flags=FLAG_UNCAPPED, capacity=6 * R * R, want_keys=True)
@@ -303,12 +328,28 @@ def test_convert_file_glb_to_ply(gpu_ctx, tmp_path, fmt):
     got = ply.read_bytes()
     hdr = oracle.ply_header(fmt, len(want))
     assert got[: len(hdr)] == hdr and len(got) == len(ref)
+    match_ply_rows(got[len(hdr):], ref[len(hdr):], fmt)
+
+
+def match_ply_rows(got_body: bytes, want_body: bytes, fmt: int, subset: bool = False) -> None:
+    """.ply bodies as multisets of rows (both are in atomic arrival order): every row of `got_body` must be a row of
+    `want_body`, equal within the encoding's tolerances; with subset = False the two have the same rows."""
     stride = {0: 248, 1: 76, 2: 48}[fmt]
-    g = np.frombuffer(got[len(hdr):], np.uint8).reshape(-1, stride)
-    w = np.frombuffer(ref[len(hdr):], np.uint8).reshape(-1, stride)
+    g = np.frombuffer(got_body, np.uint8).reshape(-1, stride)
+    w = np.frombuffer(want_body, np.uint8).reshape(-1, stride)
+    assert subset or len(g) == len(w)
     # identify rows by position (first 12 bytes: three floats, distinct per fragment within a primitive plane)
     gp, wp = g[:, :12].copy().view(np.float32), w[:, :12].copy().view(np.float32)
     go, wo = np.lexsort(np.round(gp * 4096).T), np.lexsort(np.round(wp * 4096).T)
+    if subset:   # the rows of `want` with the same rounded position, one per row of `got`
+        gk = np.round(gp.astype(np.float64) * 4096).astype(np.int64)
+        wk = np.round(wp.astype(np.float64) * 4096).astype(np.int64)
+        wmap = {tuple(r): i for i, r in enumerate(wk)}
+        assert len(wmap) == len(wk), "positions do not identify the rows"
+        idx = np.array([wmap.get(tuple(r), -1) for r in gk], np.int64)
+        assert (idx >= 0).all(), f"{np.count_nonzero(idx < 0)} rows are not rows of the expected file"
+        assert len(np.unique(idx)) == len(idx), "a row is written twice"
+        go, wo = np.arange(len(g)), idx
     assert np.allclose(gp[go], wp[wo], atol=2e-5)
     G, W = g[go], w[wo]
     if fmt == 2:  # pos f32x3 | rgba u8x4 | quat f32x4 | log-scale f32x3 | octahedral normal u8x2 | roughness, metallic u8
@@ -325,22 +366,40 @@ def test_convert_file_glb_to_ply(gpu_ctx, tmp_path, fmt):
 
 
 def test_watertight_tiling_full_size(gpu_ctx):
-    """Size-independent coverage property at R = 2048: a Delaunay tiling of the unit square (~60 k triangles of
-    every shape, sub-pixel slivers to 100-pixel triangles) emits each of the 4 194 304 pixel centres exactly
-    once, and a second run produces bit-identical records (as a set)."""
-    from util import planar_triangulation
+    """The watertight tiling at R = 2048 (4 194 304 pixel centres); see _watertight_tiling."""
+    _watertight_tiling(gpu_ctx, 2048)
+
+
+def test_watertight_tiling_max_resolution(gpu_ctx):
+    """The watertight tiling at the largest grid, R = 4096: the width the 12-bit key coordinates, box origins and block
+    rows are packed for."""
+    _watertight_tiling(gpu_ctx, 4096)
+
+
+def _watertight_tiling(gpu_ctx, R):
+    """Size-independent coverage property: a Delaunay tiling of the unit square (~60 k triangles of every shape, sub-pixel slivers to
+    100-pixel triangles) emits each of the R^2 pixel centres exactly once, into guarded buffers, and a second run
+    produces bit-identical records (as a set).  Compared on the device."""
+    import torch
+    from util import GuardedDevice, planar_triangulation
     s = planar_triangulation(30000, seed=7)
-    R = 2048
     ds = gpu_ctx.upload(s)
-    a = gpu_ctx.convert(ds, R, LAYOUT_PACKED56, flags=FLAG_UNCAPPED, capacity=R * R + 64, want_keys=True)
-    assert a.total == R * R
-    ka = a.keys_numpy()
-    assert len(np.unique(ka & np.uint64(0xFFFFFF))) == R * R
-    ra = a.numpy()[np.argsort(ka)].copy()
-    b = gpu_ctx.convert(ds, R, LAYOUT_PACKED56, flags=FLAG_UNCAPPED, capacity=R * R + 64, want_keys=True)
-    kb = b.keys_numpy()
-    assert np.array_equal(np.sort(ka), np.sort(kb))
-    assert ra.tobytes() == b.numpy()[np.argsort(kb)].tobytes()
+    n = R * R
+
+    def run():
+        out, keys = GuardedDevice(n + 64, 56, what="records"), GuardedDevice(n + 64, 8, torch.int64, what="keys")
+        o = gpu_ctx.convert(ds, R, LAYOUT_PACKED56, flags=FLAG_UNCAPPED, capacity=n + 64, out=out.view, keys=keys.view, want_keys=True)
+        assert o.total == n and o.written == n
+        out.check(n)
+        keys.check(n)
+        k, order = torch.sort(keys.view[:n])
+        return k, out.view[: n * 56].view(n, 56)[order]
+    ka, ra = run()
+    assert torch.unique(ka & 0xFFFFFF).numel() == n
+    assert bool(((ka & 0xFFF) < R).all()) and bool((((ka >> 12) & 0xFFF) < R).all())
+    kb, rb = run()
+    assert torch.equal(ka, kb)
+    assert torch.equal(ra, rb)
     ds.free()
 
 
@@ -380,8 +439,13 @@ def test_reference_shaped_interface(tmp_path):
 # ---- full-size properties (BASELINE config 2 stand-in) -------------------------------------------------
 def test_helmet_standin_density_512_full_parity(gpu_ctx):
     """BASELINE config 2 exactly as bench.py runs it: 70 074 triangles, three 2048^2 maps, density 512 — every record of
-    both layouts against the oracle."""
+    both layouts against the oracle.  Premise (asserted from the launch plan): the PACKED56 launch gives the raster warps
+    more than one unit each but fewer than three, so it takes the direct path with the late claim."""
     s = synth.helmet_standin(2048)
+    ds = gpu_ctx.upload(s)
+    plan = gpu_ctx.convert_plan(ds, 512, LAYOUT_PACKED56)
+    ds.free()
+    assert plan.multi_round and plan.direct_ok and plan.claim_late
     out = check(gpu_ctx, s, 512, LAYOUT_REF96)
     assert 0.4e6 < out.total < 1.2e6
     out2 = check(gpu_ctx, s, 512, LAYOUT_PACKED56)
@@ -478,7 +542,8 @@ def test_config4_million_triangle_sphere(gpu_ctx):
 def test_direct_path_and_queue_path_write_the_same_records(gpu_ctx):
     """PACKED56 has two routes for the small triangles of a light work unit: in a launch where the warps take several
     units each (here: 200 000 triangles in one call) the raster kernel shades them itself (direct path); with at most one
-    unit per warp (here: the same triangles in ranges of 25 000) they are queued for the fragment kernel.  Both run the
+    unit per warp (here: the same triangles in ranges of 25 000) they are queued for the fragment kernel.  The launch
+    plan asserts both premises.  Both run the
     same shading code on the same per-triangle records: the two results must be the same multiset of records, bit for
     bit, with the same fragment identities — and the whole thing must agree with the oracle."""
     tri = synth.displaced_sphere(500, 200, seed=11, amplitude=0.04)
@@ -486,11 +551,15 @@ def test_direct_path_and_queue_path_write_the_same_records(gpu_ctx):
     s.compute_bboxes()
     R = 384
     ds = gpu_ctx.upload(s)
+    plan = gpu_ctx.convert_plan(ds, R, LAYOUT_PACKED56, capacity=6 * R * R, flags=FLAG_UNCAPPED)
+    assert plan.multi_round and plan.direct_ok
     whole = gpu_ctx.convert(ds, R, LAYOUT_PACKED56, flags=FLAG_UNCAPPED, capacity=6 * R * R, want_keys=True)
     a, ak = whole.numpy().copy(), whole.keys_numpy().copy()
     parts, pk = [], []
     step = 25_000
     for first in range(0, s.triangle_count, step):
+        assert not gpu_ctx.convert_plan(ds, R, LAYOUT_PACKED56, capacity=6 * R * R, flags=FLAG_UNCAPPED, first_triangle=first,
+                                        triangle_count=min(step, s.triangle_count - first)).multi_round
         o = gpu_ctx.convert(ds, R, LAYOUT_PACKED56, flags=FLAG_UNCAPPED, capacity=6 * R * R, want_keys=True, first_triangle=first,
                             triangle_count=min(step, s.triangle_count - first))
         parts.append(o.numpy().copy()); pk.append(o.keys_numpy().copy())
@@ -633,21 +702,40 @@ def test_prepass_on_the_conversion_output(gpu_ctx, layout):
 
 @pytest.mark.parametrize("layout", [LAYOUT_REF96, LAYOUT_PACKED56])
 def test_prepass_large_input_path(gpu_ctx, layout):
-    """From 2 M records on the kernel fetches a warp's records as one contiguous span through shared memory (another code
-    path than the small-input one): 2 100 001 records (an odd count: the PACKED56 span of the last warp ends on an 8-byte
-    tail) against the oracle."""
+    """From 2 M (2 << 20) records on the kernel fetches a warp's records as one contiguous span through shared memory
+    (another code path than the small-input one): 2 100 001 records (an odd count: the PACKED56 span of the last warp
+    ends on an 8-byte tail) against the oracle, with guarded quad and depth buffers."""
+    _prepass_bounds(gpu_ctx, layout, 2_100_001)
+
+
+@pytest.mark.parametrize("count", [1, 31, 33, (1 << 21) - 1, 1 << 21])
+@pytest.mark.parametrize("layout", [LAYOUT_REF96, LAYOUT_PACKED56])
+def test_prepass_counts_around_the_thresholds(gpu_ctx, layout, count):
+    """Counts around a warp and around the staged-fetch threshold (2 << 20: the last count of the small-input path and
+    the first of the staged one) against the oracle, with guarded quad and depth buffers."""
+    _prepass_bounds(gpu_ctx, layout, count)
+
+
+def _prepass_bounds(gpu_ctx, layout, count):
+    """`count` records against the oracle; guarded quads and depths: nothing is written beyond the survivors and no
+    survivor's slot is left unwritten."""
     import torch
-    from util import assert_prepass_match
+    from util import GuardedDevice, assert_prepass_match
     c = list(_prepass_cases())[0 if layout == LAYOUT_REF96 else 3]   # gaussians whose scales suit the format (u_format 1: no std_dev factor)
     base = c["gaussians"]
-    reps = 2_100_001 // len(base) + 1
-    g = np.tile(base, (reps, 1))[:2_100_001].copy()
+    reps = count // len(base) + 1
+    g = np.tile(base, (reps, 1))[:count].copy()
     g[:, 0] += (np.arange(len(g)) // len(base)).astype(np.float32) * np.float32(2e-4)   # distinct positions per copy
     rec = g if layout == LAYOUT_REF96 else _as_packed56(g)
     g24 = g if layout == LAYOUT_REF96 else oracle.packed56_as_gaussian_vertex(rec)
     d = torch.from_numpy(np.ascontiguousarray(rec).view(np.uint8).reshape(-1)).cuda()
     fmt = 0 if layout == LAYOUT_REF96 else 1
-    quads, depths = gpu_ctx.prepass(d, len(rec), layout, c["view"], c["proj"], c["model"], c["resolution"], c["near_far"], c["std_dev"], 0)
+    gq, gd = GuardedDevice(count, _abi.QUAD_BYTES, what="quads"), GuardedDevice(count, 4, torch.float32, what="depths")
+    quads, depths = gpu_ctx.prepass(d, len(rec), layout, c["view"], c["proj"], c["model"], c["resolution"], c["near_far"], c["std_dev"], 0,
+                                    quads=gq.view, depths=gd.view)
+    gq.check(len(quads))
+    gd.check(len(depths))
     want_q, want_d = oracle.prepass(g24, c["view"], c["proj"], c["model"], c["resolution"], c["near_far"], c["std_dev"], 0, fmt, 0)
-    assert len(want_q) > 1_000_000
+    if count > 1_000_000:
+        assert len(want_q) > 1_000_000
     assert_prepass_match(quads, depths, want_q, want_d, c["resolution"], ordered=False)

@@ -149,6 +149,146 @@ def planar_triangulation(n_points: int, seed: int) -> _abi.Scene:
     return s
 
 
+def layered_tiling(k: int, R: int, kind: str = "delaunay", n: int = 2000, seed: int = 0, wide: int = 0) -> _abi.Scene:
+    """k copies of a watertight tiling of the unit square at z = 0, 0.1, .., 0.1 (k - 1), all in ONE primitive.  Every
+    layer emits each pixel centre of the R x R grid exactly once (top-left rule on shared edges), so the total is known
+    without the oracle: k R^2.
+      kind "delaunay": planar_triangulation with n random interior points (about 2 n triangles per layer);
+      kind "strips":   n vertical strips, two full-height triangles each (every triangle is as tall as the grid); the
+                       first `wide` strips are 32 pixels wide (row blocks of more fragments than a work item holds), the
+                       others share the rest of the width."""
+    if kind == "delaunay":
+        layer = planar_triangulation(n, seed).triangles.reshape(-1, 3, 12)
+    elif kind == "strips":
+        ww = min(wide * 32.0 / R, 0.5)
+        xs = np.concatenate([np.linspace(0.0, ww, wide + 1), np.linspace(ww, 1.0, n - wide + 1)[1:]]).astype(np.float32)
+        x0, x1 = xs[:-1], xs[1:]
+        z, o = np.zeros_like(x0), np.ones_like(x0)
+        a = np.stack([np.stack([x0, z], 1), np.stack([x1, z], 1), np.stack([x1, o], 1)], 1)   # (n, 3, 2)
+        b = np.stack([np.stack([x0, z], 1), np.stack([x1, o], 1), np.stack([x0, o], 1)], 1)
+        xy = np.concatenate([a, b], 0)
+        layer = np.zeros((len(xy), 3, 12), np.float32)
+        layer[:, :, 0:2] = xy
+        layer[:, :, 5] = 1.0
+        layer[:, :, 6] = 1.0; layer[:, :, 9] = 1.0
+        layer[:, :, 10:12] = xy
+    else:
+        raise ValueError(kind)
+    v = np.concatenate([layer] * k, 0)
+    v[:, :, 2] = np.repeat(np.arange(k, dtype=np.float32) * np.float32(0.1), len(layer))[:, None]
+    s = _abi.Scene(v.reshape(-1, 36), [_abi.Primitive(0, len(v), (0.9, 0.8, 0.7, 1.0), -1, -1, -1)], [])
+    s.compute_bboxes()
+    return s
+
+
+# ---- guarded output buffers: every write route must stay inside [0, written) records ------------------------------
+GUARD_BYTE = 0xA5
+GUARD_HEAD = 256          # bytes before the buffer the ABI sees (16-byte aligned)
+GUARD_TAIL_RECORDS = 64   # records after its end
+
+
+def _guard_sizes(count: int, stride: int):
+    return GUARD_HEAD, count * stride, GUARD_TAIL_RECORDS * stride
+
+
+class GuardedDevice:
+    """A device buffer of `count` records of `stride` bytes inside a larger allocation filled with GUARD_BYTE: `view`
+    (uint8, or `dtype`) goes to the ABI, check(written) asserts that nothing outside [0, written) records was written
+    and that no record inside it was left unwritten (still entirely the pattern)."""
+
+    def __init__(self, count: int, stride: int, dtype=None, what: str = "output"):
+        import torch
+        self.count, self.stride, self.what = count, stride, what
+        head, body, tail = _guard_sizes(count, stride)
+        self.raw = torch.full((head + body + tail,), GUARD_BYTE, dtype=torch.uint8, device="cuda")
+        v = self.raw[head: head + body]
+        self.view = v.view(dtype) if dtype is not None else v
+
+    def check(self, written: int) -> None:
+        import torch
+        assert 0 <= written <= self.count, (self.what, written, self.count)
+        head, body, _ = _guard_sizes(self.count, self.stride)
+        end = head + written * self.stride
+        for lo, hi in ((0, head), (end, self.raw.numel())):
+            bad = torch.nonzero(self.raw[lo:hi] != GUARD_BYTE)
+            assert bad.numel() == 0, (f"{self.what}: {bad.numel()} guard bytes overwritten, first at byte "
+                                      f"{int(bad[0]) + lo - head} of the buffer ({written} records written, stride {self.stride})")
+        chunk = max(1, (64 << 20) // self.stride)
+        for r0 in range(0, written, chunk):
+            r1 = min(written, r0 + chunk)
+            rows = self.raw[head + r0 * self.stride: head + r1 * self.stride].view(r1 - r0, self.stride)
+            holes = torch.nonzero((rows == GUARD_BYTE).all(dim=1))
+            assert holes.numel() == 0, f"{self.what}: {holes.numel()} records below `written` never written, first {int(holes[0]) + r0}"
+
+
+class GuardedHost:
+    """GuardedDevice for host (numpy) buffers."""
+
+    def __init__(self, count: int, stride: int, dtype=None, what: str = "output"):
+        self.count, self.stride, self.what = count, stride, what
+        head, body, tail = _guard_sizes(count, stride)
+        self.raw = np.full(head + body + tail, GUARD_BYTE, np.uint8)
+        v = self.raw[head: head + body]
+        self.view = v.view(dtype) if dtype is not None else v
+
+    def check(self, written: int) -> None:
+        assert 0 <= written <= self.count, (self.what, written, self.count)
+        head, body, _ = _guard_sizes(self.count, self.stride)
+        end = head + written * self.stride
+        for lo, hi in ((0, head), (end, len(self.raw))):
+            bad = np.flatnonzero(self.raw[lo:hi] != GUARD_BYTE)
+            assert len(bad) == 0, (f"{self.what}: {len(bad)} guard bytes overwritten, first at byte {int(bad[0]) + lo - head} "
+                                   f"of the buffer ({written} records written, stride {self.stride})")
+        rows = self.raw[head:end].reshape(written, self.stride)
+        holes = np.flatnonzero((rows == GUARD_BYTE).all(axis=1))
+        assert len(holes) == 0, f"{self.what}: {len(holes)} records below `written` never written, first {int(holes[0])}"
+
+
+def write_soup_glb(path: str, triangles: np.ndarray, texture: np.ndarray | None = None,
+                   base_color=(1.0, 1.0, 1.0, 1.0)) -> None:
+    """A .glb of one mesh with one non-indexed primitive: POSITION, NORMAL, TANGENT and TEXCOORD_0 straight from the
+    (T, 36) triangle array (3 x {pos3 nrm3 tan4 uv2}), optionally with a PNG base-colour texture (RGBA8)."""
+    import json
+    import struct
+    v = np.ascontiguousarray(triangles, np.float32).reshape(-1, 12)
+    blobs, views, accessors = [], [], []
+
+    def add_view(b):
+        off = sum(len(x) for x in blobs)
+        blobs.append(b + b"\x00" * ((-len(b)) % 4))
+        views.append({"buffer": 0, "byteOffset": off, "byteLength": len(b)})
+        return len(views) - 1
+
+    def add_acc(arr, typ, minmax=False):
+        a = np.ascontiguousarray(arr, np.float32)
+        acc = {"bufferView": add_view(a.tobytes()), "componentType": 5126, "count": len(a), "type": typ}
+        if minmax:
+            acc["min"] = [float(x) for x in a.min(axis=0)]; acc["max"] = [float(x) for x in a.max(axis=0)]
+        accessors.append(acc)
+        return len(accessors) - 1
+
+    attrs = {"POSITION": add_acc(v[:, 0:3], "VEC3", True), "NORMAL": add_acc(v[:, 3:6], "VEC3"),
+             "TANGENT": add_acc(v[:, 6:10], "VEC4"), "TEXCOORD_0": add_acc(v[:, 10:12], "VEC2")}
+    pbr = {"baseColorFactor": [float(x) for x in base_color]}
+    gltf = {"asset": {"version": "2.0"}, "scene": 0, "scenes": [{"nodes": [0]}], "nodes": [{"mesh": 0}],
+            "meshes": [{"name": "soup", "primitives": [{"attributes": attrs, "material": 0}]}],
+            "materials": [{"pbrMetallicRoughness": pbr}]}
+    if texture is not None:
+        gltf["images"] = [{"bufferView": add_view(png_bytes(texture)), "mimeType": "image/png"}]
+        gltf["textures"] = [{"source": 0}]
+        pbr["baseColorTexture"] = {"index": 0}
+    gltf["bufferViews"] = views
+    gltf["accessors"] = accessors
+    binblob = b"".join(blobs)
+    gltf["buffers"] = [{"byteLength": len(binblob)}]
+    js = json.dumps(gltf).encode()
+    js += b" " * ((-len(js)) % 4)
+    with open(path, "wb") as f:
+        f.write(struct.pack("<4sII", b"glTF", 2, 12 + 8 + len(js) + 8 + len(binblob)))
+        f.write(struct.pack("<I4s", len(js), b"JSON")); f.write(js)
+        f.write(struct.pack("<I4s", len(binblob), b"BIN\x00")); f.write(binblob)
+
+
 def png_encode(samples: np.ndarray, ctype: int, depth: int, interlace: bool = False, plte: bytes | None = None,
                trns: bytes | None = None) -> bytes:
     """General PNG writer for loader tests.  samples: (h, w, channels) integers < 2**depth (channels: 1 gray/palette,
