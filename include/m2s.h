@@ -16,6 +16,10 @@
  *   GaussiansPrepass::execute + gaussianSplattingPrepassCS.glsl  m2s_prepass, m2s_prepass_enqueue
  *     (src/utils/SceneManager.cpp:651-678,
  *      src/parsers/parsers.cpp:232-316,339-428,431-514,631-651)
+ *   RadixSortPass::execute + radixSortPrepass.glsl               m2s_depth_sort, m2s_depth_sort_enqueue
+ *     + glu::RadixSort + radixSortGather.glsl
+ *     (src/renderer/renderPasses/RadixSortPass.cpp:8-90,
+ *      thirdParty/RadixSort.hpp:1393-1562)
  *   SceneManager::loadModel -> execute -> exportPly             m2s_convert_file
  *     (src/utils/SceneManager.hpp:18-20)
  *
@@ -289,6 +293,21 @@ m2s_status m2s_prepass_enqueue(m2s_ctx* ctx, const void* d_records, uint64_t cou
 /* Synchronous variant on the context stream; *valid receives the counter. */
 m2s_status m2s_prepass(m2s_ctx* ctx, const void* d_records, uint64_t count, const m2s_prepass_params* params,
                        void* d_quads, float* d_depths, uint32_t* valid);
+
+/* ---- the step after the prepass: the viewer's depth sort (SURVEY 8 f-5) ----------------------------------------------
+ * RadixSortPass::execute (src/renderer/renderPasses/RadixSortPass.cpp:8-90): radixSortPrepass.glsl + glu::RadixSort
+ * + radixSortGather.glsl.  Stable ascending sort of the quads by the uint32 bits of their view depth (front to back).
+ * n = count, or min(count, *d_count) with d_count (the prepass's d_valid).  d_quads: count x 96 B, d_depths: count
+ * floats (both unchanged); d_sorted_quads: count x 96 B, n written; d_order (optional): n uint32 source indices;
+ * d_draw (optional): 5 uint32 = DrawElementsIndirectCommand {6, n, 0, 0, 0}.  count < 2^30.
+ * Deviation: with n = 0 the draw command is written too (instanceCount 0), where the reference dispatches nothing and
+ * leaves the previous frame's command in place.  Scratch is a stream-ordered allocation of the context, grown on `stream`
+ * (NULL = context stream); nothing is synchronised. */
+m2s_status m2s_depth_sort_enqueue(m2s_ctx* ctx, const void* d_quads, const float* d_depths, uint64_t count,
+                                  const uint32_t* d_count, void* d_sorted_quads, uint32_t* d_order,
+                                  uint32_t* d_draw, void* stream);
+m2s_status m2s_depth_sort(m2s_ctx* ctx, const void* d_quads, const float* d_depths, uint64_t count,
+                          void* d_sorted_quads, uint32_t* d_order, uint32_t* d_draw);   /* context stream, synchronised */
 
 #ifdef __cplusplus
 }

@@ -191,6 +191,35 @@ class Context:
         m = int(valid.value)
         return quads[: m * _abi.QUAD_BYTES].cpu().numpy().view(np.float32).reshape(m, 24).copy(), depths[:m].cpu().numpy().copy()
 
+    def depth_sort(self, quads, depths, count: int, d_count=None, sorted_quads=None, order=None, draw=None):
+        """RadixSortPass::execute on the prepass output (m2s_depth_sort): the quads (a torch uint8 device tensor of
+        count * 96 bytes) stably sorted by the uint32 bits of their view depths (a float32 device tensor of count values).
+        Returns (sorted_quads [n, 24] float32, order [n] uint32, draw [5] uint32) as numpy arrays, n = count or
+        min(count, d_count[0]).  d_count: optional uint32/int32 device tensor (the prepass's valid counter); with it the
+        call is enqueued on torch's current stream (m2s_depth_sort_enqueue).  sorted_quads / order / draw: optional
+        caller-owned device tensors of at least count * 96 bytes / count and 5 32-bit words."""
+        torch = _torch()
+        dev = quads.device
+        if sorted_quads is None:
+            sorted_quads = torch.empty(max(1, count) * _abi.QUAD_BYTES, dtype=torch.uint8, device=dev)
+        if order is None:
+            order = torch.empty(max(1, count), dtype=torch.int32, device=dev)
+        if draw is None:
+            draw = torch.empty(5, dtype=torch.int32, device=dev)
+        if d_count is None:
+            torch.cuda.synchronize(dev)   # the buffers torch filled are ready before the context stream reads them
+            check(lib().m2s_depth_sort(self.handle, quads.data_ptr(), depths.data_ptr(), count, sorted_quads.data_ptr(),
+                                       order.data_ptr(), draw.data_ptr()))
+        else:
+            check(lib().m2s_depth_sort_enqueue(self.handle, quads.data_ptr(), depths.data_ptr(), count, d_count.data_ptr(),
+                                               sorted_quads.data_ptr(), order.data_ptr(), draw.data_ptr(),
+                                               torch.cuda.current_stream(dev).cuda_stream))
+            torch.cuda.synchronize(dev)
+        d = draw[:5].cpu().numpy().view(np.uint32).copy()
+        n = int(d[1])
+        return (sorted_quads[: n * _abi.QUAD_BYTES].cpu().numpy().view(np.float32).reshape(n, 24).copy(),
+                order[:n].cpu().numpy().view(np.uint32).copy(), d)
+
     def convert_timed(self, dscene: DeviceScene, params: _abi.m2s_params, out, capacity: int):
         """One conversion with an event between the two kernels (they do not overlap): (raster_ms, fragment_ms)."""
         a, b = C.c_float(0), C.c_float(0)
@@ -239,6 +268,14 @@ class Context:
         check(lib().m2s_convert_file(self.handle, glb_path.encode(), resolution, gaussian_std, fmt, ply_path.encode(),
                                      C.byref(res)), allow=(_abi.M2S_E_CAPACITY,))
         return res
+
+
+def depth_sort_tile() -> int:
+    """Keys per tile of a depth-sort pass: the value the kernels use (m2s_debug_sort_tile, kept out of m2s.h)."""
+    fn = lib().m2s_debug_sort_tile
+    fn.restype = C.c_uint32
+    fn.argtypes = []
+    return int(fn())
 
 
 def ply_header(fmt: int, count: int) -> bytes:
@@ -323,5 +360,5 @@ class ConversionPass:
         rc.lastResult = out
 
 
-__all__ = ["Context", "DeviceScene", "ConvertOutput", "RenderContext", "SceneManager", "ConversionPass",
+__all__ = ["Context", "DeviceScene", "ConvertOutput", "RenderContext", "SceneManager", "ConversionPass", "depth_sort_tile",
            "ply_header", "ply_write", "M2SError"]

@@ -13,6 +13,7 @@
 #include "../../include/m2s.h"
 #include "m2s_device.cuh"
 #include "m2s_prepass.cuh"
+#include "m2s_sort.cuh"
 
 namespace m2s {
 int convert_warps_per_cta(int layout);
@@ -103,6 +104,8 @@ struct m2s_ctx {
     // intermediates between the raster and the fragment kernel
     void* d_trifrag = nullptr;  size_t trifrag_bytes = 0;   // TriRec per triangle of the shard
     void* d_items = nullptr;    size_t items_bytes = 0;     // FragItem queue
+    // depth sort: control words, alternate key and value buffers (SortLayout, m2s_sort.cuh)
+    void* d_sort = nullptr;     size_t sort_bytes = 0;
 };
 
 struct m2s_dscene {
@@ -241,6 +244,7 @@ M2S_EXPORT void m2s_ctx_destroy(m2s_ctx* c) {
     if (c->d_keys) cudaFreeAsync(c->d_keys, c->stream);
     if (c->d_trifrag) cudaFreeAsync(c->d_trifrag, c->stream);
     if (c->d_items) cudaFreeAsync(c->d_items, c->stream);
+    if (c->d_sort) cudaFreeAsync(c->d_sort, c->stream);
     cudaStreamSynchronize(c->stream);
     if (c->d_prepass_valid) cudaFree(c->d_prepass_valid);
     cudaFree(c->d_sched); cudaFree(c->d_counter); cudaFree(c->d_total); cudaFree(c->d_nitems);
@@ -1173,3 +1177,54 @@ M2S_EXPORT m2s_status m2s_prepass(m2s_ctx* ctx, const void* d_records, uint64_t 
     if (valid) *valid = v;
     return M2S_OK;
 }
+
+// ---- the viewer's depth sort (SURVEY 8 f-5): RadixSortPass::execute = radixSortPrepass.glsl + glu::RadixSort + radixSortGather.glsl
+static m2s_status depth_sort_check(const m2s_ctx* ctx, const void* d_quads, const float* d_depths, uint64_t count, const void* d_sorted) {
+    if (!ctx) { set_error("m2s_depth_sort: ctx is NULL"); return M2S_E_INVALID; }
+    if (count && (!d_quads || !d_depths || !d_sorted)) { set_error("m2s_depth_sort: NULL argument"); return M2S_E_INVALID; }
+    if ((reinterpret_cast<uintptr_t>(d_quads) & 15u) || (reinterpret_cast<uintptr_t>(d_sorted) & 15u)) {
+        set_error("m2s_depth_sort: the quad buffers must be 16-byte aligned"); return M2S_E_INVALID;
+    }
+    if (count >= kSortMaxCount) { set_error("m2s_depth_sort: too many quads (< 2^30 supported)"); return M2S_E_INVALID; }
+    return M2S_OK;
+}
+
+M2S_EXPORT m2s_status m2s_depth_sort_enqueue(m2s_ctx* ctx, const void* d_quads, const float* d_depths, uint64_t count,
+                                             const uint32_t* d_count, void* d_sorted_quads, uint32_t* d_order, uint32_t* d_draw,
+                                             void* stream_) {
+    m2s_status st = depth_sort_check(ctx, d_quads, d_depths, count, d_sorted_quads);
+    if (st != M2S_OK) return st;
+    if (count == 0 && !d_draw) return M2S_OK;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    cudaStream_t stream = stream_ ? (cudaStream_t)stream_ : ctx->stream;
+    const SortLayout l = sort_layout(count);
+    if (count) {
+        st = grow(ctx, &ctx->d_sort, &ctx->sort_bytes, l.total_bytes, stream);
+        if (st != M2S_OK) return st;
+    }
+    SortArgs a;
+    a.count = count;
+    a.d_count = d_count;
+    a.depth_bits = reinterpret_cast<const uint32_t*>(d_depths);
+    a.quads = static_cast<const float4*>(d_quads);
+    a.sorted = static_cast<float4*>(d_sorted_quads);
+    a.scratch = static_cast<uint32_t*>(ctx->d_sort);
+    // without a caller's order buffer the permutation goes to the second value buffer, free by the last pass
+    a.order = d_order ? d_order : (count ? a.scratch + l.ctrl_words + 3 * l.buf_words : nullptr);
+    a.draw = d_draw;
+    CUDA_TRY(sort_launch(a, ctx->sm_count, stream));
+    return M2S_OK;
+}
+
+M2S_EXPORT m2s_status m2s_depth_sort(m2s_ctx* ctx, const void* d_quads, const float* d_depths, uint64_t count, void* d_sorted_quads,
+                                     uint32_t* d_order, uint32_t* d_draw) {
+    m2s_status st = depth_sort_check(ctx, d_quads, d_depths, count, d_sorted_quads);
+    if (st != M2S_OK) return st;
+    st = m2s_depth_sort_enqueue(ctx, d_quads, d_depths, count, nullptr, d_sorted_quads, d_order, d_draw, ctx->stream);
+    if (st != M2S_OK) return st;
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return M2S_OK;
+}
+
+// Test aid (not part of m2s.h): the number of keys one tile of a sort pass holds.
+extern "C" __attribute__((visibility("default"))) uint32_t m2s_debug_sort_tile(void) { return (uint32_t)kSortTile; }

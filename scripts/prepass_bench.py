@@ -15,7 +15,7 @@ ctx = Context(0)
 scene = synth.helmet_standin(2048)
 ds = ctx.upload(scene)
 flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
-peak = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists("MEASURED_PEAKS.json") else 6650.0
+peak = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists("MEASURED_PEAKS.json") else 3350.0   # H100 SXM data sheet
 V = column_major(look_at(np.array([0.0, 0.5, 3.2]), np.zeros(3), np.array([0.0, 1.0, 0.0])).astype(np.float32))
 P = column_major(perspective(np.radians(45.0), 16 / 9, 0.01, 100.0))
 M = column_major(np.eye(4, dtype=np.float32))
