@@ -20,6 +20,9 @@
  *     + glu::RadixSort + radixSortGather.glsl
  *     (src/renderer/renderPasses/RadixSortPass.cpp:8-90,
  *      thirdParty/RadixSort.hpp:1393-1562)
+ *   GaussianSplattingPass::execute + gaussianSplattingVS.glsl     m2s_splat_draw, m2s_splat_draw_enqueue
+ *     + gaussianSplattingPS.glsl
+ *     (src/renderer/renderPasses/GaussianSplattingPass.cpp:37-97)
  *   SceneManager::loadModel -> execute -> exportPly             m2s_convert_file
  *     (src/utils/SceneManager.hpp:18-20)
  *
@@ -308,6 +311,38 @@ m2s_status m2s_depth_sort_enqueue(m2s_ctx* ctx, const void* d_quads, const float
                                   uint32_t* d_draw, void* stream);
 m2s_status m2s_depth_sort(m2s_ctx* ctx, const void* d_quads, const float* d_depths, uint64_t count,
                           void* d_sorted_quads, uint32_t* d_order, uint32_t* d_draw);   /* context stream, synchronised */
+
+/* ---- the step after the depth sort: the viewer's splat draw (SURVEY 8 f-6) ------------------------------------------
+ * GaussianSplattingPass::execute (src/renderer/renderPasses/GaussianSplattingPass.cpp:37-97) + gaussianSplattingVS.glsl
+ * + gaussianSplattingPS.glsl:29-46: every sorted quad, as the two triangles (V0,V1,V2), (V0,V2,V3), drawn into the
+ * G-buffer cleared to 0, blended front to back (dst = src * (1 - dst.a) + dst per target, with the target's own alpha;
+ * dst = src + dst in render mode 4).  The rasterisation, exp, blend and format rules the GL driver would supply are
+ * fixed in DESIGN §2.  Row 0 of every target is the bottom row (window y = 0), as glReadPixels returns it. */
+typedef struct m2s_gbuffer {
+    uint16_t* position;            /* attachment 0, RGBA16F: width x height x 4 fp16 bits, 8-byte aligned, or NULL */
+    uint16_t* normal;              /* attachment 1, RGBA16F */
+    uint8_t* albedo;               /* attachment 2, RGBA8: width x height x 4 bytes, 4-byte aligned, or NULL */
+    uint16_t* depth;               /* attachment 3, RGBA16F */
+    uint8_t* metallic_roughness;   /* attachment 4, RGBA8 */
+} m2s_gbuffer;
+typedef struct m2s_splat_params {
+    uint32_t width, height;        /* renderContext.rendererResolution: 1..4096 each */
+    uint32_t render_mode;          /* 0..6; only mode 4 (overdraw) draws differently */
+} m2s_splat_params;
+/* Enqueue-only.  n = count, or min(count, d_draw[1]) with d_draw the sort's DrawElementsIndirectCommand.  Every pixel of
+ * every non-NULL target is written exactly once (no memset needed); a NULL target is not drawn and changes nothing in
+ * the others.  max_pairs (< 2^30) is the budget of (16 x 16 tile, quad) pairs: when the n quads need more, the longest
+ * prefix of quads whose pairs fit is drawn, and the image is the reference's with that many instances.  d_drawn
+ * (optional, device uint32) receives the prefix length, d_pairs (optional, device uint64) the pairs all n quads need.
+ * count < 2^30; d_sorted_quads 16-byte aligned.  Scratch is stream-ordered context memory grown on `stream` (NULL =
+ * context stream), kept between calls; nothing is synchronised. */
+m2s_status m2s_splat_draw_enqueue(m2s_ctx* ctx, const void* d_sorted_quads, uint64_t count, const uint32_t* d_draw,
+                                  const m2s_splat_params* params, const m2s_gbuffer* gbuffer, uint64_t max_pairs,
+                                  uint64_t* d_pairs, uint32_t* d_drawn, void* stream);
+/* Synchronous form on the context stream: counts the pairs, reads the count back once, grows the scratch and draws all
+ * `count` quads.  *pairs (optional, host) receives the pair count. */
+m2s_status m2s_splat_draw(m2s_ctx* ctx, const void* d_sorted_quads, uint64_t count, const m2s_splat_params* params,
+                          const m2s_gbuffer* gbuffer, uint64_t* pairs);
 
 #ifdef __cplusplus
 }

@@ -71,6 +71,21 @@ class m2s_prepass_params(C.Structure):
 QUAD_BYTES = 96
 
 
+class m2s_gbuffer(C.Structure):
+    """include/m2s.h: the five G-buffer targets of GaussianSplattingPass (device pointers, NULL = not drawn)."""
+    _fields_ = [("position", C.c_void_p), ("normal", C.c_void_p), ("albedo", C.c_void_p), ("depth", C.c_void_p),
+                ("metallic_roughness", C.c_void_p)]
+
+
+class m2s_splat_params(C.Structure):
+    _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("render_mode", C.c_uint32)]
+
+
+# G-buffer attachments in order (renderer.cpp:325-379): name, element dtype (float16 bits or uint8)
+GBUFFER_TARGETS = (("position", np.float16), ("normal", np.float16), ("albedo", np.uint8), ("depth", np.float16),
+                   ("metallic_roughness", np.uint8))
+
+
 def make_prepass_params(world_to_view, view_to_clip, model_to_world, resolution, near_far, std_dev: float, render_mode: int, layout: int):
     p = m2s_prepass_params()
     for name, m in (("world_to_view", world_to_view), ("view_to_clip", view_to_clip), ("model_to_world", model_to_world)):

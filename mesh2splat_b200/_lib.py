@@ -20,6 +20,7 @@ SYMBOLS = [
     "m2s_ply_header", "m2s_ply_encode", "m2s_ply_write", "m2s_convert_file",
     "m2s_glb_load", "m2s_hscene_view", "m2s_hscene_primitive_name", "m2s_hscene_free",
     "m2s_prepass", "m2s_prepass_enqueue", "m2s_depth_sort", "m2s_depth_sort_enqueue",
+    "m2s_splat_draw", "m2s_splat_draw_enqueue",
 ]
 
 
@@ -110,6 +111,10 @@ def lib() -> C.CDLL:
     L.m2s_depth_sort_enqueue.argtypes = [vp, vp, vp, u64, vp, vp, vp, vp, vp]
     L.m2s_depth_sort.restype = i32
     L.m2s_depth_sort.argtypes = [vp, vp, vp, u64, vp, vp, vp]
+    L.m2s_splat_draw_enqueue.restype = i32
+    L.m2s_splat_draw_enqueue.argtypes = [vp, vp, u64, vp, C.POINTER(_abi.m2s_splat_params), C.POINTER(_abi.m2s_gbuffer), u64, vp, vp, vp]
+    L.m2s_splat_draw.restype = i32
+    L.m2s_splat_draw.argtypes = [vp, vp, u64, C.POINTER(_abi.m2s_splat_params), C.POINTER(_abi.m2s_gbuffer), C.POINTER(u64)]
     _lib = L
     return L
 

@@ -220,6 +220,46 @@ class Context:
         return (sorted_quads[: n * _abi.QUAD_BYTES].cpu().numpy().view(np.float32).reshape(n, 24).copy(),
                 order[:n].cpu().numpy().view(np.uint32).copy(), d)
 
+    def splat_draw(self, sorted_quads, count: int, width: int, height: int, render_mode: int = 0, d_draw=None,
+                   targets=tuple(name for name, _ in _abi.GBUFFER_TARGETS), max_pairs: int | None = None, gbuffer=None):
+        """GaussianSplattingPass::execute on the sorted quads (a torch uint8 device tensor of count * 96 bytes): the
+        G-buffer as {target name: numpy array (height, width, 4)}, float16 for position / normal / depth and uint8 for
+        albedo / metallic_roughness, row 0 = the bottom row; plus (drawn, pairs).  targets: the names to draw.
+        max_pairs None: m2s_splat_draw (all quads drawn).  Otherwise m2s_splat_draw_enqueue on torch's current stream with
+        that pair budget, d_draw (optional int32 device tensor, the sort's draw command) limiting n.  gbuffer: optional
+        {name: caller-owned device tensor of width * height * 4 elements} for the drawn targets."""
+        torch = _torch()
+        dev = sorted_quads.device
+        gbuffer = dict(gbuffer or {})
+        g = _abi.m2s_gbuffer()
+        for name, dt in _abi.GBUFFER_TARGETS:
+            if name not in targets:
+                continue
+            if name not in gbuffer:
+                gbuffer[name] = torch.empty(width * height * 4, dtype=torch.int16 if dt == np.float16 else torch.uint8, device=dev)
+            setattr(g, name, gbuffer[name].data_ptr())
+        p = _abi.m2s_splat_params(width, height, render_mode)
+        if max_pairs is None:
+            torch.cuda.synchronize(dev)   # the buffers torch filled are ready before the context stream reads them
+            pairs = C.c_uint64(0)
+            check(lib().m2s_splat_draw(self.handle, sorted_quads.data_ptr(), count, C.byref(p), C.byref(g), C.byref(pairs)))
+            drawn, npairs = count, int(pairs.value)
+        else:
+            out = torch.zeros(4, dtype=torch.int32, device=dev)   # pairs (uint64) | drawn (uint32)
+            check(lib().m2s_splat_draw_enqueue(self.handle, sorted_quads.data_ptr(), count,
+                                               d_draw.data_ptr() if d_draw is not None else None, C.byref(p), C.byref(g),
+                                               max_pairs, out.data_ptr(), out[2:].data_ptr(),
+                                               torch.cuda.current_stream(dev).cuda_stream))
+            torch.cuda.synchronize(dev)
+            o = out.cpu().numpy()
+            npairs, drawn = int(o[:2].view(np.uint64)[0]), int(o[2])
+        images = {}
+        for name, dt in _abi.GBUFFER_TARGETS:
+            if name in targets:
+                raw = gbuffer[name].view(torch.uint8)[: width * height * 4 * np.dtype(dt).itemsize]
+                images[name] = raw.cpu().numpy().view(dt).reshape(height, width, 4).copy()
+        return images, drawn, npairs
+
     def convert_timed(self, dscene: DeviceScene, params: _abi.m2s_params, out, capacity: int):
         """One conversion with an event between the two kernels (they do not overlap): (raster_ms, fragment_ms)."""
         a, b = C.c_float(0), C.c_float(0)

@@ -14,6 +14,7 @@
 #include "m2s_device.cuh"
 #include "m2s_prepass.cuh"
 #include "m2s_sort.cuh"
+#include "m2s_splat.cuh"
 
 namespace m2s {
 int convert_warps_per_cta(int layout);
@@ -106,6 +107,9 @@ struct m2s_ctx {
     void* d_items = nullptr;    size_t items_bytes = 0;     // FragItem queue
     // depth sort: control words, alternate key and value buffers (SortLayout, m2s_sort.cuh)
     void* d_sort = nullptr;     size_t sort_bytes = 0;
+    // splat draw: per-quad counts and tile ranges (SplatLayout, m2s_splat.cuh), and the pair sort (SortLayout)
+    void* d_splat = nullptr;    size_t splat_bytes = 0;
+    void* d_splat_pairs = nullptr; size_t splat_pairs_bytes = 0;
 };
 
 struct m2s_dscene {
@@ -245,6 +249,8 @@ M2S_EXPORT void m2s_ctx_destroy(m2s_ctx* c) {
     if (c->d_trifrag) cudaFreeAsync(c->d_trifrag, c->stream);
     if (c->d_items) cudaFreeAsync(c->d_items, c->stream);
     if (c->d_sort) cudaFreeAsync(c->d_sort, c->stream);
+    if (c->d_splat) cudaFreeAsync(c->d_splat, c->stream);
+    if (c->d_splat_pairs) cudaFreeAsync(c->d_splat_pairs, c->stream);
     cudaStreamSynchronize(c->stream);
     if (c->d_prepass_valid) cudaFree(c->d_prepass_valid);
     cudaFree(c->d_sched); cudaFree(c->d_counter); cudaFree(c->d_total); cudaFree(c->d_nitems);
@@ -1228,3 +1234,87 @@ M2S_EXPORT m2s_status m2s_depth_sort(m2s_ctx* ctx, const void* d_quads, const fl
 
 // Test aid (not part of m2s.h): the number of keys one tile of a sort pass holds.
 extern "C" __attribute__((visibility("default"))) uint32_t m2s_debug_sort_tile(void) { return (uint32_t)kSortTile; }
+
+// ---- the viewer's splat draw (SURVEY 8 f-6): GaussianSplattingPass::execute + gaussianSplattingVS/PS.glsl ----------
+static m2s_status splat_check(const m2s_ctx* ctx, const void* d_quads, uint64_t count, const m2s_splat_params* p, const m2s_gbuffer* g,
+                              uint64_t max_pairs) {
+    if (!ctx || !p || !g) { set_error("m2s_splat_draw: NULL argument"); return M2S_E_INVALID; }
+    if (count && !d_quads) { set_error("m2s_splat_draw: NULL quads"); return M2S_E_INVALID; }
+    if (reinterpret_cast<uintptr_t>(d_quads) & 15u) { set_error("m2s_splat_draw: the quad buffer must be 16-byte aligned"); return M2S_E_INVALID; }
+    if (count >= kSplatMaxCount) { set_error("m2s_splat_draw: too many quads (< 2^30 supported)"); return M2S_E_INVALID; }
+    if (max_pairs >= kSplatMaxPairs) { set_error("m2s_splat_draw: max_pairs too large (< 2^30 supported)"); return M2S_E_INVALID; }
+    if (p->width < 1 || p->width > kSplatMaxSide || p->height < 1 || p->height > kSplatMaxSide) {
+        set_error("m2s_splat_draw: width and height must be 1..4096"); return M2S_E_INVALID;
+    }
+    if (p->render_mode > 6) { set_error("m2s_splat_draw: render modes 0..6 only"); return M2S_E_INVALID; }
+    if (!g->position && !g->normal && !g->albedo && !g->depth && !g->metallic_roughness) {
+        set_error("m2s_splat_draw: no targets"); return M2S_E_INVALID;
+    }
+    if ((reinterpret_cast<uintptr_t>(g->position) | reinterpret_cast<uintptr_t>(g->normal) | reinterpret_cast<uintptr_t>(g->depth)) & 7u ||
+        (reinterpret_cast<uintptr_t>(g->albedo) | reinterpret_cast<uintptr_t>(g->metallic_roughness)) & 3u) {
+        set_error("m2s_splat_draw: RGBA16F targets must be 8-byte aligned, RGBA8 targets 4-byte aligned"); return M2S_E_INVALID;
+    }
+    return M2S_OK;
+}
+
+static SplatArgs splat_args(m2s_ctx* ctx, const void* d_quads, uint64_t count, const uint32_t* d_draw, const m2s_splat_params* p,
+                            const m2s_gbuffer* g) {
+    SplatArgs a;
+    std::memset(&a, 0, sizeof(a));
+    a.quads = static_cast<const float4*>(d_quads);
+    a.count = count;
+    a.d_draw = d_draw;
+    a.width = p->width; a.height = p->height; a.mode = p->render_mode;
+    a.position = g->position; a.normal = g->normal; a.albedo = g->albedo; a.depth = g->depth; a.metallic_roughness = g->metallic_roughness;
+    a.scratch = static_cast<unsigned char*>(ctx->d_splat);
+    return a;
+}
+
+M2S_EXPORT m2s_status m2s_splat_draw_enqueue(m2s_ctx* ctx, const void* d_sorted_quads, uint64_t count, const uint32_t* d_draw,
+                                             const m2s_splat_params* p, const m2s_gbuffer* g, uint64_t max_pairs, uint64_t* d_pairs,
+                                             uint32_t* d_drawn, void* stream_) {
+    m2s_status st = splat_check(ctx, d_sorted_quads, count, p, g, max_pairs);
+    if (st != M2S_OK) return st;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    cudaStream_t stream = stream_ ? (cudaStream_t)stream_ : ctx->stream;
+    st = grow(ctx, &ctx->d_splat, &ctx->splat_bytes, splat_layout(count, p->width, p->height).total_bytes, stream);
+    if (st != M2S_OK) return st;
+    if (max_pairs) {
+        st = grow(ctx, &ctx->d_splat_pairs, &ctx->splat_pairs_bytes, sort_layout(max_pairs).total_bytes, stream);
+        if (st != M2S_OK) return st;
+    }
+    SplatArgs a = splat_args(ctx, d_sorted_quads, count, d_draw, p, g);
+    a.max_pairs = max_pairs;
+    a.pairs = static_cast<uint32_t*>(ctx->d_splat_pairs);
+    CUDA_TRY(splat_count_launch(a, stream));
+    CUDA_TRY(splat_draw_launch(a, ctx->sm_count, stream));
+    if (d_pairs) CUDA_TRY(cudaMemcpyAsync(d_pairs, a.scratch, sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
+    if (d_drawn) CUDA_TRY(cudaMemcpyAsync(d_drawn, a.scratch + 8, sizeof(uint32_t), cudaMemcpyDeviceToDevice, stream));
+    return M2S_OK;
+}
+
+M2S_EXPORT m2s_status m2s_splat_draw(m2s_ctx* ctx, const void* d_sorted_quads, uint64_t count, const m2s_splat_params* p,
+                                     const m2s_gbuffer* g, uint64_t* pairs) {
+    m2s_status st = splat_check(ctx, d_sorted_quads, count, p, g, 0);
+    if (st != M2S_OK) return st;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    cudaStream_t stream = ctx->stream;
+    st = grow(ctx, &ctx->d_splat, &ctx->splat_bytes, splat_layout(count, p->width, p->height).total_bytes, stream);
+    if (st != M2S_OK) return st;
+    SplatArgs a = splat_args(ctx, d_sorted_quads, count, nullptr, p, g);
+    CUDA_TRY(splat_count_launch(a, stream));
+    CUDA_TRY(cudaMemcpyAsync(ctx->h_total, a.scratch, sizeof(uint64_t), cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    const uint64_t total = *ctx->h_total;
+    if (total >= kSplatMaxPairs) { set_error("m2s_splat_draw: the quads need 2^30 or more (tile, quad) pairs"); return M2S_E_INVALID; }
+    if (total) {
+        st = grow(ctx, &ctx->d_splat_pairs, &ctx->splat_pairs_bytes, sort_layout(total).total_bytes, stream);
+        if (st != M2S_OK) return st;
+    }
+    a.max_pairs = total;
+    a.pairs = static_cast<uint32_t*>(ctx->d_splat_pairs);
+    CUDA_TRY(splat_draw_launch(a, ctx->sm_count, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    if (pairs) *pairs = total;
+    return M2S_OK;
+}

@@ -237,4 +237,26 @@ cudaError_t sort_launch(const SortArgs& a, int sm_count, cudaStream_t stream) {
     return cudaGetLastError();
 }
 
+cudaError_t sort_pairs16_launch(uint32_t* scratch, uint64_t capacity, const uint32_t* d_n, int sm_count, cudaStream_t stream) {
+    if (capacity == 0) return cudaSuccess;
+    const SortLayout l = sort_layout(capacity);
+    uint32_t* hist = scratch;
+    uint32_t* counters = scratch + kSortPasses * 256;
+    uint32_t* status = counters + 32;
+    uint32_t* kb[2] = {scratch + l.ctrl_words, sort_pairs16_keys(scratch, capacity)};
+    uint32_t* vb[2] = {scratch + l.ctrl_words + l.buf_words, sort_pairs16_vals(scratch, capacity)};
+    cudaError_t e = cudaMemsetAsync(scratch, 0, l.ctrl_words * sizeof(uint32_t), stream);
+    if (e != cudaSuccess) return e;
+    const unsigned hist_grid = (unsigned)std::min<uint64_t>(l.tiles, 2ull * sm_count);
+    sort_hist_kernel<<<hist_grid, kSortThreads, 0, stream>>>(kb[1], capacity, d_n, hist);
+    sort_scan_kernel<<<1, kSortThreads, 0, stream>>>(hist);
+    const unsigned grid = (unsigned)l.tiles;
+    const size_t sw = l.tiles * 256;
+    sort_pass_kernel<false, false><<<grid, kSortThreads, 0, stream>>>(kb[1], vb[1], kb[0], vb[0], capacity, d_n,
+                                                                       hist + 0 * 256, counters + 0, status + 0 * sw, 0u);
+    sort_pass_kernel<false, false><<<grid, kSortThreads, 0, stream>>>(kb[0], vb[0], kb[1], vb[1], capacity, d_n,
+                                                                       hist + 1 * 256, counters + 1, status + 1 * sw, 8u);
+    return cudaGetLastError();
+}
+
 }  // namespace m2s

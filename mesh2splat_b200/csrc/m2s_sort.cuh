@@ -46,4 +46,17 @@ struct SortArgs {
 
 cudaError_t sort_launch(const SortArgs& args, int sm_count, cudaStream_t stream);
 
+// The splat draw's (tile, quad) pairs: a stable sort of n = *d_n <= capacity (key < 2^16, value) pairs with the same
+// histogram, scan and onesweep pass kernels, two passes (digits 0 and 1).  The pairs go in, and come out, in key and
+// value buffer 1 of SortLayout(capacity) at `scratch`.
+inline uint32_t* sort_pairs16_keys(uint32_t* scratch, uint64_t capacity) {
+    const SortLayout l = sort_layout(capacity);
+    return scratch + l.ctrl_words + 2 * l.buf_words;
+}
+inline uint32_t* sort_pairs16_vals(uint32_t* scratch, uint64_t capacity) {
+    const SortLayout l = sort_layout(capacity);
+    return scratch + l.ctrl_words + 3 * l.buf_words;
+}
+cudaError_t sort_pairs16_launch(uint32_t* scratch, uint64_t capacity, const uint32_t* d_n, int sm_count, cudaStream_t stream);
+
 }  // namespace m2s
