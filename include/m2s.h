@@ -23,6 +23,13 @@
  *   GaussianSplattingPass::execute + gaussianSplattingVS.glsl     m2s_splat_draw, m2s_splat_draw_enqueue
  *     + gaussianSplattingPS.glsl
  *     (src/renderer/renderPasses/GaussianSplattingPass.cpp:37-97)
+ *   GaussianShadowPass::execute                                 m2s_shadow_map, m2s_shadow_map_enqueue
+ *     + gaussianPointShadowMappingCS.glsl
+ *     + gaussianPointLightCubeMapShadowVS/PS.glsl
+ *     (src/renderer/renderPasses/GaussianShadowPass.cpp:83-236)
+ *   GaussianRelightingPass::execute                             m2s_deferred_light, m2s_deferred_light_enqueue
+ *     + gaussianSplattingDeferredVS/PS.glsl
+ *     (src/renderer/renderPasses/GaussianRelightingPass.cpp:42-150)
  *   SceneManager::loadModel -> execute -> exportPly             m2s_convert_file
  *     (src/utils/SceneManager.hpp:18-20)
  *
@@ -343,6 +350,71 @@ m2s_status m2s_splat_draw_enqueue(m2s_ctx* ctx, const void* d_sorted_quads, uint
  * `count` quads.  *pairs (optional, host) receives the pair count. */
 m2s_status m2s_splat_draw(m2s_ctx* ctx, const void* d_sorted_quads, uint64_t count, const m2s_splat_params* params,
                           const m2s_gbuffer* gbuffer, uint64_t* pairs);
+
+/* ---- the shadow pass (SURVEY 8 f-7) ------------------------------------------------------------------------------------
+ * GaussianShadowPass::execute (src/renderer/renderPasses/GaussianShadowPass.cpp:83-236): the light prepass
+ * (gaussianPointShadowMappingCS.glsl:58-207) and six face draws (gaussianPointLightCubeMapShadowVS/PS.glsl) into a
+ * point-light depth cube map.  Per gaussian: world position, cube face of normalize(ws - light) (x wins ties over y and
+ * z, y over z; a NaN direction gives face 5), that face's glm::lookAt view and glm::perspective(90 deg, 1, near, far),
+ * the main prepass's 1.05 w cull, covariance, EWA projection and axes (with the renderer's resolution, sic), then one
+ * quad drawn into its face with gl_FragDepth = length(ws - light) / far, depth test LESS on a D24 face cleared to 1.
+ * The D24 code, rasteriser and sampling rules are DESIGN §2.  Deviation: one light record per source gaussian instead
+ * of the reference's per-face buckets of 7 000 000 (an overflowing bucket writes past its region there). */
+typedef struct m2s_shadow_params {
+    float model_to_world[16];  /* renderContext.modelMat, column-major */
+    float light_position[3];   /* pointLightModel[3].xyz */
+    float near_far[2];
+    float resolution[2];       /* renderContext.rendererResolution (not the face size: sic, the reference's u_resolution) */
+    float std_dev;             /* gaussianStd / resolutionTarget */
+    uint32_t layout;           /* M2S_LAYOUT_REF96 or M2S_LAYOUT_PACKED56 */
+    uint32_t size;             /* face size S: 1..1024 (the reference uses 1024) */
+} m2s_shadow_params;
+#define M2S_LIGHT_RECORD_BYTES 32u
+/* Enqueue-only.  n = count, or min(count, *d_count) with d_count the conversion's device counter (uint64).  d_cube:
+ * 6 x S x S floats, face-major in the order +X -X +Y -Y +Z -Z, row 0 = window y 0 of the face's draw; each texel is
+ * the D24 value as a sampler returns it, (float)code / 16777215.  Every texel is written exactly once, clear
+ * included; n = 0 gives the cleared map.  d_light_quads (optional, 16-byte aligned, count x 32 B; NULL = context
+ * scratch) receives the light records 0..n-1 in source order: mean NDC x, y, the four quadScaleNdc values, the
+ * gl_FragDepth, and the face as a uint32 (0xFFFFFFFF and zeros for a culled gaussian).  max_pairs (< 2^30) is the budget
+ * of (16 x 16 face tile, record) pairs: when the n records need more, the longest prefix of records whose pairs fit is
+ * drawn.  d_drawn (optional, device uint32) receives the prefix length, d_pairs (optional, device uint64) the pairs all
+ * n records need.  count < 2^30; d_records 16-byte aligned.  Scratch is stream-ordered context memory grown on
+ * `stream` (NULL = context stream); nothing is synchronised. */
+m2s_status m2s_shadow_map_enqueue(m2s_ctx* ctx, const void* d_records, uint64_t count, const uint64_t* d_count,
+                                  const m2s_shadow_params* params, float* d_cube, void* d_light_quads, uint64_t max_pairs,
+                                  uint64_t* d_pairs, uint32_t* d_drawn, void* stream);
+/* Synchronous form on the context stream: counts the pairs, reads the count back once, grows the scratch and draws all
+ * `count` records.  *pairs (optional, host) receives the pair count. */
+m2s_status m2s_shadow_map(m2s_ctx* ctx, const void* d_records, uint64_t count, const m2s_shadow_params* params,
+                          float* d_cube, void* d_light_quads, uint64_t* pairs);
+
+/* ---- the deferred lighting (SURVEY 8 f-8) ------------------------------------------------------------------------------
+ * GaussianRelightingPass::execute (src/renderer/renderPasses/GaussianRelightingPass.cpp:42-150) +
+ * gaussianSplattingDeferredPS.glsl:32-165: pixel (x, y) reads G-buffer texel (x, y) and writes RGBA8 (no sRGB).
+ *   render mode 5       (metallic_roughness.rg, 0, 1)
+ *   modes 0-4           (albedo.rgb, 1)
+ *   mode 6 (FINAL)      GGX with one point light (1/d^2), 20-tap PCF of the cube map (bias 0.05), ambient 0.3 albedo,
+ *                       Reinhard, pow 1/2.2 — with the shader's quirks kept (DESIGN §6)
+ * Required: albedo (every mode), metallic_roughness (modes 5, 6), position, normal and d_cube (mode 6); the rest may
+ * be NULL.  d_cube as m2s_shadow_map writes it, with shadow_size = S.  The pow, sampling and format rules are DESIGN §2.
+ * Not built: split screen and the mesh G-buffer (GaussianRelightingPass.cpp:90-135). */
+typedef struct m2s_light_params {
+    uint32_t width, height;    /* renderContext.rendererResolution: 1..4096 each */
+    uint32_t render_mode;      /* 0..6 */
+    float light_position[3];
+    float light_color[3];
+    float light_intensity;
+    float cam_pos[3];
+    float far_plane;
+    uint32_t shadow_size;      /* S of d_cube: 1..1024 (mode 6) */
+} m2s_light_params;
+/* Enqueue-only.  d_image: width x height x 4 bytes, 4-byte aligned, row 0 = the bottom row.  Every pixel is written
+ * once.  Nothing is synchronised. */
+m2s_status m2s_deferred_light_enqueue(m2s_ctx* ctx, const m2s_gbuffer* gbuffer, const float* d_cube,
+                                      const m2s_light_params* params, uint8_t* d_image, void* stream);
+/* Synchronous form on the context stream. */
+m2s_status m2s_deferred_light(m2s_ctx* ctx, const m2s_gbuffer* gbuffer, const float* d_cube,
+                              const m2s_light_params* params, uint8_t* d_image);
 
 #ifdef __cplusplus
 }

@@ -81,6 +81,43 @@ class m2s_splat_params(C.Structure):
     _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("render_mode", C.c_uint32)]
 
 
+class m2s_shadow_params(C.Structure):
+    """include/m2s.h: the uniforms of GaussianShadowPass::execute; model_to_world column-major (glm::mat4)."""
+    _fields_ = [("model_to_world", C.c_float * 16), ("light_position", C.c_float * 3), ("near_far", C.c_float * 2),
+                ("resolution", C.c_float * 2), ("std_dev", C.c_float), ("layout", C.c_uint32), ("size", C.c_uint32)]
+
+
+class m2s_light_params(C.Structure):
+    """include/m2s.h: the uniforms of GaussianRelightingPass::execute."""
+    _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("render_mode", C.c_uint32), ("light_position", C.c_float * 3),
+                ("light_color", C.c_float * 3), ("light_intensity", C.c_float), ("cam_pos", C.c_float * 3), ("far_plane", C.c_float),
+                ("shadow_size", C.c_uint32)]
+
+
+LIGHT_RECORD_BYTES = 32
+
+
+def make_shadow_params(model_to_world, light_position, near_far, resolution, std_dev: float, layout: int, size: int = 1024):
+    p = m2s_shadow_params()
+    p.model_to_world = (C.c_float * 16)(*[float(v) for v in np.asarray(model_to_world, np.float32).ravel()])
+    p.light_position = (C.c_float * 3)(*[float(v) for v in light_position])
+    p.near_far = (C.c_float * 2)(float(near_far[0]), float(near_far[1]))
+    p.resolution = (C.c_float * 2)(float(resolution[0]), float(resolution[1]))
+    p.std_dev, p.layout, p.size = float(std_dev), int(layout), int(size)
+    return p
+
+
+def make_light_params(width: int, height: int, render_mode: int, light_position=(0.0, 0.0, 0.0), light_color=(1.0, 1.0, 1.0),
+                      light_intensity: float = 1.0, cam_pos=(0.0, 0.0, 0.0), far_plane: float = 100.0, shadow_size: int = 1024):
+    p = m2s_light_params()
+    p.width, p.height, p.render_mode = int(width), int(height), int(render_mode)
+    p.light_position = (C.c_float * 3)(*[float(v) for v in light_position])
+    p.light_color = (C.c_float * 3)(*[float(v) for v in light_color])
+    p.cam_pos = (C.c_float * 3)(*[float(v) for v in cam_pos])
+    p.light_intensity, p.far_plane, p.shadow_size = float(light_intensity), float(far_plane), int(shadow_size)
+    return p
+
+
 # G-buffer attachments in order (renderer.cpp:325-379): name, element dtype (float16 bits or uint8)
 GBUFFER_TARGETS = (("position", np.float16), ("normal", np.float16), ("albedo", np.uint8), ("depth", np.float16),
                    ("metallic_roughness", np.uint8))

@@ -20,7 +20,8 @@ SYMBOLS = [
     "m2s_ply_header", "m2s_ply_encode", "m2s_ply_write", "m2s_convert_file",
     "m2s_glb_load", "m2s_hscene_view", "m2s_hscene_primitive_name", "m2s_hscene_free",
     "m2s_prepass", "m2s_prepass_enqueue", "m2s_depth_sort", "m2s_depth_sort_enqueue",
-    "m2s_splat_draw", "m2s_splat_draw_enqueue",
+    "m2s_splat_draw", "m2s_splat_draw_enqueue", "m2s_shadow_map", "m2s_shadow_map_enqueue",
+    "m2s_deferred_light", "m2s_deferred_light_enqueue",
 ]
 
 
@@ -115,6 +116,14 @@ def lib() -> C.CDLL:
     L.m2s_splat_draw_enqueue.argtypes = [vp, vp, u64, vp, C.POINTER(_abi.m2s_splat_params), C.POINTER(_abi.m2s_gbuffer), u64, vp, vp, vp]
     L.m2s_splat_draw.restype = i32
     L.m2s_splat_draw.argtypes = [vp, vp, u64, C.POINTER(_abi.m2s_splat_params), C.POINTER(_abi.m2s_gbuffer), C.POINTER(u64)]
+    L.m2s_shadow_map_enqueue.restype = i32
+    L.m2s_shadow_map_enqueue.argtypes = [vp, vp, u64, vp, C.POINTER(_abi.m2s_shadow_params), vp, vp, u64, vp, vp, vp]
+    L.m2s_shadow_map.restype = i32
+    L.m2s_shadow_map.argtypes = [vp, vp, u64, C.POINTER(_abi.m2s_shadow_params), vp, vp, C.POINTER(u64)]
+    L.m2s_deferred_light_enqueue.restype = i32
+    L.m2s_deferred_light_enqueue.argtypes = [vp, C.POINTER(_abi.m2s_gbuffer), vp, C.POINTER(_abi.m2s_light_params), vp, vp]
+    L.m2s_deferred_light.restype = i32
+    L.m2s_deferred_light.argtypes = [vp, C.POINTER(_abi.m2s_gbuffer), vp, C.POINTER(_abi.m2s_light_params), vp]
     _lib = L
     return L
 

@@ -260,6 +260,64 @@ class Context:
                 images[name] = raw.cpu().numpy().view(dt).reshape(height, width, 4).copy()
         return images, drawn, npairs
 
+    def shadow_map(self, records, count: int, layout: int, model_to_world, light_position, near_far, resolution, std_dev: float,
+                   size: int = 1024, max_pairs: int | None = None, d_count=None, cube=None, light_quads=None):
+        """GaussianShadowPass::execute on device-resident records (a torch uint8 tensor, e.g. ConvertOutput.data): returns
+        (cube [6, S, S] float32, light records [count, 8] float32 (word 7: face bits), drawn, pairs) as numpy values.
+        max_pairs None: m2s_shadow_map (all records drawn).  Otherwise m2s_shadow_map_enqueue on torch's current stream
+        with that pair budget and d_count (optional uint64 device tensor, the conversion's counter) limiting n.  cube /
+        light_quads: optional caller-owned device tensors of at least 6 S^2 floats / count * 32 bytes."""
+        torch = _torch()
+        dev = records.device
+        if cube is None:
+            cube = torch.empty(6 * size * size, dtype=torch.float32, device=dev)
+        if light_quads is None:
+            light_quads = torch.empty(max(1, count) * _abi.LIGHT_RECORD_BYTES, dtype=torch.uint8, device=dev)
+        p = _abi.make_shadow_params(model_to_world, light_position, near_far, resolution, std_dev, layout, size)
+        if max_pairs is None:
+            torch.cuda.synchronize(dev)   # the buffers torch filled are ready before the context stream reads them
+            pairs = C.c_uint64(0)
+            check(lib().m2s_shadow_map(self.handle, records.data_ptr(), count, C.byref(p), cube.data_ptr(), light_quads.data_ptr(),
+                                       C.byref(pairs)))
+            drawn, npairs = count, int(pairs.value)
+        else:
+            out = torch.zeros(4, dtype=torch.int32, device=dev)   # pairs (uint64) | drawn (uint32)
+            check(lib().m2s_shadow_map_enqueue(self.handle, records.data_ptr(), count, d_count.data_ptr() if d_count is not None else None,
+                                               C.byref(p), cube.data_ptr(), light_quads.data_ptr(), max_pairs, out.data_ptr(),
+                                               out[2:].data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+            torch.cuda.synchronize(dev)
+            o = out.cpu().numpy()
+            npairs, drawn = int(o[:2].view(np.uint64)[0]), int(o[2])
+        lq = light_quads.view(torch.uint8)[: count * _abi.LIGHT_RECORD_BYTES].cpu().numpy().view(np.float32).reshape(count, 8).copy()
+        return cube[: 6 * size * size].cpu().numpy().reshape(6, size, size).copy(), lq, drawn, npairs
+
+    def deferred_light(self, gbuffer: dict, cube, width: int, height: int, render_mode: int = 6, light_position=(0.0, 0.0, 0.0),
+                       light_color=(1.0, 1.0, 1.0), light_intensity: float = 1.0, cam_pos=(0.0, 0.0, 0.0), far_plane: float = 100.0,
+                       shadow_size: int = 1024, image=None, enqueue: bool = False):
+        """GaussianRelightingPass::execute: the RGBA8 image (height, width, 4) uint8, row 0 = the bottom row, as numpy.
+        gbuffer: {target name: device tensor} (the splat draw's targets; the mode's required ones must be present);
+        cube: device float32 tensor of 6 S^2 values or None (modes 0-5).  enqueue: m2s_deferred_light_enqueue on torch's
+        current stream instead of the synchronous m2s_deferred_light.  image: optional caller-owned device tensor of
+        width * height * 4 bytes."""
+        torch = _torch()
+        dev = next((t.device for t in gbuffer.values() if t is not None), cube.device if cube is not None else None)
+        g = _abi.m2s_gbuffer()
+        for name, t in gbuffer.items():
+            if t is not None:
+                setattr(g, name, t.data_ptr())
+        if image is None:
+            image = torch.empty(width * height * 4, dtype=torch.uint8, device=dev)
+        p = _abi.make_light_params(width, height, render_mode, light_position, light_color, light_intensity, cam_pos, far_plane, shadow_size)
+        cp = cube.data_ptr() if cube is not None else None
+        if enqueue:
+            check(lib().m2s_deferred_light_enqueue(self.handle, C.byref(g), cp, C.byref(p), image.data_ptr(),
+                                                   torch.cuda.current_stream(dev).cuda_stream))
+        else:
+            torch.cuda.synchronize(dev)
+            check(lib().m2s_deferred_light(self.handle, C.byref(g), cp, C.byref(p), image.data_ptr()))
+        torch.cuda.synchronize(dev)
+        return image.view(torch.uint8)[: width * height * 4].cpu().numpy().reshape(height, width, 4).copy()
+
     def convert_timed(self, dscene: DeviceScene, params: _abi.m2s_params, out, capacity: int):
         """One conversion with an event between the two kernels (they do not overlap): (raster_ms, fragment_ms)."""
         a, b = C.c_float(0), C.c_float(0)

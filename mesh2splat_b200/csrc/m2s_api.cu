@@ -12,6 +12,7 @@
 
 #include "../../include/m2s.h"
 #include "m2s_device.cuh"
+#include "m2s_light.cuh"
 #include "m2s_prepass.cuh"
 #include "m2s_sort.cuh"
 #include "m2s_splat.cuh"
@@ -110,6 +111,11 @@ struct m2s_ctx {
     // splat draw: per-quad counts and tile ranges (SplatLayout, m2s_splat.cuh), and the pair sort (SortLayout)
     void* d_splat = nullptr;    size_t splat_bytes = 0;
     void* d_splat_pairs = nullptr; size_t splat_pairs_bytes = 0;
+    // shadow pass: light records when the caller passes none, per-record counts and tile ranges (shadow_layout,
+    // m2s_light.cuh), and the pair sort (SortLayout)
+    void* d_light_quads = nullptr; size_t light_quads_bytes = 0;
+    void* d_shadow = nullptr;   size_t shadow_bytes = 0;
+    void* d_shadow_pairs = nullptr; size_t shadow_pairs_bytes = 0;
 };
 
 struct m2s_dscene {
@@ -251,6 +257,9 @@ M2S_EXPORT void m2s_ctx_destroy(m2s_ctx* c) {
     if (c->d_sort) cudaFreeAsync(c->d_sort, c->stream);
     if (c->d_splat) cudaFreeAsync(c->d_splat, c->stream);
     if (c->d_splat_pairs) cudaFreeAsync(c->d_splat_pairs, c->stream);
+    if (c->d_light_quads) cudaFreeAsync(c->d_light_quads, c->stream);
+    if (c->d_shadow) cudaFreeAsync(c->d_shadow, c->stream);
+    if (c->d_shadow_pairs) cudaFreeAsync(c->d_shadow_pairs, c->stream);
     cudaStreamSynchronize(c->stream);
     if (c->d_prepass_valid) cudaFree(c->d_prepass_valid);
     cudaFree(c->d_sched); cudaFree(c->d_counter); cudaFree(c->d_total); cudaFree(c->d_nitems);
@@ -1316,5 +1325,199 @@ M2S_EXPORT m2s_status m2s_splat_draw(m2s_ctx* ctx, const void* d_sorted_quads, u
     CUDA_TRY(splat_draw_launch(a, ctx->sm_count, stream));
     CUDA_TRY(cudaStreamSynchronize(stream));
     if (pairs) *pairs = total;
+    return M2S_OK;
+}
+
+// ---- the viewer's shadow pass (SURVEY 8 f-7): GaussianShadowPass::execute + gaussianPointShadowMappingCS.glsl + the
+// cube face draws.  The uniforms are built on the host in fp32 with GLM's own formulas (lookAt, perspective, length,
+// inverse(mat3)), the oracle restates the same steps (oracle/m2s_light_oracle.c orc_light_uniforms).
+static void glm_normalize3(float v[3]) {
+    const float inv = 1.0f / std::sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+    v[0] = v[0] * inv; v[1] = v[1] * inv; v[2] = v[2] * inv;
+}
+static void glm_cross(const float a[3], const float b[3], float r[3]) {
+    r[0] = a[1] * b[2] - b[1] * a[2]; r[1] = a[2] * b[0] - b[2] * a[0]; r[2] = a[0] * b[1] - b[0] * a[1];
+}
+
+static void shadow_uniforms(const m2s_shadow_params* p, ShadowArgs& a) {
+    static const float kDir[6][3] = {{1, 0, 0}, {-1, 0, 0}, {0, 1, 0}, {0, -1, 0}, {0, 0, 1}, {0, 0, -1}};
+    static const float kUp[6][3] = {{0, -1, 0}, {0, -1, 0}, {0, 0, 1}, {0, 0, -1}, {0, -1, 0}, {0, -1, 0}};
+    const float* e = p->light_position;
+    for (int f = 0; f < 6; ++f) {   // GaussianShadowPass.cpp:91-108: glm::lookAt(light, light + dir, up)
+        float fw[3] = {(e[0] + kDir[f][0]) - e[0], (e[1] + kDir[f][1]) - e[1], (e[2] + kDir[f][2]) - e[2]}, s[3], u[3];
+        glm_normalize3(fw);
+        glm_cross(fw, kUp[f], s);
+        glm_normalize3(s);
+        glm_cross(s, fw, u);
+        float* V = a.V[f];
+        std::memset(V, 0, 64);
+        V[0] = s[0]; V[4] = s[1]; V[8] = s[2];
+        V[1] = u[0]; V[5] = u[1]; V[9] = u[2];
+        V[2] = -fw[0]; V[6] = -fw[1]; V[10] = -fw[2];
+        V[12] = -(s[0] * e[0] + s[1] * e[1] + s[2] * e[2]);
+        V[13] = -(u[0] * e[0] + u[1] * e[1] + u[2] * e[2]);
+        V[14] = fw[0] * e[0] + fw[1] * e[1] + fw[2] * e[2];
+        V[15] = 1.0f;
+    }
+    // glm::perspective(glm::radians(90.0f), 1.0f, near, far) (:85), RH_NO
+    const float n = p->near_far[0], fa = p->near_far[1];
+    const float th = std::tan((90.0f * 0.01745329251994329576923690768489f) / 2.0f);
+    std::memset(a.P, 0, 64);
+    a.P[0] = 1.0f / (1.0f * th); a.P[5] = 1.0f / th;
+    a.P[10] = -(fa + n) / (fa - n); a.P[11] = -1.0f; a.P[14] = -(2.0f * fa * n) / (fa - n);
+    std::memcpy(a.M, p->model_to_world, 64);
+    const float* M = p->model_to_world;
+    // inverse(mat3(M)) (gaussianPointShadowMappingCS.glsl:104-110), GLM's compute_inverse<3, 3>; m[c][r] = M[4c + r]
+    auto m = [M](int c, int r) { return M[4 * c + r]; };
+    const float ood = 1.0f / (m(0, 0) * (m(1, 1) * m(2, 2) - m(2, 1) * m(1, 2)) - m(1, 0) * (m(0, 1) * m(2, 2) - m(2, 1) * m(0, 2)) +
+                              m(2, 0) * (m(0, 1) * m(1, 2) - m(1, 1) * m(0, 2)));
+    float* R = a.Rinv;   // column-major 3 x 3
+    R[0] = (m(1, 1) * m(2, 2) - m(2, 1) * m(1, 2)) * ood;
+    R[3] = -(m(1, 0) * m(2, 2) - m(2, 0) * m(1, 2)) * ood;
+    R[6] = (m(1, 0) * m(2, 1) - m(2, 0) * m(1, 1)) * ood;
+    R[1] = -(m(0, 1) * m(2, 2) - m(2, 1) * m(0, 2)) * ood;
+    R[4] = (m(0, 0) * m(2, 2) - m(2, 0) * m(0, 2)) * ood;
+    R[7] = -(m(0, 0) * m(2, 1) - m(2, 0) * m(0, 1)) * ood;
+    R[2] = (m(0, 1) * m(1, 2) - m(1, 1) * m(0, 2)) * ood;
+    R[5] = -(m(0, 0) * m(1, 2) - m(1, 0) * m(0, 2)) * ood;
+    R[8] = (m(0, 0) * m(1, 1) - m(1, 0) * m(0, 1)) * ood;
+    // modelScale = (length(M[0]), length(M[0]), length(M[1])) (:97), GLM vec4 dot (x x + y y) + (z z + w w); squared
+    const float l0 = std::sqrt((M[0] * M[0] + M[1] * M[1]) + (M[2] * M[2] + M[3] * M[3]));
+    const float l1 = std::sqrt((M[4] * M[4] + M[5] * M[5]) + (M[6] * M[6] + M[7] * M[7]));
+    a.mscale2[0] = l0 * l0; a.mscale2[1] = l0 * l0; a.mscale2[2] = l1 * l1;
+    for (int k = 0; k < 3; ++k) a.light[k] = e[k];
+    a.res[0] = p->resolution[0]; a.res[1] = p->resolution[1];
+    a.near_far[0] = n; a.near_far[1] = fa;
+    a.std_dev = p->std_dev;
+    a.layout = p->layout == M2S_LAYOUT_REF96 ? 0u : 1u;
+    a.size = p->size;
+}
+
+static m2s_status shadow_check(const m2s_ctx* ctx, const void* d_records, uint64_t count, const m2s_shadow_params* p, const float* d_cube,
+                               const void* d_light_quads, uint64_t max_pairs) {
+    if (!ctx || !p || !d_cube) { set_error("m2s_shadow_map: NULL argument"); return M2S_E_INVALID; }
+    if (count && !d_records) { set_error("m2s_shadow_map: NULL records"); return M2S_E_INVALID; }
+    if (p->layout != M2S_LAYOUT_REF96 && p->layout != M2S_LAYOUT_PACKED56) { set_error("m2s_shadow_map: layouts REF96 and PACKED56 only"); return M2S_E_INVALID; }
+    if ((reinterpret_cast<uintptr_t>(d_records) | reinterpret_cast<uintptr_t>(d_light_quads)) & 15u || reinterpret_cast<uintptr_t>(d_cube) & 3u) {
+        set_error("m2s_shadow_map: the record and light-record buffers must be 16-byte aligned, the cube 4-byte aligned"); return M2S_E_INVALID;
+    }
+    if (count >= kShadowMaxCount) { set_error("m2s_shadow_map: too many gaussians (< 2^30 supported)"); return M2S_E_INVALID; }
+    if (max_pairs >= kSplatMaxPairs) { set_error("m2s_shadow_map: max_pairs too large (< 2^30 supported)"); return M2S_E_INVALID; }
+    if (p->size < 1 || p->size > kShadowMaxSize) { set_error("m2s_shadow_map: size must be 1..1024"); return M2S_E_INVALID; }
+    return M2S_OK;
+}
+
+// the light prepass and the pair count; a.light_quads / a.scratch set up
+static m2s_status shadow_front(m2s_ctx* ctx, const void* d_records, uint64_t count, const uint64_t* d_count, const m2s_shadow_params* p,
+                               float* d_cube, void* d_light_quads, cudaStream_t stream, ShadowArgs& a) {
+    std::memset(&a, 0, sizeof(a));
+    shadow_uniforms(p, a);
+    if (!d_light_quads && count) {
+        m2s_status st = grow(ctx, &ctx->d_light_quads, &ctx->light_quads_bytes, count * kLightRecordBytes, stream);
+        if (st != M2S_OK) return st;
+        d_light_quads = ctx->d_light_quads;
+    }
+    m2s_status st = grow(ctx, &ctx->d_shadow, &ctx->shadow_bytes, shadow_layout(count, p->size).total_bytes, stream);
+    if (st != M2S_OK) return st;
+    a.records = static_cast<const unsigned char*>(d_records);
+    a.count = count;
+    a.d_count = reinterpret_cast<const unsigned long long*>(d_count);
+    a.light_quads = static_cast<float4*>(d_light_quads);
+    a.cube = d_cube;
+    a.scratch = static_cast<unsigned char*>(ctx->d_shadow);
+    CUDA_TRY(light_prepass_launch(a, stream));
+    CUDA_TRY(shadow_count_launch(a, stream));
+    return M2S_OK;
+}
+
+M2S_EXPORT m2s_status m2s_shadow_map_enqueue(m2s_ctx* ctx, const void* d_records, uint64_t count, const uint64_t* d_count,
+                                             const m2s_shadow_params* p, float* d_cube, void* d_light_quads, uint64_t max_pairs,
+                                             uint64_t* d_pairs, uint32_t* d_drawn, void* stream_) {
+    m2s_status st = shadow_check(ctx, d_records, count, p, d_cube, d_light_quads, max_pairs);
+    if (st != M2S_OK) return st;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    cudaStream_t stream = stream_ ? (cudaStream_t)stream_ : ctx->stream;
+    if (max_pairs) {
+        st = grow(ctx, &ctx->d_shadow_pairs, &ctx->shadow_pairs_bytes, sort_layout(max_pairs).total_bytes, stream);
+        if (st != M2S_OK) return st;
+    }
+    ShadowArgs a;
+    st = shadow_front(ctx, d_records, count, d_count, p, d_cube, d_light_quads, stream, a);
+    if (st != M2S_OK) return st;
+    a.max_pairs = max_pairs;
+    a.pairs = static_cast<uint32_t*>(ctx->d_shadow_pairs);
+    CUDA_TRY(shadow_draw_launch(a, ctx->sm_count, stream));
+    if (d_pairs) CUDA_TRY(cudaMemcpyAsync(d_pairs, a.scratch, sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
+    if (d_drawn) CUDA_TRY(cudaMemcpyAsync(d_drawn, a.scratch + 8, sizeof(uint32_t), cudaMemcpyDeviceToDevice, stream));
+    return M2S_OK;
+}
+
+M2S_EXPORT m2s_status m2s_shadow_map(m2s_ctx* ctx, const void* d_records, uint64_t count, const m2s_shadow_params* p, float* d_cube,
+                                     void* d_light_quads, uint64_t* pairs) {
+    m2s_status st = shadow_check(ctx, d_records, count, p, d_cube, d_light_quads, 0);
+    if (st != M2S_OK) return st;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    cudaStream_t stream = ctx->stream;
+    ShadowArgs a;
+    st = shadow_front(ctx, d_records, count, nullptr, p, d_cube, d_light_quads, stream, a);
+    if (st != M2S_OK) return st;
+    CUDA_TRY(cudaMemcpyAsync(ctx->h_total, a.scratch, sizeof(uint64_t), cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    const uint64_t total = *ctx->h_total;
+    if (total >= kSplatMaxPairs) { set_error("m2s_shadow_map: the records need 2^30 or more (tile, record) pairs"); return M2S_E_INVALID; }
+    if (total) {
+        st = grow(ctx, &ctx->d_shadow_pairs, &ctx->shadow_pairs_bytes, sort_layout(total).total_bytes, stream);
+        if (st != M2S_OK) return st;
+    }
+    a.max_pairs = total;
+    a.pairs = static_cast<uint32_t*>(ctx->d_shadow_pairs);
+    CUDA_TRY(shadow_draw_launch(a, ctx->sm_count, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    if (pairs) *pairs = total;
+    return M2S_OK;
+}
+
+// ---- the viewer's deferred lighting (SURVEY 8 f-8): GaussianRelightingPass::execute + gaussianSplattingDeferredPS.glsl
+static m2s_status light_check(const m2s_ctx* ctx, const m2s_gbuffer* g, const float* d_cube, const m2s_light_params* p, const uint8_t* d_image) {
+    if (!ctx || !g || !p || !d_image) { set_error("m2s_deferred_light: NULL argument"); return M2S_E_INVALID; }
+    if (p->width < 1 || p->width > kSplatMaxSide || p->height < 1 || p->height > kSplatMaxSide) {
+        set_error("m2s_deferred_light: width and height must be 1..4096"); return M2S_E_INVALID;
+    }
+    if (p->render_mode > 6) { set_error("m2s_deferred_light: render modes 0..6 only"); return M2S_E_INVALID; }
+    const bool lit = p->render_mode == 6;
+    if (!g->albedo || ((p->render_mode == 5 || lit) && !g->metallic_roughness) || (lit && (!g->position || !g->normal || !d_cube))) {
+        set_error("m2s_deferred_light: NULL target or cube the render mode needs"); return M2S_E_INVALID;
+    }
+    if (lit && (p->shadow_size < 1 || p->shadow_size > kShadowMaxSize)) { set_error("m2s_deferred_light: shadow_size must be 1..1024"); return M2S_E_INVALID; }
+    if ((reinterpret_cast<uintptr_t>(g->position) | reinterpret_cast<uintptr_t>(g->normal)) & 7u ||
+        (reinterpret_cast<uintptr_t>(g->albedo) | reinterpret_cast<uintptr_t>(g->metallic_roughness) | reinterpret_cast<uintptr_t>(d_image) |
+         reinterpret_cast<uintptr_t>(d_cube)) & 3u) {
+        set_error("m2s_deferred_light: RGBA16F targets must be 8-byte aligned, RGBA8 targets, the image and the cube 4-byte aligned");
+        return M2S_E_INVALID;
+    }
+    return M2S_OK;
+}
+
+M2S_EXPORT m2s_status m2s_deferred_light_enqueue(m2s_ctx* ctx, const m2s_gbuffer* g, const float* d_cube, const m2s_light_params* p,
+                                                 uint8_t* d_image, void* stream_) {
+    m2s_status st = light_check(ctx, g, d_cube, p, d_image);
+    if (st != M2S_OK) return st;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    LightArgs a;
+    std::memset(&a, 0, sizeof(a));
+    a.position = g->position; a.normal = g->normal; a.albedo = g->albedo; a.metallic_roughness = g->metallic_roughness;
+    a.cube = d_cube;
+    a.width = p->width; a.height = p->height; a.mode = p->render_mode; a.shadow_size = p->shadow_size;
+    for (int k = 0; k < 3; ++k) { a.light[k] = p->light_position[k]; a.light_color[k] = p->light_color[k]; a.cam[k] = p->cam_pos[k]; }
+    a.light_intensity = p->light_intensity; a.far_plane = p->far_plane;
+    a.image = d_image;
+    CUDA_TRY(deferred_light_launch(a, stream_ ? (cudaStream_t)stream_ : ctx->stream));
+    return M2S_OK;
+}
+
+M2S_EXPORT m2s_status m2s_deferred_light(m2s_ctx* ctx, const m2s_gbuffer* g, const float* d_cube, const m2s_light_params* p, uint8_t* d_image) {
+    m2s_status st = m2s_deferred_light_enqueue(ctx, g, d_cube, p, d_image, nullptr);
+    if (st != M2S_OK) return st;
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return M2S_OK;
 }
