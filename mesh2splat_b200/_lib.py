@@ -21,7 +21,8 @@ SYMBOLS = [
     "m2s_glb_load", "m2s_hscene_view", "m2s_hscene_primitive_name", "m2s_hscene_free",
     "m2s_prepass", "m2s_prepass_enqueue", "m2s_depth_sort", "m2s_depth_sort_enqueue",
     "m2s_splat_draw", "m2s_splat_draw_enqueue", "m2s_shadow_map", "m2s_shadow_map_enqueue",
-    "m2s_deferred_light", "m2s_deferred_light_enqueue",
+    "m2s_deferred_light", "m2s_deferred_light_enqueue", "m2s_mesh_depth", "m2s_mesh_depth_enqueue",
+    "m2s_prepass_mesh_depth", "m2s_prepass_mesh_depth_enqueue",
 ]
 
 
@@ -124,6 +125,14 @@ def lib() -> C.CDLL:
     L.m2s_deferred_light_enqueue.argtypes = [vp, C.POINTER(_abi.m2s_gbuffer), vp, C.POINTER(_abi.m2s_light_params), vp, vp]
     L.m2s_deferred_light.restype = i32
     L.m2s_deferred_light.argtypes = [vp, C.POINTER(_abi.m2s_gbuffer), vp, C.POINTER(_abi.m2s_light_params), vp]
+    L.m2s_mesh_depth_enqueue.restype = i32
+    L.m2s_mesh_depth_enqueue.argtypes = [vp, vp, C.POINTER(_abi.m2s_mesh_depth_params), vp, u64, vp, vp, vp]
+    L.m2s_mesh_depth.restype = i32
+    L.m2s_mesh_depth.argtypes = [vp, vp, C.POINTER(_abi.m2s_mesh_depth_params), vp, C.POINTER(u64)]
+    L.m2s_prepass_mesh_depth_enqueue.restype = i32
+    L.m2s_prepass_mesh_depth_enqueue.argtypes = [vp, vp, u64, vp, C.POINTER(_abi.m2s_prepass_params), vp, u32, u32, vp, vp, vp, vp]
+    L.m2s_prepass_mesh_depth.restype = i32
+    L.m2s_prepass_mesh_depth.argtypes = [vp, vp, u64, C.POINTER(_abi.m2s_prepass_params), vp, u32, u32, vp, vp, C.POINTER(u32)]
     _lib = L
     return L
 

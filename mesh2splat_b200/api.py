@@ -175,10 +175,12 @@ class Context:
                                         total.data_ptr() if total is not None else None, stream or None))
 
     def prepass(self, records, count: int, layout: int, world_to_view, view_to_clip, model_to_world, resolution, near_far,
-                std_dev: float, render_mode: int = 0, quads=None, depths=None):
+                std_dev: float, render_mode: int = 0, quads=None, depths=None, mesh_depth=None):
         """GaussiansPrepass::execute on device-resident records (a torch uint8 tensor, e.g. ConvertOutput.data): returns
         (quads [m, 24] float32, depths [m] float32) as numpy arrays, in atomic arrival order (m2s_prepass).
-        quads / depths: optional caller-owned device tensors of at least count * 96 bytes / count floats."""
+        quads / depths: optional caller-owned device tensors of at least count * 96 bytes / count floats.
+        mesh_depth: None, or a float32 device tensor (H, W) from mesh_depth(..., depth=...): the prepass with the mesh
+        depth test (m2s_prepass_mesh_depth)."""
         import torch
         dev = records.device
         if quads is None:
@@ -187,7 +189,16 @@ class Context:
             depths = torch.empty(max(1, count), dtype=torch.float32, device=dev)
         p = _abi.make_prepass_params(world_to_view, view_to_clip, model_to_world, resolution, near_far, std_dev, render_mode, layout)
         valid = C.c_uint32(0)
-        check(lib().m2s_prepass(self.handle, records.data_ptr(), count, C.byref(p), quads.data_ptr(), depths.data_ptr(), C.byref(valid)))
+        if mesh_depth is None:
+            check(lib().m2s_prepass(self.handle, records.data_ptr(), count, C.byref(p), quads.data_ptr(), depths.data_ptr(), C.byref(valid)))
+        else:
+            if (mesh_depth.dim() != 2 or mesh_depth.dtype != torch.float32 or mesh_depth.device != dev
+                    or not mesh_depth.is_contiguous()):
+                raise ValueError("mesh_depth must be a contiguous (height, width) float32 tensor on the records' device")
+            h, w = mesh_depth.shape
+            torch.cuda.synchronize(dev)   # the map torch holds is ready before the context stream reads it
+            check(lib().m2s_prepass_mesh_depth(self.handle, records.data_ptr(), count, C.byref(p), mesh_depth.data_ptr(), w, h,
+                                               quads.data_ptr(), depths.data_ptr(), C.byref(valid)))
         m = int(valid.value)
         return quads[: m * _abi.QUAD_BYTES].cpu().numpy().view(np.float32).reshape(m, 24).copy(), depths[:m].cpu().numpy().copy()
 
@@ -259,6 +270,33 @@ class Context:
                 raw = gbuffer[name].view(torch.uint8)[: width * height * 4 * np.dtype(dt).itemsize]
                 images[name] = raw.cpu().numpy().view(dt).reshape(height, width, 4).copy()
         return images, drawn, npairs
+
+    def mesh_depth(self, dscene: DeviceScene, world_to_view, view_to_clip, model_to_world, width: int, height: int,
+                   max_pairs: int | None = None, depth=None):
+        """DepthPrepass::execute on an uploaded scene: returns (map (height, width) float32 numpy, row 0 = window y 0,
+        drawn, pairs).  max_pairs None: m2s_mesh_depth (every triangle drawn).  Otherwise m2s_mesh_depth_enqueue on torch's
+        current stream with that pair budget.  depth: optional caller-owned float32 device tensor of at least
+        width * height values (pass it on to prepass(mesh_depth=...) viewed as (height, width))."""
+        torch = _torch()
+        dev = torch.device("cuda", self.device)
+        if depth is None:
+            depth = torch.empty(width * height, dtype=torch.float32, device=dev)
+        elif depth.dtype != torch.float32 or depth.device != dev or not depth.is_contiguous() or depth.numel() < width * height:
+            raise ValueError("depth must be a contiguous float32 tensor of at least width * height values on the context's device")
+        p = _abi.make_mesh_depth_params(world_to_view, view_to_clip, model_to_world, width, height)
+        if max_pairs is None:
+            torch.cuda.synchronize(dev)
+            pairs = C.c_uint64(0)
+            check(lib().m2s_mesh_depth(self.handle, dscene.handle, C.byref(p), depth.data_ptr(), C.byref(pairs)))
+            drawn, npairs = dscene.triangle_count, int(pairs.value)
+        else:
+            out = torch.zeros(4, dtype=torch.int32, device=dev)   # pairs (uint64) | drawn (uint32)
+            check(lib().m2s_mesh_depth_enqueue(self.handle, dscene.handle, C.byref(p), depth.data_ptr(), max_pairs, out.data_ptr(),
+                                               out[2:].data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+            torch.cuda.synchronize(dev)
+            o = out.cpu().numpy()
+            npairs, drawn = int(o[:2].view(np.uint64)[0]), int(o[2])
+        return depth.reshape(-1)[: width * height].cpu().numpy().reshape(height, width).copy(), drawn, npairs
 
     def shadow_map(self, records, count: int, layout: int, model_to_world, light_position, near_far, resolution, std_dev: float,
                    size: int = 1024, max_pairs: int | None = None, d_count=None, cube=None, light_quads=None):

@@ -11,6 +11,7 @@
 #include <vector>
 
 #include "../../include/m2s.h"
+#include "m2s_depth.cuh"
 #include "m2s_device.cuh"
 #include "m2s_light.cuh"
 #include "m2s_prepass.cuh"
@@ -116,6 +117,9 @@ struct m2s_ctx {
     void* d_light_quads = nullptr; size_t light_quads_bytes = 0;
     void* d_shadow = nullptr;   size_t shadow_bytes = 0;
     void* d_shadow_pairs = nullptr; size_t shadow_pairs_bytes = 0;
+    // mesh depth pre-pass: per-triangle counts and tile ranges (SplatLayout), and the pair sort (SortLayout)
+    void* d_mdepth = nullptr;   size_t mdepth_bytes = 0;
+    void* d_mdepth_pairs = nullptr; size_t mdepth_pairs_bytes = 0;
 };
 
 struct m2s_dscene {
@@ -260,6 +264,8 @@ M2S_EXPORT void m2s_ctx_destroy(m2s_ctx* c) {
     if (c->d_light_quads) cudaFreeAsync(c->d_light_quads, c->stream);
     if (c->d_shadow) cudaFreeAsync(c->d_shadow, c->stream);
     if (c->d_shadow_pairs) cudaFreeAsync(c->d_shadow_pairs, c->stream);
+    if (c->d_mdepth) cudaFreeAsync(c->d_mdepth, c->stream);
+    if (c->d_mdepth_pairs) cudaFreeAsync(c->d_mdepth_pairs, c->stream);
     cudaStreamSynchronize(c->stream);
     if (c->d_prepass_valid) cudaFree(c->d_prepass_valid);
     cudaFree(c->d_sched); cudaFree(c->d_counter); cudaFree(c->d_total); cudaFree(c->d_nitems);
@@ -1141,18 +1147,22 @@ static bool invert4(const double m[16], double inv[16]) {   // column-major, cof
     return true;
 }
 
-M2S_EXPORT m2s_status m2s_prepass_enqueue(m2s_ctx* ctx, const void* d_records, uint64_t count, const uint64_t* d_count,
-                                          const m2s_prepass_params* p, void* d_quads, float* d_depths, uint32_t* d_valid, void* stream_) {
-    if (!ctx || !p || !d_valid || (count && (!d_records || !d_quads || !d_depths))) { set_error("m2s_prepass: NULL argument"); return M2S_E_INVALID; }
+// d_valid: the enqueue forms' counter (the synchronous forms use the context's, never NULL)
+static m2s_status prepass_check(const m2s_ctx* ctx, const void* d_records, uint64_t count, const m2s_prepass_params* p, const void* d_quads,
+                                const float* d_depths, bool has_valid) {
+    if (!ctx || !p || !has_valid || (count && (!d_records || !d_quads || !d_depths))) { set_error("m2s_prepass: NULL argument"); return M2S_E_INVALID; }
     if (p->layout != M2S_LAYOUT_REF96 && p->layout != M2S_LAYOUT_PACKED56) { set_error("m2s_prepass: layouts REF96 and PACKED56 only"); return M2S_E_INVALID; }
     if (p->render_mode == 3 || (p->render_mode > 2 && p->render_mode != 6)) { set_error("m2s_prepass: render modes 0 (6), 1 and 2 only"); return M2S_E_INVALID; }
     if (count >= (1ull << 32)) { set_error("m2s_prepass: too many gaussians (< 2^32 supported)"); return M2S_E_INVALID; }
     if ((reinterpret_cast<uintptr_t>(d_quads) & 15u) || (reinterpret_cast<uintptr_t>(d_records) & 15u)) {
         set_error("m2s_prepass: the record and quad buffers must be 16-byte aligned"); return M2S_E_INVALID;
     }
-    CUDA_TRY(cudaSetDevice(ctx->device));
-    cudaStream_t stream = stream_ ? (cudaStream_t)stream_ : ctx->stream;
-    PrepassArgs a;
+    return M2S_OK;
+}
+
+// the kernel's arguments: the uniforms of GaussiansPrepass::execute; M2S_E_INVALID for a singular model matrix
+static m2s_status prepass_fill(const void* d_records, uint64_t count, const uint64_t* d_count, const m2s_prepass_params* p, void* d_quads,
+                               float* d_depths, uint32_t* d_valid, PrepassArgs& a) {
     std::memset(&a, 0, sizeof(a));
     std::memcpy(a.V, p->world_to_view, 64); std::memcpy(a.P, p->view_to_clip, 64); std::memcpy(a.M, p->model_to_world, 64);
     double M[16], Mi[16];
@@ -1174,8 +1184,50 @@ M2S_EXPORT m2s_status m2s_prepass_enqueue(m2s_ctx* ctx, const void* d_records, u
     a.std_dev = p->std_dev; a.render_mode = p->render_mode; a.layout = p->layout == M2S_LAYOUT_REF96 ? 0u : 1u;
     a.count = count; a.d_count = (const unsigned long long*)d_count;
     a.records = (const unsigned char*)d_records; a.quads = (float4*)d_quads; a.depths = d_depths; a.valid = d_valid;
+    return M2S_OK;
+}
+
+M2S_EXPORT m2s_status m2s_prepass_enqueue(m2s_ctx* ctx, const void* d_records, uint64_t count, const uint64_t* d_count,
+                                          const m2s_prepass_params* p, void* d_quads, float* d_depths, uint32_t* d_valid, void* stream_) {
+    m2s_status st = prepass_check(ctx, d_records, count, p, d_quads, d_depths, d_valid != nullptr);
+    if (st != M2S_OK) return st;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    cudaStream_t stream = stream_ ? (cudaStream_t)stream_ : ctx->stream;
+    PrepassArgs a;
+    st = prepass_fill(d_records, count, d_count, p, d_quads, d_depths, d_valid, a);
+    if (st != M2S_OK) return st;
     CUDA_TRY(cudaMemsetAsync(d_valid, 0, sizeof(uint32_t), stream));
     CUDA_TRY(prepass_launch(a, stream));
+    return M2S_OK;
+}
+
+static m2s_status prepass_depth_check(const m2s_ctx* ctx, const void* d_records, uint64_t count, const m2s_prepass_params* p,
+                                      const float* d_mesh_depth, uint32_t depth_width, uint32_t depth_height, const void* d_quads,
+                                      const float* d_depths, bool has_valid) {
+    m2s_status st = prepass_check(ctx, d_records, count, p, d_quads, d_depths, has_valid);
+    if (st != M2S_OK) return st;
+    if (!d_mesh_depth || (reinterpret_cast<uintptr_t>(d_mesh_depth) & 3u)) {
+        set_error("m2s_prepass_mesh_depth: the depth map must be a non-NULL, 4-byte aligned device buffer"); return M2S_E_INVALID;
+    }
+    if (depth_width < 1 || depth_width > kSplatMaxSide || depth_height < 1 || depth_height > kSplatMaxSide) {
+        set_error("m2s_prepass_mesh_depth: depth_width and depth_height must be 1..4096"); return M2S_E_INVALID;
+    }
+    return M2S_OK;
+}
+
+M2S_EXPORT m2s_status m2s_prepass_mesh_depth_enqueue(m2s_ctx* ctx, const void* d_records, uint64_t count, const uint64_t* d_count,
+                                                     const m2s_prepass_params* p, const float* d_mesh_depth, uint32_t depth_width,
+                                                     uint32_t depth_height, void* d_quads, float* d_depths, uint32_t* d_valid, void* stream_) {
+    m2s_status st = prepass_depth_check(ctx, d_records, count, p, d_mesh_depth, depth_width, depth_height, d_quads, d_depths, d_valid != nullptr);
+    if (st != M2S_OK) return st;
+    PrepassDepthArgs a;
+    st = prepass_fill(d_records, count, d_count, p, d_quads, d_depths, d_valid, a.p);
+    if (st != M2S_OK) return st;
+    a.map = d_mesh_depth; a.width = depth_width; a.height = depth_height;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    cudaStream_t stream = stream_ ? (cudaStream_t)stream_ : ctx->stream;
+    CUDA_TRY(cudaMemsetAsync(d_valid, 0, sizeof(uint32_t), stream));
+    CUDA_TRY(prepass_depth_launch(a, stream));
     return M2S_OK;
 }
 
@@ -1185,6 +1237,23 @@ M2S_EXPORT m2s_status m2s_prepass(m2s_ctx* ctx, const void* d_records, uint64_t 
     CUDA_TRY(cudaSetDevice(ctx->device));
     if (!ctx->d_prepass_valid) CUDA_TRY(cudaMalloc(&ctx->d_prepass_valid, sizeof(uint32_t)));
     m2s_status st = m2s_prepass_enqueue(ctx, d_records, count, nullptr, p, d_quads, d_depths, ctx->d_prepass_valid, ctx->stream);
+    if (st != M2S_OK) return st;
+    uint32_t v = 0;
+    CUDA_TRY(cudaMemcpyAsync(&v, ctx->d_prepass_valid, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    if (valid) *valid = v;
+    return M2S_OK;
+}
+
+M2S_EXPORT m2s_status m2s_prepass_mesh_depth(m2s_ctx* ctx, const void* d_records, uint64_t count, const m2s_prepass_params* p,
+                                             const float* d_mesh_depth, uint32_t depth_width, uint32_t depth_height, void* d_quads,
+                                             float* d_depths, uint32_t* valid) {
+    m2s_status st = prepass_depth_check(ctx, d_records, count, p, d_mesh_depth, depth_width, depth_height, d_quads, d_depths, true);
+    if (st != M2S_OK) return st;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    if (!ctx->d_prepass_valid) CUDA_TRY(cudaMalloc(&ctx->d_prepass_valid, sizeof(uint32_t)));
+    st = m2s_prepass_mesh_depth_enqueue(ctx, d_records, count, nullptr, p, d_mesh_depth, depth_width, depth_height, d_quads, d_depths,
+                                        ctx->d_prepass_valid, ctx->stream);
     if (st != M2S_OK) return st;
     uint32_t v = 0;
     CUDA_TRY(cudaMemcpyAsync(&v, ctx->d_prepass_valid, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1519,5 +1588,93 @@ M2S_EXPORT m2s_status m2s_deferred_light(m2s_ctx* ctx, const m2s_gbuffer* g, con
     m2s_status st = m2s_deferred_light_enqueue(ctx, g, d_cube, p, d_image, nullptr);
     if (st != M2S_OK) return st;
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return M2S_OK;
+}
+
+// ---- the viewer's mesh depth pre-pass (SURVEY 8 f-9): DepthPrepass::execute + depthPrepassVS/PS.glsl ----------------
+// u_viewToClip * u_worldToView * u_modelToWorld as GLM evaluates it: (P V) M, each product GLM's mat4 * mat4 in fp32,
+// r[c][row] = ((a[0][row] b[c][0] + a[1][row] b[c][1]) + a[2][row] b[c][2]) + a[3][row] b[c][3]
+static void glm_mat4_mul(const float* a, const float* b, float* r) {
+    for (int c = 0; c < 4; ++c)
+        for (int row = 0; row < 4; ++row)
+            r[c * 4 + row] = ((a[row] * b[c * 4] + a[4 + row] * b[c * 4 + 1]) + a[8 + row] * b[c * 4 + 2]) + a[12 + row] * b[c * 4 + 3];
+}
+
+static m2s_status mesh_depth_check(const m2s_ctx* ctx, const m2s_dscene* scene, const m2s_mesh_depth_params* p, const float* d_depth,
+                                   uint64_t max_pairs) {
+    if (!ctx || !scene || !p || !d_depth) { set_error("m2s_mesh_depth: NULL argument"); return M2S_E_INVALID; }
+    if (reinterpret_cast<uintptr_t>(d_depth) & 3u) { set_error("m2s_mesh_depth: the depth map must be 4-byte aligned"); return M2S_E_INVALID; }
+    if (p->width < 1 || p->width > kSplatMaxSide || p->height < 1 || p->height > kSplatMaxSide) {
+        set_error("m2s_mesh_depth: width and height must be 1..4096"); return M2S_E_INVALID;
+    }
+    if (scene->ntri >= kDepthMaxTris) { set_error("m2s_mesh_depth: too many triangles (< 2^29 supported)"); return M2S_E_INVALID; }
+    if (max_pairs >= kSplatMaxPairs) { set_error("m2s_mesh_depth: max_pairs too large (< 2^30 supported)"); return M2S_E_INVALID; }
+    return M2S_OK;
+}
+
+// the pair count; a.scratch set up
+static m2s_status mesh_depth_front(m2s_ctx* ctx, const m2s_dscene* scene, const m2s_mesh_depth_params* p, float* d_depth,
+                                   cudaStream_t stream, DepthArgs& a) {
+    std::memset(&a, 0, sizeof(a));
+    float pv[16];
+    glm_mat4_mul(p->view_to_clip, p->world_to_view, pv);
+    glm_mat4_mul(pv, p->model_to_world, a.pvm);
+    a.tris = scene->d_tris;
+    a.ntri = scene->ntri;
+    a.ranges = scene->d_ranges;
+    a.nranges = scene->nranges;
+    a.prims = scene->d_prims;
+    a.width = p->width;
+    a.height = p->height;
+    a.depth = d_depth;
+    m2s_status st = grow(ctx, &ctx->d_mdepth, &ctx->mdepth_bytes, splat_layout(a.ntri, a.width, a.height).total_bytes, stream);
+    if (st != M2S_OK) return st;
+    a.scratch = static_cast<unsigned char*>(ctx->d_mdepth);
+    CUDA_TRY(depth_count_launch(a, stream));
+    return M2S_OK;
+}
+
+M2S_EXPORT m2s_status m2s_mesh_depth_enqueue(m2s_ctx* ctx, const m2s_dscene* scene, const m2s_mesh_depth_params* p, float* d_depth,
+                                             uint64_t max_pairs, uint64_t* d_pairs, uint32_t* d_drawn, void* stream_) {
+    m2s_status st = mesh_depth_check(ctx, scene, p, d_depth, max_pairs);
+    if (st != M2S_OK) return st;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    cudaStream_t stream = stream_ ? (cudaStream_t)stream_ : ctx->stream;
+    if (max_pairs) {
+        st = grow(ctx, &ctx->d_mdepth_pairs, &ctx->mdepth_pairs_bytes, sort_layout(max_pairs).total_bytes, stream);
+        if (st != M2S_OK) return st;
+    }
+    DepthArgs a;
+    st = mesh_depth_front(ctx, scene, p, d_depth, stream, a);
+    if (st != M2S_OK) return st;
+    a.max_pairs = max_pairs;
+    a.pairs = static_cast<uint32_t*>(ctx->d_mdepth_pairs);
+    CUDA_TRY(depth_draw_launch(a, ctx->sm_count, stream));
+    if (d_pairs) CUDA_TRY(cudaMemcpyAsync(d_pairs, a.scratch, sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
+    if (d_drawn) CUDA_TRY(cudaMemcpyAsync(d_drawn, a.scratch + 8, sizeof(uint32_t), cudaMemcpyDeviceToDevice, stream));
+    return M2S_OK;
+}
+
+M2S_EXPORT m2s_status m2s_mesh_depth(m2s_ctx* ctx, const m2s_dscene* scene, const m2s_mesh_depth_params* p, float* d_depth, uint64_t* pairs) {
+    m2s_status st = mesh_depth_check(ctx, scene, p, d_depth, 0);
+    if (st != M2S_OK) return st;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    cudaStream_t stream = ctx->stream;
+    DepthArgs a;
+    st = mesh_depth_front(ctx, scene, p, d_depth, stream, a);
+    if (st != M2S_OK) return st;
+    CUDA_TRY(cudaMemcpyAsync(ctx->h_total, a.scratch, sizeof(uint64_t), cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    const uint64_t total = *ctx->h_total;
+    if (total >= kSplatMaxPairs) { set_error("m2s_mesh_depth: the triangles need 2^30 or more (tile, triangle) pairs"); return M2S_E_INVALID; }
+    if (total) {
+        st = grow(ctx, &ctx->d_mdepth_pairs, &ctx->mdepth_pairs_bytes, sort_layout(total).total_bytes, stream);
+        if (st != M2S_OK) return st;
+    }
+    a.max_pairs = total;
+    a.pairs = static_cast<uint32_t*>(ctx->d_mdepth_pairs);
+    CUDA_TRY(depth_draw_launch(a, ctx->sm_count, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    if (pairs) *pairs = total;
     return M2S_OK;
 }

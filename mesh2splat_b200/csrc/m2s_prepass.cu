@@ -24,8 +24,32 @@ constexpr int kPrepassThreads = 256;
 
 // kStage: fetch the warp's records as one contiguous span through shared memory (large inputs: fewer, wider memory
 // transactions) or with six strided 16-byte loads per lane straight into registers (small inputs: one dependent stage less)
-template <bool kStage>
-__global__ void __launch_bounds__(kPrepassThreads) prepass_kernel(const __grid_constant__ PrepassArgs a) {
+// GLM mat4 * vec4: (m0 x + m1 y) + (m2 z + m3 w), round-to-nearest fp32, no contraction
+__device__ __forceinline__ float m4row_rn(const float* m, int row, float x, float y, float z, float w) {
+    return __fadd_rn(__fadd_rn(__fmul_rn(m[row], x), __fmul_rn(m[4 + row], y)), __fadd_rn(__fmul_rn(m[8 + row], z), __fmul_rn(m[12 + row], w)));
+}
+
+// the mesh depth test (gaussianSplattingPrepassCS.glsl:78-91, u_depthTestMesh 1, DESIGN §2): pos2d again in GLSL / GLM
+// order without contraction, uv and myDepth as the shader writes them, the map read NEAREST + CLAMP_TO_EDGE (a NaN
+// coordinate reads texel 0); true if the gaussian is behind the mesh
+__device__ __forceinline__ bool prepass_behind_mesh(const PrepassArgs& a, const float* map, uint32_t dw, uint32_t dh,
+                                                    float px, float py, float pz) {
+    const float w0 = m4row_rn(a.M, 0, px, py, pz, 1.0f), w1 = m4row_rn(a.M, 1, px, py, pz, 1.0f), w2 = m4row_rn(a.M, 2, px, py, pz, 1.0f);
+    const float v0 = m4row_rn(a.V, 0, w0, w1, w2, 1.0f), v1 = m4row_rn(a.V, 1, w0, w1, w2, 1.0f), v2 = m4row_rn(a.V, 2, w0, w1, w2, 1.0f),
+                v3 = m4row_rn(a.V, 3, w0, w1, w2, 1.0f);
+    const float c0 = m4row_rn(a.P, 0, v0, v1, v2, v3), c1 = m4row_rn(a.P, 1, v0, v1, v2, v3), c2 = m4row_rn(a.P, 2, v0, v1, v2, v3),
+                c3 = m4row_rn(a.P, 3, v0, v1, v2, v3);
+    const float u = __fadd_rn(__fmul_rn(__fdiv_rn(c0, c3), 0.5f), 0.5f), v = __fadd_rn(__fmul_rn(__fdiv_rn(c1, c3), 0.5f), 0.5f);
+    const uint32_t i = (uint32_t)fminf(fmaxf(floorf(__fmul_rn(u, (float)dw)), 0.0f), (float)(dw - 1));
+    const uint32_t j = (uint32_t)fminf(fmaxf(floorf(__fmul_rn(v, (float)dh)), 0.0f), (float)(dh - 1));
+    const float depth = __ldg(map + (size_t)j * dw + i);
+    const float my = __fadd_rn(__fmul_rn(__fdiv_rn(c2, c3), 0.5f), 0.5f);
+    return my > __fadd_rn(depth, 0.00002f);
+}
+
+// kDepth: the prepass with the mesh depth test (map: dw x dh floats as m2s_mesh_depth writes them)
+template <bool kStage, bool kDepth>
+__device__ __forceinline__ void prepass_body(const PrepassArgs& a, const float* map, uint32_t dw, uint32_t dh) {
     __shared__ float4 stage[kPrepassThreads / 32][32 * 6];   // 3 KB per warp: the warp's surviving quads
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     unsigned long long n = a.count;
@@ -87,6 +111,7 @@ __global__ void __launch_bounds__(kPrepassThreads) prepass_kernel(const __grid_c
         c3 = a.P[3] * vs0 + a.P[7] * vs1 + a.P[11] * vs2 + a.P[15] * vs3;
         const float clip = 1.05f * c3;                                   // :72-76
         if (c2 < -clip || c0 < -clip || c0 > clip || c1 < -clip || c1 > clip) alive = false;
+        if (kDepth && alive && a.layout == 0 && ca > 0.95f && prepass_behind_mesh(a, map, dw, dh, px, py, pz)) alive = false;
     }
     float4 q0, q1, q2, q3, q4, q5;
     q0 = q1 = q2 = q3 = q4 = q5 = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -179,11 +204,29 @@ __global__ void __launch_bounds__(kPrepassThreads) prepass_kernel(const __grid_c
     for (unsigned i = lane; i < cnt * 6; i += 32) dst[i] = stage[warp][i];
 }
 
+template <bool kStage>
+__global__ void __launch_bounds__(kPrepassThreads) prepass_kernel(const __grid_constant__ PrepassArgs a) {
+    prepass_body<kStage, false>(a, nullptr, 0, 0);
+}
+
+template <bool kStage>
+__global__ void __launch_bounds__(kPrepassThreads) prepass_depth_kernel(const __grid_constant__ PrepassDepthArgs a) {
+    prepass_body<kStage, true>(a.p, a.map, a.width, a.height);
+}
+
 cudaError_t prepass_launch(const PrepassArgs& args, cudaStream_t stream) {
     if (args.count == 0) return cudaSuccess;
     const unsigned long long blocks = (args.count + kPrepassThreads - 1) / kPrepassThreads;
     if (args.count >= (2ull << 20)) prepass_kernel<true><<<(unsigned)blocks, kPrepassThreads, 0, stream>>>(args);
     else prepass_kernel<false><<<(unsigned)blocks, kPrepassThreads, 0, stream>>>(args);
+    return cudaGetLastError();
+}
+
+cudaError_t prepass_depth_launch(const PrepassDepthArgs& args, cudaStream_t stream) {
+    if (args.p.count == 0) return cudaSuccess;
+    const unsigned long long blocks = (args.p.count + kPrepassThreads - 1) / kPrepassThreads;
+    if (args.p.count >= (2ull << 20)) prepass_depth_kernel<true><<<(unsigned)blocks, kPrepassThreads, 0, stream>>>(args);
+    else prepass_depth_kernel<false><<<(unsigned)blocks, kPrepassThreads, 0, stream>>>(args);
     return cudaGetLastError();
 }
 

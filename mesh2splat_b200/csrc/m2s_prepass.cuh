@@ -21,6 +21,14 @@ struct PrepassArgs {
     uint32_t* valid;
 };
 
+// the prepass with the mesh depth test: map is width x height floats, row 0 = window y 0 (m2s_depth.cu's output)
+struct PrepassDepthArgs {
+    PrepassArgs p;
+    const float* map;
+    uint32_t width, height;
+};
+
 cudaError_t prepass_launch(const PrepassArgs& args, cudaStream_t stream);
+cudaError_t prepass_depth_launch(const PrepassDepthArgs& args, cudaStream_t stream);
 
 }  // namespace m2s

@@ -49,7 +49,7 @@ struct SplatArgs {
     uint32_t* pairs;                // SortLayout(max_pairs) words (m2s_sort.cuh): the pair keys and values and their sort
 };
 
-// ---- shared with the cube raster of the shadow pass (m2s_light.cu) ------------------------------------------------
+// ---- shared with the cube raster of the shadow pass (m2s_light.cu) and the mesh depth pre-pass (m2s_depth.cu) ---
 // ---- the rasteriser's set-up (DESIGN §2): viewport transform, 1/256 snap, sign-normalised edge functions ----------
 // E_k(i, j) = A_k i + B_k j + C_k at the centre of pixel (i, j); inside iff E_k >= 0 where the edge owns its samples
 // (top-left rule), E_k > 0 elsewhere.  |X|, |Y| <= 2^21, so |A|, |B| <= 2^30 fit 32 bits.
@@ -60,15 +60,20 @@ struct SplatTri {
     int x0, x1, y0, y1;   // candidate pixel box, empty if x1 < x0 (also for a dropped or degenerate triangle)
 };
 
-__device__ __forceinline__ void splat_corner(const float4& m, const float4& s, float vx, float vy, float hw, float hh,
-                                             bool& ok, int& X, int& Y) {
-    // gaussianSplattingVS.glsl:32: mean.xy + (vx * scale.xy + vy * scale.zw), then xw = ndc * (W/2) + W/2
-    const float nx = __fadd_rn(m.x, __fadd_rn(__fmul_rn(vx, s.x), __fmul_rn(vy, s.z)));
-    const float ny = __fadd_rn(m.y, __fadd_rn(__fmul_rn(vx, s.y), __fmul_rn(vy, s.w)));
+// the viewport transform xw = ndc * (W/2) + W/2 and the 1/256 snap; ok is false outside the +-8192 guard band
+__device__ __forceinline__ void splat_snap(float nx, float ny, float hw, float hh, bool& ok, int& X, int& Y) {
     const float xw = __fadd_rn(__fmul_rn(nx, hw), hw), yw = __fadd_rn(__fmul_rn(ny, hh), hh);
     ok = isfinite(xw) && isfinite(yw) && fabsf(xw) <= 8192.0f && fabsf(yw) <= 8192.0f;
     X = ok ? __float2int_rn(__fmul_rn(xw, 256.0f)) : 0;
     Y = ok ? __float2int_rn(__fmul_rn(yw, 256.0f)) : 0;
+}
+
+__device__ __forceinline__ void splat_corner(const float4& m, const float4& s, float vx, float vy, float hw, float hh,
+                                             bool& ok, int& X, int& Y) {
+    // gaussianSplattingVS.glsl:32: mean.xy + (vx * scale.xy + vy * scale.zw)
+    const float nx = __fadd_rn(m.x, __fadd_rn(__fmul_rn(vx, s.x), __fmul_rn(vy, s.z)));
+    const float ny = __fadd_rn(m.y, __fadd_rn(__fmul_rn(vx, s.y), __fmul_rn(vy, s.w)));
+    splat_snap(nx, ny, hw, hh, ok, X, Y);
 }
 
 __device__ inline void splat_tri_setup(const int X[3], const int Y[3], bool ok, int W, int H, SplatTri& t) {
