@@ -11,6 +11,7 @@
 #include <vector>
 
 #include "../../include/m2s.h"
+#include "m2s_bin.cuh"
 #include "m2s_depth.cuh"
 #include "m2s_device.cuh"
 #include "m2s_light.cuh"
@@ -56,6 +57,12 @@ struct VRangeSlot {        // v-range reduction of one pipeline chunk: device bu
     unsigned long long* h_tag_dev = nullptr;
     unsigned long long tag = 0;               // the tag the current reduction will publish
     cudaEvent_t ev = nullptr;    // recorded behind the publish kernel (error path: a failed launch never writes the tag)
+};
+// scratch of one binned pass (the splat draw, the cube raster, the mesh depth pre-pass): per-item counts and tile ranges
+// (BinLayout, m2s_bin.cuh), and the pair sort (SortLayout, m2s_sort.cuh)
+struct BinScratch {
+    void* scratch = nullptr; size_t bytes = 0;
+    void* pairs = nullptr;   size_t pair_bytes = 0;
 };
 struct m2s_ctx {
     int device = 0;
@@ -109,17 +116,10 @@ struct m2s_ctx {
     void* d_items = nullptr;    size_t items_bytes = 0;     // FragItem queue
     // depth sort: control words, alternate key and value buffers (SortLayout, m2s_sort.cuh)
     void* d_sort = nullptr;     size_t sort_bytes = 0;
-    // splat draw: per-quad counts and tile ranges (SplatLayout, m2s_splat.cuh), and the pair sort (SortLayout)
-    void* d_splat = nullptr;    size_t splat_bytes = 0;
-    void* d_splat_pairs = nullptr; size_t splat_pairs_bytes = 0;
-    // shadow pass: light records when the caller passes none, per-record counts and tile ranges (shadow_layout,
-    // m2s_light.cuh), and the pair sort (SortLayout)
+    // the binned passes: splat draw, cube raster of the shadow pass, mesh depth pre-pass
+    BinScratch splat_bins, shadow_bins, depth_bins;
+    // shadow pass: light records when the caller passes none
     void* d_light_quads = nullptr; size_t light_quads_bytes = 0;
-    void* d_shadow = nullptr;   size_t shadow_bytes = 0;
-    void* d_shadow_pairs = nullptr; size_t shadow_pairs_bytes = 0;
-    // mesh depth pre-pass: per-triangle counts and tile ranges (SplatLayout), and the pair sort (SortLayout)
-    void* d_mdepth = nullptr;   size_t mdepth_bytes = 0;
-    void* d_mdepth_pairs = nullptr; size_t mdepth_pairs_bytes = 0;
 };
 
 struct m2s_dscene {
@@ -259,13 +259,11 @@ M2S_EXPORT void m2s_ctx_destroy(m2s_ctx* c) {
     if (c->d_trifrag) cudaFreeAsync(c->d_trifrag, c->stream);
     if (c->d_items) cudaFreeAsync(c->d_items, c->stream);
     if (c->d_sort) cudaFreeAsync(c->d_sort, c->stream);
-    if (c->d_splat) cudaFreeAsync(c->d_splat, c->stream);
-    if (c->d_splat_pairs) cudaFreeAsync(c->d_splat_pairs, c->stream);
     if (c->d_light_quads) cudaFreeAsync(c->d_light_quads, c->stream);
-    if (c->d_shadow) cudaFreeAsync(c->d_shadow, c->stream);
-    if (c->d_shadow_pairs) cudaFreeAsync(c->d_shadow_pairs, c->stream);
-    if (c->d_mdepth) cudaFreeAsync(c->d_mdepth, c->stream);
-    if (c->d_mdepth_pairs) cudaFreeAsync(c->d_mdepth_pairs, c->stream);
+    for (BinScratch* b : {&c->splat_bins, &c->shadow_bins, &c->depth_bins}) {
+        if (b->scratch) cudaFreeAsync(b->scratch, c->stream);
+        if (b->pairs) cudaFreeAsync(b->pairs, c->stream);
+    }
     cudaStreamSynchronize(c->stream);
     if (c->d_prepass_valid) cudaFree(c->d_prepass_valid);
     cudaFree(c->d_sched); cudaFree(c->d_counter); cudaFree(c->d_total); cudaFree(c->d_nitems);
@@ -1313,6 +1311,45 @@ M2S_EXPORT m2s_status m2s_depth_sort(m2s_ctx* ctx, const void* d_quads, const fl
 // Test aid (not part of m2s.h): the number of keys one tile of a sort pass holds.
 extern "C" __attribute__((visibility("default"))) uint32_t m2s_debug_sort_tile(void) { return (uint32_t)kSortTile; }
 
+// ---- the binned passes (splat draw, cube raster, mesh depth pre-pass): count -> size -> draw ----------------------
+// The steps after the pass's own front step has filled `a`, all on `stream`: size the pass's scratch (scratch_bytes,
+// its BinLayout), count the pairs, size the pair sort for the budget, then emit, sort and draw.
+//   enqueue form (sync false): the budget is max_pairs; the pair total and the drawn prefix are copied to the device
+//       words pairs and d_drawn (either may be NULL).
+//   synchronous form (sync true): the pair total is read back once and is the budget, 2^30 or more is rejected with
+//       the pass's message too_many; the stream is synchronised and the total stored in the host word *pairs (may be
+//       NULL).
+template <typename Args>
+static m2s_status bin_pass(m2s_ctx* ctx, BinScratch& s, size_t scratch_bytes, Args& a, cudaError_t (*count)(const Args&, cudaStream_t),
+                           cudaError_t (*draw)(const Args&, int, cudaStream_t), cudaStream_t stream, bool sync, uint64_t max_pairs,
+                           uint64_t* pairs, uint32_t* d_drawn, const char* too_many) {
+    m2s_status st = grow(ctx, &s.scratch, &s.bytes, scratch_bytes, stream);
+    if (st != M2S_OK) return st;
+    a.scratch = static_cast<unsigned char*>(s.scratch);
+    CUDA_TRY(count(a, stream));
+    if (sync) {
+        CUDA_TRY(cudaMemcpyAsync(ctx->h_total, a.scratch, sizeof(uint64_t), cudaMemcpyDeviceToHost, stream));
+        CUDA_TRY(cudaStreamSynchronize(stream));
+        max_pairs = *ctx->h_total;
+        if (max_pairs >= kSplatMaxPairs) { set_error(too_many); return M2S_E_INVALID; }
+    }
+    if (max_pairs) {
+        st = grow(ctx, &s.pairs, &s.pair_bytes, sort_layout(max_pairs).total_bytes, stream);
+        if (st != M2S_OK) return st;
+    }
+    a.max_pairs = max_pairs;
+    a.pairs = static_cast<uint32_t*>(s.pairs);
+    CUDA_TRY(draw(a, ctx->sm_count, stream));
+    if (sync) {
+        CUDA_TRY(cudaStreamSynchronize(stream));
+        if (pairs) *pairs = max_pairs;
+        return M2S_OK;
+    }
+    if (pairs) CUDA_TRY(cudaMemcpyAsync(pairs, a.scratch, sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
+    if (d_drawn) CUDA_TRY(cudaMemcpyAsync(d_drawn, a.scratch + 8, sizeof(uint32_t), cudaMemcpyDeviceToDevice, stream));
+    return M2S_OK;
+}
+
 // ---- the viewer's splat draw (SURVEY 8 f-6): GaussianSplattingPass::execute + gaussianSplattingVS/PS.glsl ----------
 static m2s_status splat_check(const m2s_ctx* ctx, const void* d_quads, uint64_t count, const m2s_splat_params* p, const m2s_gbuffer* g,
                               uint64_t max_pairs) {
@@ -1335,8 +1372,7 @@ static m2s_status splat_check(const m2s_ctx* ctx, const void* d_quads, uint64_t 
     return M2S_OK;
 }
 
-static SplatArgs splat_args(m2s_ctx* ctx, const void* d_quads, uint64_t count, const uint32_t* d_draw, const m2s_splat_params* p,
-                            const m2s_gbuffer* g) {
+static SplatArgs splat_args(const void* d_quads, uint64_t count, const uint32_t* d_draw, const m2s_splat_params* p, const m2s_gbuffer* g) {
     SplatArgs a;
     std::memset(&a, 0, sizeof(a));
     a.quads = static_cast<const float4*>(d_quads);
@@ -1344,7 +1380,6 @@ static SplatArgs splat_args(m2s_ctx* ctx, const void* d_quads, uint64_t count, c
     a.d_draw = d_draw;
     a.width = p->width; a.height = p->height; a.mode = p->render_mode;
     a.position = g->position; a.normal = g->normal; a.albedo = g->albedo; a.depth = g->depth; a.metallic_roughness = g->metallic_roughness;
-    a.scratch = static_cast<unsigned char*>(ctx->d_splat);
     return a;
 }
 
@@ -1354,21 +1389,9 @@ M2S_EXPORT m2s_status m2s_splat_draw_enqueue(m2s_ctx* ctx, const void* d_sorted_
     m2s_status st = splat_check(ctx, d_sorted_quads, count, p, g, max_pairs);
     if (st != M2S_OK) return st;
     CUDA_TRY(cudaSetDevice(ctx->device));
-    cudaStream_t stream = stream_ ? (cudaStream_t)stream_ : ctx->stream;
-    st = grow(ctx, &ctx->d_splat, &ctx->splat_bytes, splat_layout(count, p->width, p->height).total_bytes, stream);
-    if (st != M2S_OK) return st;
-    if (max_pairs) {
-        st = grow(ctx, &ctx->d_splat_pairs, &ctx->splat_pairs_bytes, sort_layout(max_pairs).total_bytes, stream);
-        if (st != M2S_OK) return st;
-    }
-    SplatArgs a = splat_args(ctx, d_sorted_quads, count, d_draw, p, g);
-    a.max_pairs = max_pairs;
-    a.pairs = static_cast<uint32_t*>(ctx->d_splat_pairs);
-    CUDA_TRY(splat_count_launch(a, stream));
-    CUDA_TRY(splat_draw_launch(a, ctx->sm_count, stream));
-    if (d_pairs) CUDA_TRY(cudaMemcpyAsync(d_pairs, a.scratch, sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
-    if (d_drawn) CUDA_TRY(cudaMemcpyAsync(d_drawn, a.scratch + 8, sizeof(uint32_t), cudaMemcpyDeviceToDevice, stream));
-    return M2S_OK;
+    SplatArgs a = splat_args(d_sorted_quads, count, d_draw, p, g);
+    return bin_pass(ctx, ctx->splat_bins, bin_layout(count, splat_tiles(p->width, p->height)).total_bytes, a, splat_count_launch,
+                    splat_draw_launch, stream_ ? (cudaStream_t)stream_ : ctx->stream, false, max_pairs, d_pairs, d_drawn, nullptr);
 }
 
 M2S_EXPORT m2s_status m2s_splat_draw(m2s_ctx* ctx, const void* d_sorted_quads, uint64_t count, const m2s_splat_params* p,
@@ -1376,25 +1399,9 @@ M2S_EXPORT m2s_status m2s_splat_draw(m2s_ctx* ctx, const void* d_sorted_quads, u
     m2s_status st = splat_check(ctx, d_sorted_quads, count, p, g, 0);
     if (st != M2S_OK) return st;
     CUDA_TRY(cudaSetDevice(ctx->device));
-    cudaStream_t stream = ctx->stream;
-    st = grow(ctx, &ctx->d_splat, &ctx->splat_bytes, splat_layout(count, p->width, p->height).total_bytes, stream);
-    if (st != M2S_OK) return st;
-    SplatArgs a = splat_args(ctx, d_sorted_quads, count, nullptr, p, g);
-    CUDA_TRY(splat_count_launch(a, stream));
-    CUDA_TRY(cudaMemcpyAsync(ctx->h_total, a.scratch, sizeof(uint64_t), cudaMemcpyDeviceToHost, stream));
-    CUDA_TRY(cudaStreamSynchronize(stream));
-    const uint64_t total = *ctx->h_total;
-    if (total >= kSplatMaxPairs) { set_error("m2s_splat_draw: the quads need 2^30 or more (tile, quad) pairs"); return M2S_E_INVALID; }
-    if (total) {
-        st = grow(ctx, &ctx->d_splat_pairs, &ctx->splat_pairs_bytes, sort_layout(total).total_bytes, stream);
-        if (st != M2S_OK) return st;
-    }
-    a.max_pairs = total;
-    a.pairs = static_cast<uint32_t*>(ctx->d_splat_pairs);
-    CUDA_TRY(splat_draw_launch(a, ctx->sm_count, stream));
-    CUDA_TRY(cudaStreamSynchronize(stream));
-    if (pairs) *pairs = total;
-    return M2S_OK;
+    SplatArgs a = splat_args(d_sorted_quads, count, nullptr, p, g);
+    return bin_pass(ctx, ctx->splat_bins, bin_layout(count, splat_tiles(p->width, p->height)).total_bytes, a, splat_count_launch,
+                    splat_draw_launch, ctx->stream, true, 0, pairs, nullptr, "m2s_splat_draw: the quads need 2^30 or more (tile, quad) pairs");
 }
 
 // ---- the viewer's shadow pass (SURVEY 8 f-7): GaussianShadowPass::execute + gaussianPointShadowMappingCS.glsl + the
@@ -1476,7 +1483,7 @@ static m2s_status shadow_check(const m2s_ctx* ctx, const void* d_records, uint64
     return M2S_OK;
 }
 
-// the light prepass and the pair count; a.light_quads / a.scratch set up
+// the uniforms, the light records (the context's when the caller passes none) and the light prepass
 static m2s_status shadow_front(m2s_ctx* ctx, const void* d_records, uint64_t count, const uint64_t* d_count, const m2s_shadow_params* p,
                                float* d_cube, void* d_light_quads, cudaStream_t stream, ShadowArgs& a) {
     std::memset(&a, 0, sizeof(a));
@@ -1486,16 +1493,12 @@ static m2s_status shadow_front(m2s_ctx* ctx, const void* d_records, uint64_t cou
         if (st != M2S_OK) return st;
         d_light_quads = ctx->d_light_quads;
     }
-    m2s_status st = grow(ctx, &ctx->d_shadow, &ctx->shadow_bytes, shadow_layout(count, p->size).total_bytes, stream);
-    if (st != M2S_OK) return st;
     a.records = static_cast<const unsigned char*>(d_records);
     a.count = count;
     a.d_count = reinterpret_cast<const unsigned long long*>(d_count);
     a.light_quads = static_cast<float4*>(d_light_quads);
     a.cube = d_cube;
-    a.scratch = static_cast<unsigned char*>(ctx->d_shadow);
     CUDA_TRY(light_prepass_launch(a, stream));
-    CUDA_TRY(shadow_count_launch(a, stream));
     return M2S_OK;
 }
 
@@ -1506,19 +1509,11 @@ M2S_EXPORT m2s_status m2s_shadow_map_enqueue(m2s_ctx* ctx, const void* d_records
     if (st != M2S_OK) return st;
     CUDA_TRY(cudaSetDevice(ctx->device));
     cudaStream_t stream = stream_ ? (cudaStream_t)stream_ : ctx->stream;
-    if (max_pairs) {
-        st = grow(ctx, &ctx->d_shadow_pairs, &ctx->shadow_pairs_bytes, sort_layout(max_pairs).total_bytes, stream);
-        if (st != M2S_OK) return st;
-    }
     ShadowArgs a;
     st = shadow_front(ctx, d_records, count, d_count, p, d_cube, d_light_quads, stream, a);
     if (st != M2S_OK) return st;
-    a.max_pairs = max_pairs;
-    a.pairs = static_cast<uint32_t*>(ctx->d_shadow_pairs);
-    CUDA_TRY(shadow_draw_launch(a, ctx->sm_count, stream));
-    if (d_pairs) CUDA_TRY(cudaMemcpyAsync(d_pairs, a.scratch, sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
-    if (d_drawn) CUDA_TRY(cudaMemcpyAsync(d_drawn, a.scratch + 8, sizeof(uint32_t), cudaMemcpyDeviceToDevice, stream));
-    return M2S_OK;
+    return bin_pass(ctx, ctx->shadow_bins, bin_layout(count, shadow_tiles(p->size)).total_bytes, a, shadow_count_launch, shadow_draw_launch,
+                    stream, false, max_pairs, d_pairs, d_drawn, nullptr);
 }
 
 M2S_EXPORT m2s_status m2s_shadow_map(m2s_ctx* ctx, const void* d_records, uint64_t count, const m2s_shadow_params* p, float* d_cube,
@@ -1526,24 +1521,11 @@ M2S_EXPORT m2s_status m2s_shadow_map(m2s_ctx* ctx, const void* d_records, uint64
     m2s_status st = shadow_check(ctx, d_records, count, p, d_cube, d_light_quads, 0);
     if (st != M2S_OK) return st;
     CUDA_TRY(cudaSetDevice(ctx->device));
-    cudaStream_t stream = ctx->stream;
     ShadowArgs a;
-    st = shadow_front(ctx, d_records, count, nullptr, p, d_cube, d_light_quads, stream, a);
+    st = shadow_front(ctx, d_records, count, nullptr, p, d_cube, d_light_quads, ctx->stream, a);
     if (st != M2S_OK) return st;
-    CUDA_TRY(cudaMemcpyAsync(ctx->h_total, a.scratch, sizeof(uint64_t), cudaMemcpyDeviceToHost, stream));
-    CUDA_TRY(cudaStreamSynchronize(stream));
-    const uint64_t total = *ctx->h_total;
-    if (total >= kSplatMaxPairs) { set_error("m2s_shadow_map: the records need 2^30 or more (tile, record) pairs"); return M2S_E_INVALID; }
-    if (total) {
-        st = grow(ctx, &ctx->d_shadow_pairs, &ctx->shadow_pairs_bytes, sort_layout(total).total_bytes, stream);
-        if (st != M2S_OK) return st;
-    }
-    a.max_pairs = total;
-    a.pairs = static_cast<uint32_t*>(ctx->d_shadow_pairs);
-    CUDA_TRY(shadow_draw_launch(a, ctx->sm_count, stream));
-    CUDA_TRY(cudaStreamSynchronize(stream));
-    if (pairs) *pairs = total;
-    return M2S_OK;
+    return bin_pass(ctx, ctx->shadow_bins, bin_layout(count, shadow_tiles(p->size)).total_bytes, a, shadow_count_launch, shadow_draw_launch,
+                    ctx->stream, true, 0, pairs, nullptr, "m2s_shadow_map: the records need 2^30 or more (tile, record) pairs");
 }
 
 // ---- the viewer's deferred lighting (SURVEY 8 f-8): GaussianRelightingPass::execute + gaussianSplattingDeferredPS.glsl
@@ -1612,9 +1594,8 @@ static m2s_status mesh_depth_check(const m2s_ctx* ctx, const m2s_dscene* scene, 
     return M2S_OK;
 }
 
-// the pair count; a.scratch set up
-static m2s_status mesh_depth_front(m2s_ctx* ctx, const m2s_dscene* scene, const m2s_mesh_depth_params* p, float* d_depth,
-                                   cudaStream_t stream, DepthArgs& a) {
+static DepthArgs mesh_depth_args(const m2s_dscene* scene, const m2s_mesh_depth_params* p, float* d_depth) {
+    DepthArgs a;
     std::memset(&a, 0, sizeof(a));
     float pv[16];
     glm_mat4_mul(p->view_to_clip, p->world_to_view, pv);
@@ -1627,11 +1608,7 @@ static m2s_status mesh_depth_front(m2s_ctx* ctx, const m2s_dscene* scene, const 
     a.width = p->width;
     a.height = p->height;
     a.depth = d_depth;
-    m2s_status st = grow(ctx, &ctx->d_mdepth, &ctx->mdepth_bytes, splat_layout(a.ntri, a.width, a.height).total_bytes, stream);
-    if (st != M2S_OK) return st;
-    a.scratch = static_cast<unsigned char*>(ctx->d_mdepth);
-    CUDA_TRY(depth_count_launch(a, stream));
-    return M2S_OK;
+    return a;
 }
 
 M2S_EXPORT m2s_status m2s_mesh_depth_enqueue(m2s_ctx* ctx, const m2s_dscene* scene, const m2s_mesh_depth_params* p, float* d_depth,
@@ -1639,42 +1616,16 @@ M2S_EXPORT m2s_status m2s_mesh_depth_enqueue(m2s_ctx* ctx, const m2s_dscene* sce
     m2s_status st = mesh_depth_check(ctx, scene, p, d_depth, max_pairs);
     if (st != M2S_OK) return st;
     CUDA_TRY(cudaSetDevice(ctx->device));
-    cudaStream_t stream = stream_ ? (cudaStream_t)stream_ : ctx->stream;
-    if (max_pairs) {
-        st = grow(ctx, &ctx->d_mdepth_pairs, &ctx->mdepth_pairs_bytes, sort_layout(max_pairs).total_bytes, stream);
-        if (st != M2S_OK) return st;
-    }
-    DepthArgs a;
-    st = mesh_depth_front(ctx, scene, p, d_depth, stream, a);
-    if (st != M2S_OK) return st;
-    a.max_pairs = max_pairs;
-    a.pairs = static_cast<uint32_t*>(ctx->d_mdepth_pairs);
-    CUDA_TRY(depth_draw_launch(a, ctx->sm_count, stream));
-    if (d_pairs) CUDA_TRY(cudaMemcpyAsync(d_pairs, a.scratch, sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
-    if (d_drawn) CUDA_TRY(cudaMemcpyAsync(d_drawn, a.scratch + 8, sizeof(uint32_t), cudaMemcpyDeviceToDevice, stream));
-    return M2S_OK;
+    DepthArgs a = mesh_depth_args(scene, p, d_depth);
+    return bin_pass(ctx, ctx->depth_bins, bin_layout(a.ntri, splat_tiles(a.width, a.height)).total_bytes, a, depth_count_launch,
+                    depth_draw_launch, stream_ ? (cudaStream_t)stream_ : ctx->stream, false, max_pairs, d_pairs, d_drawn, nullptr);
 }
 
 M2S_EXPORT m2s_status m2s_mesh_depth(m2s_ctx* ctx, const m2s_dscene* scene, const m2s_mesh_depth_params* p, float* d_depth, uint64_t* pairs) {
     m2s_status st = mesh_depth_check(ctx, scene, p, d_depth, 0);
     if (st != M2S_OK) return st;
     CUDA_TRY(cudaSetDevice(ctx->device));
-    cudaStream_t stream = ctx->stream;
-    DepthArgs a;
-    st = mesh_depth_front(ctx, scene, p, d_depth, stream, a);
-    if (st != M2S_OK) return st;
-    CUDA_TRY(cudaMemcpyAsync(ctx->h_total, a.scratch, sizeof(uint64_t), cudaMemcpyDeviceToHost, stream));
-    CUDA_TRY(cudaStreamSynchronize(stream));
-    const uint64_t total = *ctx->h_total;
-    if (total >= kSplatMaxPairs) { set_error("m2s_mesh_depth: the triangles need 2^30 or more (tile, triangle) pairs"); return M2S_E_INVALID; }
-    if (total) {
-        st = grow(ctx, &ctx->d_mdepth_pairs, &ctx->mdepth_pairs_bytes, sort_layout(total).total_bytes, stream);
-        if (st != M2S_OK) return st;
-    }
-    a.max_pairs = total;
-    a.pairs = static_cast<uint32_t*>(ctx->d_mdepth_pairs);
-    CUDA_TRY(depth_draw_launch(a, ctx->sm_count, stream));
-    CUDA_TRY(cudaStreamSynchronize(stream));
-    if (pairs) *pairs = total;
-    return M2S_OK;
+    DepthArgs a = mesh_depth_args(scene, p, d_depth);
+    return bin_pass(ctx, ctx->depth_bins, bin_layout(a.ntri, splat_tiles(a.width, a.height)).total_bytes, a, depth_count_launch,
+                    depth_draw_launch, ctx->stream, true, 0, pairs, nullptr, "m2s_mesh_depth: the triangles need 2^30 or more (tile, triangle) pairs");
 }

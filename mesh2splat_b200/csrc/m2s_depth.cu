@@ -3,23 +3,18 @@
 // opaque primitive (baseColorFactor.a == 1.0f) drawn into a W x H D24 map cleared to 1, depth test LESS, no culling.
 //
 // Shape (the shadow pass's cube raster over one W x H viewport, DESIGN §2 "The mesh depth pre-pass"):
-//   depth_count_kernel   per source triangle: transform, clip (six planes, guard factor 2 in x and y), fan, snap, and
-//                        the 16 x 16 tiles each fan triangle touches; scanned within the block
-//   depth_scan_kernel    one CTA: exclusive prefix over the block sums; the total number of pairs
-//   depth_emit_kernel    (tile, source triangle << 3 | fan triangle) pairs of the longest prefix of source triangles
-//                        that fits the budget
-//   sort_pairs16_launch  the depth sort's stable onesweep sort of the pairs by tile id (m2s_sort.cu)
-//   depth_ranges_kernel  each tile's run in the sorted pairs
+//   binning (m2s_bin.cuh) per source triangle: transform, clip (six planes, guard factor 2 in x and y), fan, snap,
+//                        and the 16 x 16 tiles each fan triangle touches; (tile, source triangle << 3 | fan triangle)
+//                        pairs of the longest prefix of source triangles that fits the budget, stably sorted by tile;
+//                        each tile's run
 //   depth_tile_kernel    one CTA per tile, one thread per pixel: fan triangles staged in shared memory, depth from the
 //                        exact edge values in fp64, the minimum D24 code in a register, one store per texel
 // The unit of a pair is the fan triangle, so the tile kernel stages one triangle per pair; it re-clips the source
 // triangle to find it (a triangle that needs no clipping is its own fan of one).  Every operation that decides a bit of
 // the map is round-to-nearest fp32 / fp64 with no contraction (__f*_rn, __d*_rn), integer, or a conversion of DESIGN
 // §2, so the map equals the oracle's (oracle/m2s_depth_oracle.c) bit for bit.
-#include <algorithm>
-
+#include "m2s_bin.cuh"
 #include "m2s_depth.cuh"
-#include "m2s_sort.cuh"
 
 namespace m2s {
 
@@ -143,121 +138,29 @@ __device__ __forceinline__ uint32_t depth_for_each_tile(const SplatTri& t, int t
     return c;
 }
 
-constexpr int kDepthScanThreads = 1024;
 }  // namespace
 
-__global__ void __launch_bounds__(kSplatBlock) depth_count_kernel(DepthArgs a) {
-    __shared__ uint32_t s_warp[kSplatBlock / 32];
-    const SplatLayout l = splat_layout(a.ntri, a.width, a.height);
-    uint32_t* excl = reinterpret_cast<uint32_t*>(a.scratch + l.excl_off);
-    unsigned long long* blocks = reinterpret_cast<unsigned long long*>(a.scratch + l.blocks_off);
-    const uint64_t i = (uint64_t)blockIdx.x * kSplatBlock + threadIdx.x;
-    uint32_t cnt = 0;
-    if (i < a.ntri) {
+// the binning (m2s_bin.cuh): source triangles, n = ntri, one pair per tile each fan triangle touches, pair value =
+// source triangle << 3 | fan triangle
+struct DepthBins {
+    DepthArgs a;
+    __host__ __device__ unsigned long long items() const { return a.ntri; }
+    __host__ __device__ uint64_t tiles() const { return splat_tiles(a.width, a.height); }
+    __device__ __forceinline__ uint32_t n() const { return (uint32_t)a.ntri; }
+    template <typename F>
+    __device__ __forceinline__ uint32_t visit(uint32_t i, F&& f) const {
         float4 v[kDepthMaxPoly];
-        const int n = depth_poly(a, (uint32_t)i, v);
+        const int np = depth_poly(a, i, v);
         const int tx = depth_tiles_x(a);
-        for (int k = 0; k + 2 < n; ++k) {
+        uint32_t cnt = 0;
+        for (int k = 0; k + 2 < np; ++k) {
             DepthTri d;
             depth_fan(a, v, k, d);
-            cnt += depth_for_each_tile(d.t, tx, [](uint32_t, uint32_t) {});
+            cnt += depth_for_each_tile(d.t, tx, [&](uint32_t, uint32_t tile) { f(tile, i << 3 | (uint32_t)k); });
         }
+        return cnt;
     }
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t x = cnt;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
-        if (lane >= o) x += y;
-    }
-    if (lane == 31) s_warp[warp] = x;
-    __syncthreads();
-    uint32_t before = 0, total = 0;
-#pragma unroll
-    for (int w = 0; w < kSplatBlock / 32; ++w) {
-        before += w < warp ? s_warp[w] : 0u;
-        total += s_warp[w];
-    }
-    if (i < a.ntri) excl[i] = before + x - cnt;
-    if (threadIdx.x == 0) blocks[blockIdx.x] = total;
-}
-
-__global__ void __launch_bounds__(kDepthScanThreads) depth_scan_kernel(DepthArgs a) {
-    __shared__ unsigned long long s_warp[kDepthScanThreads / 32];
-    __shared__ unsigned long long s_carry;
-    const SplatLayout l = splat_layout(a.ntri, a.width, a.height);
-    unsigned long long* blocks = reinterpret_cast<unsigned long long*>(a.scratch + l.blocks_off);
-    const uint32_t nb = (uint32_t)l.blocks;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) s_carry = 0;
-    __syncthreads();
-    for (uint32_t base = 0; base < nb; base += kDepthScanThreads) {
-        const uint32_t b = base + threadIdx.x;
-        const unsigned long long v = b < nb ? blocks[b] : 0ull;
-        unsigned long long x = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
-            if (lane >= o) x += y;
-        }
-        if (lane == 31) s_warp[warp] = x;
-        __syncthreads();
-        unsigned long long before = s_carry, chunk = 0;
-        for (int w = 0; w < kDepthScanThreads / 32; ++w) {
-            before += w < warp ? s_warp[w] : 0ull;
-            chunk += s_warp[w];
-        }
-        if (b < nb) blocks[b] = before + x - v;
-        __syncthreads();
-        if (threadIdx.x == 0) s_carry += chunk;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *reinterpret_cast<unsigned long long*>(a.scratch) = s_carry;
-}
-
-__global__ void __launch_bounds__(kSplatBlock) depth_emit_kernel(DepthArgs a, uint32_t* keys, uint32_t* vals) {
-    const SplatLayout l = splat_layout(a.ntri, a.width, a.height);
-    const uint32_t* excl = reinterpret_cast<const uint32_t*>(a.scratch + l.excl_off);
-    const unsigned long long* blocks = reinterpret_cast<const unsigned long long*>(a.scratch + l.blocks_off);
-    uint32_t* ctrl = reinterpret_cast<uint32_t*>(a.scratch);
-    const unsigned long long total = *reinterpret_cast<const unsigned long long*>(a.scratch);
-    const uint32_t n = (uint32_t)a.ntri;
-    const uint64_t i64 = (uint64_t)blockIdx.x * kSplatBlock + threadIdx.x;
-    if (i64 >= n) return;
-    const uint32_t i = (uint32_t)i64;
-    auto offset = [&](uint32_t k) { return k < n ? blocks[k / kSplatBlock] + excl[k] : total; };
-    const unsigned long long start = offset(i), end = offset(i + 1);
-    if (end > a.max_pairs) return;   // not in the prefix whose pairs fit
-    if (i + 1 == n || offset(i + 2) > a.max_pairs) {   // the prefix's last triangle
-        ctrl[2] = i + 1;
-        ctrl[3] = (uint32_t)end;
-    }
-    if (end == start) return;
-    float4 v[kDepthMaxPoly];
-    const int np = depth_poly(a, i, v);
-    const int tx = depth_tiles_x(a);
-    unsigned long long at = start;
-    for (int k = 0; k + 2 < np; ++k) {
-        DepthTri d;
-        depth_fan(a, v, k, d);
-        at += depth_for_each_tile(d.t, tx, [&](uint32_t c, uint32_t tile) {
-            keys[at + c] = tile;
-            vals[at + c] = i << 3 | (uint32_t)k;
-        });
-    }
-}
-
-__global__ void depth_ranges_kernel(DepthArgs a, const uint32_t* keys) {
-    const SplatLayout l = splat_layout(a.ntri, a.width, a.height);
-    uint32_t* start = reinterpret_cast<uint32_t*>(a.scratch + l.ranges_off);
-    uint32_t* end = start + l.tiles;
-    const uint32_t np = reinterpret_cast<const uint32_t*>(a.scratch)[3];
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < np; i += gridDim.x * blockDim.x) {
-        const uint32_t k = keys[i];
-        if (i == 0 || keys[i - 1] != k) start[k] = i;
-        if (i + 1 == np || keys[i + 1] != k) end[k] = i + 1;
-    }
-}
+};
 
 struct DepthStage {
     int32_t A[3][kSplatThreads], B[3][kSplatThreads];
@@ -288,7 +191,7 @@ __device__ __noinline__ void depth_stage(const DepthArgs& a, uint32_t v, int ox,
 
 __global__ void __launch_bounds__(kSplatThreads) depth_tile_kernel(const __grid_constant__ DepthArgs a, const uint32_t* __restrict__ vals) {
     __shared__ DepthStage s;
-    const SplatLayout l = splat_layout(a.ntri, a.width, a.height);
+    const BinLayout l = bin_layout(a.ntri, splat_tiles(a.width, a.height));
     const uint32_t* start = reinterpret_cast<const uint32_t*>(a.scratch + l.ranges_off);
     const uint32_t tile = blockIdx.x, tx = (uint32_t)depth_tiles_x(a);
     const int ox = (int)(tile % tx) * kSplatTile, oy = (int)(tile / tx) * kSplatTile;
@@ -326,29 +229,13 @@ __global__ void __launch_bounds__(kSplatThreads) depth_tile_kernel(const __grid_
 }
 
 // ---- launches -------------------------------------------------------------------------------------------------------
-cudaError_t depth_count_launch(const DepthArgs& a, cudaStream_t stream) {
-    cudaError_t e = cudaMemsetAsync(a.scratch, 0, 16, stream);   // total pairs, drawn, pairs emitted
-    if (e != cudaSuccess) return e;
-    const SplatLayout l = splat_layout(a.ntri, a.width, a.height);
-    if (l.blocks) depth_count_kernel<<<(unsigned)l.blocks, kSplatBlock, 0, stream>>>(a);
-    depth_scan_kernel<<<1, kDepthScanThreads, 0, stream>>>(a);
-    return cudaGetLastError();
-}
+cudaError_t depth_count_launch(const DepthArgs& a, cudaStream_t stream) { return bin_count_launch(DepthBins{a}, stream); }
 
 cudaError_t depth_draw_launch(const DepthArgs& a, int sm_count, cudaStream_t stream) {
-    const SplatLayout l = splat_layout(a.ntri, a.width, a.height);
-    cudaError_t e = cudaMemsetAsync(a.scratch + l.ranges_off, 0, l.tiles * 8, stream);
+    const DepthBins b{a};
+    const cudaError_t e = bin_pairs_launch(b, sm_count, stream);
     if (e != cudaSuccess) return e;
-    uint32_t* keys = a.max_pairs ? sort_pairs16_keys(a.pairs, a.max_pairs) : nullptr;
-    uint32_t* vals = a.max_pairs ? sort_pairs16_vals(a.pairs, a.max_pairs) : nullptr;
-    if (l.blocks) depth_emit_kernel<<<(unsigned)l.blocks, kSplatBlock, 0, stream>>>(a, keys, vals);
-    if (a.max_pairs > 0) {
-        e = sort_pairs16_launch(a.pairs, a.max_pairs, reinterpret_cast<const uint32_t*>(a.scratch) + 3, sm_count, stream);
-        if (e != cudaSuccess) return e;
-        const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((a.max_pairs + 255) / 256, 8ull * sm_count));
-        depth_ranges_kernel<<<grid, 256, 0, stream>>>(a, keys);
-    }
-    depth_tile_kernel<<<(unsigned)l.tiles, kSplatThreads, 0, stream>>>(a, vals);
+    depth_tile_kernel<<<(unsigned)b.tiles(), kSplatThreads, 0, stream>>>(a, bin_vals(b));
     return cudaGetLastError();
 }
 

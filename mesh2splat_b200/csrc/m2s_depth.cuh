@@ -15,7 +15,7 @@ constexpr int kDepthMaxPoly = 9;                    // a triangle clipped by six
 constexpr float kDepthGuard = 2.0f;                 // x, y clipped to +-G w: |xw| <= 1.5 * 4096 < 8192 (DESIGN §2)
 constexpr uint32_t kDepthClearCode = 0xFFFFFFu;     // D24 clear value 1.0 = 2^24 - 1
 
-// Scratch: the splat draw's layout (SplatLayout) with one pair count per SOURCE triangle, W x H pixels.
+// Scratch: bin_layout (m2s_bin.cuh) with one pair count per SOURCE triangle, W x H pixels.
 struct DepthArgs {
     const float4* tris;             // the scene's triangle soup, 9 float4 per triangle (m2s_device.cuh)
     unsigned long long ntri;        // < kDepthMaxTris
@@ -26,7 +26,7 @@ struct DepthArgs {
     uint32_t width, height;
     float* depth;                   // W x H floats: (float)code / 16777215, row 0 = window y 0
     unsigned long long max_pairs;   // (tile, fan triangle) pair budget (< kSplatMaxPairs)
-    unsigned char* scratch;         // splat_layout(ntri, width, height)
+    unsigned char* scratch;         // bin_layout(ntri, splat_tiles(width, height))
     uint32_t* pairs;                // SortLayout(max_pairs) words (m2s_sort.cuh)
 };
 

@@ -8,23 +8,19 @@
 //
 // Shape:
 //   light_prepass_kernel   one thread per source record: one 32-byte light record in source order (no per-face append)
-//   shadow_count_kernel    per record: the 16 x 16 tiles of its face its two triangles touch (the splat draw's binning
-//                          over 6 faces), scanned within the block
-//   shadow_scan_kernel     one CTA: exclusive prefix over the block sums; the total number of pairs
-//   shadow_emit_kernel     (tile, record) pairs of the longest prefix that fits the budget
-//   sort_pairs16_launch    the depth sort's stable onesweep sort of the pairs by tile id (m2s_sort.cu)
-//   shadow_ranges_kernel   each tile's run in the sorted pairs
+//   binning (m2s_bin.cuh)  per record: the 16 x 16 tiles of its face its two triangles touch (the splat draw's test
+//                          over 6 faces); (tile, record) pairs of the longest prefix that fits the budget, stably sorted
+//                          by tile; each tile's run
 //   shadow_tile_kernel     one CTA per tile, one thread per texel: the minimum depth code in registers (depth is constant
 //                          per quad and the test is LESS, so the result does not depend on draw order), one store
 //   deferred_light_kernel  one thread per pixel: fetch, shade, RGBA8
 // Every operation that decides a bit of the output is round-to-nearest fp32 with no contraction (__f*_rn), integer, or
 // one of the conversions of DESIGN §2, so the records, the cube and the image equal the oracle's
 // (oracle/m2s_light_oracle.c) bit for bit.
-#include <algorithm>
 #include <cuda_fp16.h>
 
+#include "m2s_bin.cuh"
 #include "m2s_light.cuh"
-#include "m2s_sort.cuh"
 
 namespace m2s {
 
@@ -140,12 +136,6 @@ __global__ void __launch_bounds__(kLightPrepassThreads) light_prepass_kernel(con
 }
 
 // ---- cube raster ----------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t shadow_n(const ShadowArgs& a) {
-    unsigned long long n = a.count;
-    if (a.d_count) n = min(n, *a.d_count);
-    return (uint32_t)n;   // count < 2^30
-}
-
 // D24 (DESIGN §2): round-half-even(clamp(d, 0, 1) * (2^24 - 1)), the product exact in fp64; false for NaN (no write)
 __device__ __forceinline__ bool shadow_code(float d, uint32_t& code) {
     if (d != d) return false;
@@ -165,114 +155,27 @@ __device__ __forceinline__ bool shadow_setup(const float4* r, uint32_t S, SplatT
 
 __device__ __forceinline__ int shadow_tiles_x(uint32_t S) { return (int)((S + kSplatTile - 1) / kSplatTile); }
 
-template <typename F>
-__device__ __forceinline__ uint32_t shadow_for_each_tile(const float4* r, uint32_t S, F&& f) {
-    SplatTri t[2];
-    uint32_t face, code;
-    if (!shadow_setup(r, S, t, face, code)) return 0;
-    const int tx = shadow_tiles_x(S);
-    const uint32_t base = face * (uint32_t)(tx * tx);
-    return splat_for_each_tile(t, tx, [&](uint32_t c, uint32_t tile) { f(c, base + tile); });
-}
-
-__global__ void __launch_bounds__(kSplatBlock) shadow_count_kernel(ShadowArgs a) {
-    __shared__ uint32_t s_warp[kSplatBlock / 32];
-    const SplatLayout l = shadow_layout(a.count, a.size);
-    uint32_t* excl = reinterpret_cast<uint32_t*>(a.scratch + l.excl_off);
-    unsigned long long* blocks = reinterpret_cast<unsigned long long*>(a.scratch + l.blocks_off);
-    const uint32_t n = shadow_n(a);
-    const uint64_t i = (uint64_t)blockIdx.x * kSplatBlock + threadIdx.x;
-    if ((uint64_t)blockIdx.x * kSplatBlock >= n) return;
-    const uint32_t cnt = i < n ? shadow_for_each_tile(a.light_quads + i * 2, a.size, [](uint32_t, uint32_t) {}) : 0u;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t x = cnt;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
-        if (lane >= o) x += y;
+// the binning (m2s_bin.cuh): light records, n = min(count, *d_count), tile = face * (S/16)^2 + tile of the face, pair
+// value = record index
+struct ShadowBins {
+    ShadowArgs a;
+    __host__ __device__ unsigned long long items() const { return a.count; }
+    __host__ __device__ uint64_t tiles() const { return shadow_tiles(a.size); }
+    __device__ __forceinline__ uint32_t n() const {
+        unsigned long long n = a.count;
+        if (a.d_count) n = min(n, *a.d_count);
+        return (uint32_t)n;   // count < 2^30
     }
-    if (lane == 31) s_warp[warp] = x;
-    __syncthreads();
-    uint32_t before = 0, total = 0;
-#pragma unroll
-    for (int w = 0; w < kSplatBlock / 32; ++w) {
-        before += w < warp ? s_warp[w] : 0u;
-        total += s_warp[w];
+    template <typename F>
+    __device__ __forceinline__ uint32_t visit(uint32_t i, F&& f) const {
+        SplatTri t[2];
+        uint32_t face, code;
+        if (!shadow_setup(a.light_quads + (uint64_t)i * 2, a.size, t, face, code)) return 0;
+        const int tx = shadow_tiles_x(a.size);
+        const uint32_t base = face * (uint32_t)(tx * tx);
+        return splat_for_each_tile(t, tx, [&](uint32_t, uint32_t tile) { f(base + tile, i); });
     }
-    if (i < n) excl[i] = before + x - cnt;
-    if (threadIdx.x == 0) blocks[blockIdx.x] = total;
-}
-
-constexpr int kShadowScanThreads = 1024;
-
-__global__ void __launch_bounds__(kShadowScanThreads) shadow_scan_kernel(ShadowArgs a) {
-    __shared__ unsigned long long s_warp[kShadowScanThreads / 32];
-    __shared__ unsigned long long s_carry;
-    const SplatLayout l = shadow_layout(a.count, a.size);
-    unsigned long long* blocks = reinterpret_cast<unsigned long long*>(a.scratch + l.blocks_off);
-    const uint32_t nb = (shadow_n(a) + kSplatBlock - 1) / kSplatBlock;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) s_carry = 0;
-    __syncthreads();
-    for (uint32_t base = 0; base < nb; base += kShadowScanThreads) {
-        const uint32_t b = base + threadIdx.x;
-        const unsigned long long v = b < nb ? blocks[b] : 0ull;
-        unsigned long long x = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
-            if (lane >= o) x += y;
-        }
-        if (lane == 31) s_warp[warp] = x;
-        __syncthreads();
-        unsigned long long before = s_carry, chunk = 0;
-        for (int w = 0; w < kShadowScanThreads / 32; ++w) {
-            before += w < warp ? s_warp[w] : 0ull;
-            chunk += s_warp[w];
-        }
-        if (b < nb) blocks[b] = before + x - v;
-        __syncthreads();
-        if (threadIdx.x == 0) s_carry += chunk;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *reinterpret_cast<unsigned long long*>(a.scratch) = s_carry;
-}
-
-__global__ void __launch_bounds__(kSplatBlock) shadow_emit_kernel(ShadowArgs a, uint32_t* keys, uint32_t* vals) {
-    const SplatLayout l = shadow_layout(a.count, a.size);
-    const uint32_t* excl = reinterpret_cast<const uint32_t*>(a.scratch + l.excl_off);
-    const unsigned long long* blocks = reinterpret_cast<const unsigned long long*>(a.scratch + l.blocks_off);
-    uint32_t* ctrl = reinterpret_cast<uint32_t*>(a.scratch);
-    const unsigned long long total = *reinterpret_cast<const unsigned long long*>(a.scratch);
-    const uint32_t n = shadow_n(a);
-    const uint64_t i64 = (uint64_t)blockIdx.x * kSplatBlock + threadIdx.x;
-    if (i64 >= n) return;
-    const uint32_t i = (uint32_t)i64;
-    auto offset = [&](uint32_t k) { return k < n ? blocks[k / kSplatBlock] + excl[k] : total; };
-    const unsigned long long start = offset(i), end = offset(i + 1);
-    if (end > a.max_pairs) return;   // not in the prefix whose pairs fit
-    if (i + 1 == n || offset(i + 2) > a.max_pairs) {   // the prefix's last record
-        ctrl[2] = i + 1;
-        ctrl[3] = (uint32_t)end;
-    }
-    if (end == start) return;
-    shadow_for_each_tile(a.light_quads + (uint64_t)i * 2, a.size, [&](uint32_t c, uint32_t tile) {
-        keys[start + c] = tile;
-        vals[start + c] = i;
-    });
-}
-
-__global__ void shadow_ranges_kernel(ShadowArgs a, const uint32_t* keys) {
-    const SplatLayout l = shadow_layout(a.count, a.size);
-    uint32_t* start = reinterpret_cast<uint32_t*>(a.scratch + l.ranges_off);
-    uint32_t* end = start + l.tiles;
-    const uint32_t np = reinterpret_cast<const uint32_t*>(a.scratch)[3];
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < np; i += gridDim.x * blockDim.x) {
-        const uint32_t k = keys[i];
-        if (i == 0 || keys[i - 1] != k) start[k] = i;
-        if (i + 1 == np || keys[i + 1] != k) end[k] = i + 1;
-    }
-}
+};
 
 struct ShadowStage {
     int32_t A[6][kSplatThreads], B[6][kSplatThreads];
@@ -282,7 +185,7 @@ struct ShadowStage {
 
 __global__ void __launch_bounds__(kSplatThreads) shadow_tile_kernel(ShadowArgs a, const uint32_t* __restrict__ vals) {
     __shared__ ShadowStage s;
-    const SplatLayout l = shadow_layout(a.count, a.size);
+    const BinLayout l = bin_layout(a.count, shadow_tiles(a.size));
     const uint32_t* start = reinterpret_cast<const uint32_t*>(a.scratch + l.ranges_off);
     const uint32_t S = a.size, tx = (uint32_t)shadow_tiles_x(S), tpf = tx * tx;
     const uint32_t tile = blockIdx.x, face = tile / tpf, lt = tile % tpf;
@@ -495,29 +398,13 @@ cudaError_t light_prepass_launch(const ShadowArgs& a, cudaStream_t stream) {
     return cudaGetLastError();
 }
 
-cudaError_t shadow_count_launch(const ShadowArgs& a, cudaStream_t stream) {
-    cudaError_t e = cudaMemsetAsync(a.scratch, 0, 16, stream);   // total pairs, drawn, pairs emitted
-    if (e != cudaSuccess) return e;
-    const SplatLayout l = shadow_layout(a.count, a.size);
-    if (l.blocks) shadow_count_kernel<<<(unsigned)l.blocks, kSplatBlock, 0, stream>>>(a);
-    shadow_scan_kernel<<<1, kShadowScanThreads, 0, stream>>>(a);
-    return cudaGetLastError();
-}
+cudaError_t shadow_count_launch(const ShadowArgs& a, cudaStream_t stream) { return bin_count_launch(ShadowBins{a}, stream); }
 
 cudaError_t shadow_draw_launch(const ShadowArgs& a, int sm_count, cudaStream_t stream) {
-    const SplatLayout l = shadow_layout(a.count, a.size);
-    cudaError_t e = cudaMemsetAsync(a.scratch + l.ranges_off, 0, l.tiles * 8, stream);
+    const ShadowBins b{a};
+    const cudaError_t e = bin_pairs_launch(b, sm_count, stream);
     if (e != cudaSuccess) return e;
-    uint32_t* keys = a.max_pairs ? sort_pairs16_keys(a.pairs, a.max_pairs) : nullptr;
-    uint32_t* vals = a.max_pairs ? sort_pairs16_vals(a.pairs, a.max_pairs) : nullptr;
-    if (l.blocks) shadow_emit_kernel<<<(unsigned)l.blocks, kSplatBlock, 0, stream>>>(a, keys, vals);
-    if (a.max_pairs > 0) {
-        e = sort_pairs16_launch(a.pairs, a.max_pairs, reinterpret_cast<const uint32_t*>(a.scratch) + 3, sm_count, stream);
-        if (e != cudaSuccess) return e;
-        const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((a.max_pairs + 255) / 256, 8ull * sm_count));
-        shadow_ranges_kernel<<<grid, 256, 0, stream>>>(a, keys);
-    }
-    shadow_tile_kernel<<<(unsigned)l.tiles, kSplatThreads, 0, stream>>>(a, vals);
+    shadow_tile_kernel<<<(unsigned)b.tiles(), kSplatThreads, 0, stream>>>(a, bin_vals(b));
     return cudaGetLastError();
 }
 

@@ -21,13 +21,8 @@ constexpr int kLightThreads = 256;                        // deferred lighting: 
 // face is 0..5 (+X -X +Y -Y +Z -Z), or kShadowCulled with every other word 0.
 constexpr size_t kLightRecordBytes = 32;
 
-// Cube raster scratch: the splat draw's layout (SplatLayout) over 6 faces of S x S pixels, i.e. 6 S ceil(S/16) tiles.
-__host__ __device__ inline SplatLayout shadow_layout(uint64_t count, uint32_t size) {
-    SplatLayout l = splat_layout(count, size, size);
-    l.tiles *= 6;
-    l.total_bytes = l.ranges_off + l.tiles * 8;
-    return l;
-}
+// the cube raster's tiles: 6 faces of S x S pixels, each ceil(S/16)^2 tiles of 16 x 16
+__host__ __device__ inline uint64_t shadow_tiles(uint32_t size) { return splat_tiles(size, size) * 6; }
 
 struct ShadowArgs {
     // light prepass (gaussianPointShadowMappingCS.glsl)
@@ -49,15 +44,16 @@ struct ShadowArgs {
     uint32_t size;
     float* cube;                    // 6 x size x size floats: (float)code / 16777215
     unsigned long long max_pairs;   // (tile, record) pair budget (< kSplatMaxPairs)
-    unsigned char* scratch;         // shadow_layout(count, size)
+    unsigned char* scratch;         // bin_layout(count, shadow_tiles(size)) (m2s_bin.cuh)
     uint32_t* pairs;                // SortLayout(max_pairs) words (m2s_sort.cuh)
 };
 
 // the light prepass: one 32-byte record per source gaussian
 cudaError_t light_prepass_launch(const ShadowArgs& a, cudaStream_t stream);
-// counts and scans the (tile, record) pairs of the n light records; the total lands in the scratch's ctrl words
+// counts and scans the (tile, record) pairs of the n light records (bin_count_launch); the total lands in the ctrl words
 cudaError_t shadow_count_launch(const ShadowArgs& a, cudaStream_t stream);
-// emits and sorts the pairs of the longest prefix that fits max_pairs, then writes every texel of the cube
+// emits and sorts the pairs of the longest prefix that fits max_pairs (bin_pairs_launch), then writes every texel of the
+// cube
 cudaError_t shadow_draw_launch(const ShadowArgs& a, int sm_count, cudaStream_t stream);
 
 struct LightArgs {

@@ -4,147 +4,40 @@
 // (GL_ONE_MINUS_DST_ALPHA, GL_ONE; GL_ONE, GL_ONE in render mode 4).  The fixed-function parts follow DESIGN §2.
 //
 // Shape: a tiled rasteriser that keeps GL's per-pixel order (instance, then triangle):
-//   splat_count_kernel    per quad: snap the four corners, set up both triangles, count the 16 x 16 tiles they touch
-//                         (edge functions against the tile's pixel-centre box), scan the counts within the block
-//   splat_scan_kernel     one CTA: exclusive prefix over the block sums; the total number of pairs
-//   splat_emit_kernel     per quad of the prefix whose pairs fit the budget: its (tile, quad) pairs at its scan offset, so
-//                         the pairs come out in quad order; the prefix length and its pair count
-//   sort_pairs16_launch   stable onesweep sort of the pairs by tile id (the depth sort's kernels, m2s_sort.cu)
-//   splat_ranges_kernel   each tile's run in the sorted pairs
+//   binning (m2s_bin.cuh) per quad: snap the four corners, set up both triangles, the 16 x 16 tiles they touch (edge
+//                         functions against the tile's pixel-centre box); (tile, quad) pairs of the longest prefix of
+//                         quads that fits the budget, in quad order, stably sorted by tile; each tile's run
 //   splat_tile_kernel     one CTA per tile, one thread per pixel: the tile's quads staged in shared memory in batches,
 //                         coverage, fragment shader and blends in registers (each target rounded to its format after
 //                         every blend), one coalesced store per live target
 // All arithmetic that decides a bit of the image is round-to-nearest fp32 with no contraction (__f*_rn), integer, or
 // the conversions to the target formats, so the image equals the oracle's (oracle/m2s_splat_oracle.c) bit for bit.
-#include <algorithm>
 #include <cuda_fp16.h>
 
-#include "m2s_sort.cuh"
+#include "m2s_bin.cuh"
 #include "m2s_splat.cuh"
 
 namespace m2s {
 
-__device__ __forceinline__ uint32_t splat_n(const SplatArgs& a) {
-    unsigned long long n = a.count;
-    if (a.d_draw) n = min(n, (unsigned long long)a.d_draw[1]);
-    return (uint32_t)n;   // count < 2^30
-}
-
 __device__ __forceinline__ int splat_tiles_x(const SplatArgs& a) { return (int)((a.width + kSplatTile - 1) / kSplatTile); }
 
-// ---- count and scan ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kSplatBlock) splat_count_kernel(SplatArgs a) {
-    __shared__ uint32_t s_warp[kSplatBlock / 32];
-    const SplatLayout l = splat_layout(a.count, a.width, a.height);
-    uint32_t* excl = reinterpret_cast<uint32_t*>(a.scratch + l.excl_off);
-    unsigned long long* blocks = reinterpret_cast<unsigned long long*>(a.scratch + l.blocks_off);
-    const uint32_t n = splat_n(a);
-    const uint64_t i = (uint64_t)blockIdx.x * kSplatBlock + threadIdx.x;
-    if ((uint64_t)blockIdx.x * kSplatBlock >= n) return;   // blocks at or past n are never read
-    uint32_t cnt = 0;
-    if (i < n) {
+// ---- binning (m2s_bin.cuh): quads, n = min(count, d_draw[1]), pair value = quad index -------------------------------
+struct SplatBins {
+    SplatArgs a;
+    __host__ __device__ unsigned long long items() const { return a.count; }
+    __host__ __device__ uint64_t tiles() const { return splat_tiles(a.width, a.height); }
+    __device__ __forceinline__ uint32_t n() const {
+        unsigned long long n = a.count;
+        if (a.d_draw) n = min(n, (unsigned long long)a.d_draw[1]);
+        return (uint32_t)n;   // count < 2^30
+    }
+    template <typename F>
+    __device__ __forceinline__ uint32_t visit(uint32_t i, F&& f) const {
         SplatTri t[2];
-        splat_quad_setup(a.quads + i * 6, (int)a.width, (int)a.height, t);
-        cnt = splat_for_each_tile(t, splat_tiles_x(a), [](uint32_t, uint32_t) {});
+        splat_quad_setup(a.quads + (uint64_t)i * 6, (int)a.width, (int)a.height, t);
+        return splat_for_each_tile(t, splat_tiles_x(a), [&](uint32_t, uint32_t tile) { f(tile, i); });
     }
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t x = cnt;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
-        if (lane >= o) x += y;
-    }
-    if (lane == 31) s_warp[warp] = x;
-    __syncthreads();
-    uint32_t before = 0, total = 0;
-#pragma unroll
-    for (int w = 0; w < kSplatBlock / 32; ++w) {
-        before += w < warp ? s_warp[w] : 0u;
-        total += s_warp[w];
-    }
-    if (i < n) excl[i] = before + x - cnt;
-    if (threadIdx.x == 0) blocks[blockIdx.x] = total;
-}
-
-constexpr int kSplatScanThreads = 1024;
-
-__global__ void __launch_bounds__(kSplatScanThreads) splat_scan_kernel(SplatArgs a) {
-    __shared__ unsigned long long s_warp[kSplatScanThreads / 32];
-    __shared__ unsigned long long s_carry;
-    const SplatLayout l = splat_layout(a.count, a.width, a.height);
-    unsigned long long* blocks = reinterpret_cast<unsigned long long*>(a.scratch + l.blocks_off);
-    const uint32_t n = splat_n(a);
-    const uint32_t nb = (n + kSplatBlock - 1) / kSplatBlock;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) s_carry = 0;
-    __syncthreads();
-    for (uint32_t base = 0; base < nb; base += kSplatScanThreads) {
-        const uint32_t b = base + threadIdx.x;
-        const unsigned long long v = b < nb ? blocks[b] : 0ull;
-        unsigned long long x = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
-            if (lane >= o) x += y;
-        }
-        if (lane == 31) s_warp[warp] = x;
-        __syncthreads();
-        unsigned long long before = s_carry, chunk = 0;
-        for (int w = 0; w < kSplatScanThreads / 32; ++w) {
-            before += w < warp ? s_warp[w] : 0ull;
-            chunk += s_warp[w];
-        }
-        if (b < nb) blocks[b] = before + x - v;
-        __syncthreads();
-        if (threadIdx.x == 0) s_carry += chunk;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *reinterpret_cast<unsigned long long*>(a.scratch) = s_carry;
-}
-
-// ---- pair emission -------------------------------------------------------------------------------------------------
-__device__ __forceinline__ unsigned long long splat_offset(const uint32_t* excl, const unsigned long long* blocks, uint32_t i,
-                                                           uint32_t n, unsigned long long total) {
-    return i < n ? blocks[i / kSplatBlock] + excl[i] : total;
-}
-
-__global__ void __launch_bounds__(kSplatBlock) splat_emit_kernel(SplatArgs a, uint32_t* keys, uint32_t* vals) {
-    const SplatLayout l = splat_layout(a.count, a.width, a.height);
-    const uint32_t* excl = reinterpret_cast<const uint32_t*>(a.scratch + l.excl_off);
-    const unsigned long long* blocks = reinterpret_cast<const unsigned long long*>(a.scratch + l.blocks_off);
-    uint32_t* ctrl = reinterpret_cast<uint32_t*>(a.scratch);
-    const unsigned long long total = *reinterpret_cast<const unsigned long long*>(a.scratch);
-    const uint32_t n = splat_n(a);
-    const uint64_t i64 = (uint64_t)blockIdx.x * kSplatBlock + threadIdx.x;
-    if (i64 >= n) return;
-    const uint32_t i = (uint32_t)i64;
-    const unsigned long long start = splat_offset(excl, blocks, i, n, total);
-    const unsigned long long end = splat_offset(excl, blocks, i + 1, n, total);
-    if (end > a.max_pairs) return;   // not in the prefix whose pairs fit
-    if (i + 1 == n || splat_offset(excl, blocks, i + 2, n, total) > a.max_pairs) {   // the prefix's last quad
-        ctrl[2] = i + 1;
-        ctrl[3] = (uint32_t)end;
-    }
-    if (end == start) return;
-    SplatTri t[2];
-    splat_quad_setup(a.quads + (uint64_t)i * 6, (int)a.width, (int)a.height, t);
-    splat_for_each_tile(t, splat_tiles_x(a), [&](uint32_t c, uint32_t tile) {
-        keys[start + c] = tile;
-        vals[start + c] = i;
-    });
-}
-
-__global__ void splat_ranges_kernel(SplatArgs a, const uint32_t* keys) {
-    const SplatLayout l = splat_layout(a.count, a.width, a.height);
-    uint32_t* start = reinterpret_cast<uint32_t*>(a.scratch + l.ranges_off);
-    uint32_t* end = start + l.tiles;
-    const uint32_t np = reinterpret_cast<const uint32_t*>(a.scratch)[3];
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < np; i += gridDim.x * blockDim.x) {
-        const uint32_t k = keys[i];
-        if (i == 0 || keys[i - 1] != k) start[k] = i;
-        if (i + 1 == np || keys[i + 1] != k) end[k] = i + 1;
-    }
-}
+};
 
 // ---- fragment shader, blend, formats -------------------------------------------------------------------------------
 
@@ -188,7 +81,7 @@ struct SplatStage {
 
 __global__ void __launch_bounds__(kSplatThreads) splat_tile_kernel(SplatArgs a, const uint32_t* __restrict__ vals) {
     __shared__ SplatStage s;
-    const SplatLayout l = splat_layout(a.count, a.width, a.height);
+    const BinLayout l = bin_layout(a.count, splat_tiles(a.width, a.height));
     const uint32_t* start = reinterpret_cast<const uint32_t*>(a.scratch + l.ranges_off);
     const uint32_t tiles_x = (uint32_t)splat_tiles_x(a);
     const uint32_t tile = blockIdx.x;
@@ -288,33 +181,13 @@ __global__ void __launch_bounds__(kSplatThreads) splat_tile_kernel(SplatArgs a, 
 }
 
 // ---- launches ------------------------------------------------------------------------------------------------------
-cudaError_t splat_count_launch(const SplatArgs& a, cudaStream_t stream) {
-    cudaError_t e = cudaMemsetAsync(a.scratch, 0, 16, stream);   // total pairs, drawn, pairs emitted
-    if (e != cudaSuccess) return e;
-    const SplatLayout l = splat_layout(a.count, a.width, a.height);
-    if (l.blocks) splat_count_kernel<<<(unsigned)l.blocks, kSplatBlock, 0, stream>>>(a);
-    splat_scan_kernel<<<1, kSplatScanThreads, 0, stream>>>(a);
-    return cudaGetLastError();
-}
+cudaError_t splat_count_launch(const SplatArgs& a, cudaStream_t stream) { return bin_count_launch(SplatBins{a}, stream); }
 
 cudaError_t splat_draw_launch(const SplatArgs& a, int sm_count, cudaStream_t stream) {
-    const SplatLayout l = splat_layout(a.count, a.width, a.height);
-    cudaError_t e = cudaMemsetAsync(a.scratch + l.ranges_off, 0, l.tiles * 8, stream);
+    const SplatBins b{a};
+    const cudaError_t e = bin_pairs_launch(b, sm_count, stream);
     if (e != cudaSuccess) return e;
-    // with no budget the emission still finds the prefix (the leading quads that touch no tile) and writes no pair
-    uint32_t* keys = a.max_pairs ? sort_pairs16_keys(a.pairs, a.max_pairs) : nullptr;
-    uint32_t* vals = a.max_pairs ? sort_pairs16_vals(a.pairs, a.max_pairs) : nullptr;
-    if (l.blocks) splat_emit_kernel<<<(unsigned)l.blocks, kSplatBlock, 0, stream>>>(a, keys, vals);
-    if (a.max_pairs > 0) {
-        const uint32_t* d_np = reinterpret_cast<const uint32_t*>(a.scratch) + 3;
-        e = sort_pairs16_launch(a.pairs, a.max_pairs, d_np, sm_count, stream);
-        if (e != cudaSuccess) return e;
-        const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((a.max_pairs + 255) / 256, 8ull * sm_count));
-        splat_ranges_kernel<<<grid, 256, 0, stream>>>(a, keys);
-        splat_tile_kernel<<<(unsigned)l.tiles, kSplatThreads, 0, stream>>>(a, vals);
-    } else {
-        splat_tile_kernel<<<(unsigned)l.tiles, kSplatThreads, 0, stream>>>(a, nullptr);
-    }
+    splat_tile_kernel<<<(unsigned)b.tiles(), kSplatThreads, 0, stream>>>(a, bin_vals(b));
     return cudaGetLastError();
 }
 

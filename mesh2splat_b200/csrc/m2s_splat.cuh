@@ -9,29 +9,13 @@ namespace m2s {
 
 constexpr int kSplatTile = 16;                           // screen tiles of 16 x 16 pixels, one CTA per tile
 constexpr int kSplatThreads = kSplatTile * kSplatTile;   // tile kernel: one thread per pixel
-constexpr int kSplatBlock = 512;                         // quads per CTA of the per-quad kernels (and per scan block)
 constexpr uint32_t kSplatMaxSide = 4096;                 // 256 x 256 tiles: a tile id fits in 16 bits
 constexpr uint64_t kSplatMaxCount = 1ull << 30;
 constexpr uint64_t kSplatMaxPairs = 1ull << 30;          // the pair sort's count limit (kSortMaxCount)
 
-// Per-call scratch (bytes), one allocation:
-//   ctrl    uint64 total pairs | uint32 drawn | uint32 pairs emitted (= pairs of the drawn prefix)
-//   excl    uint32 per quad: exclusive prefix of the pair counts within its block of kSplatBlock quads
-//   blocks  uint64 per block: its pair count, then (in place) the exclusive prefix over the blocks
-//   ranges  uint32 [2][tiles]: start and end of each tile's run in the sorted pairs (zeroed per call)
-struct SplatLayout {
-    uint64_t blocks, tiles;
-    size_t excl_off, blocks_off, ranges_off, total_bytes;
-};
-__host__ __device__ inline SplatLayout splat_layout(uint64_t count, uint32_t width, uint32_t height) {
-    SplatLayout l;
-    l.blocks = (count + kSplatBlock - 1) / kSplatBlock;
-    l.tiles = (uint64_t)((width + kSplatTile - 1) / kSplatTile) * ((height + kSplatTile - 1) / kSplatTile);
-    l.excl_off = 256;
-    l.blocks_off = (l.excl_off + count * 4 + 255) & ~size_t(255);
-    l.ranges_off = (l.blocks_off + l.blocks * 8 + 255) & ~size_t(255);
-    l.total_bytes = l.ranges_off + l.tiles * 8;
-    return l;
+// the 16 x 16 tiles of a W x H viewport
+__host__ __device__ inline uint64_t splat_tiles(uint32_t width, uint32_t height) {
+    return (uint64_t)((width + kSplatTile - 1) / kSplatTile) * ((height + kSplatTile - 1) / kSplatTile);
 }
 
 struct SplatArgs {
@@ -45,7 +29,7 @@ struct SplatArgs {
     uint16_t* depth;
     uint8_t* metallic_roughness;
     unsigned long long max_pairs;   // pair budget (< kSplatMaxPairs)
-    unsigned char* scratch;         // SplatLayout of (count, width, height)
+    unsigned char* scratch;         // bin_layout(count, splat_tiles(width, height)) (m2s_bin.cuh)
     uint32_t* pairs;                // SortLayout(max_pairs) words (m2s_sort.cuh): the pair keys and values and their sort
 };
 
@@ -164,9 +148,9 @@ __device__ __forceinline__ float splat_exp(float x) {
     return __fmul_rn(__fmul_rn(p, __int_as_float((k1 + 127) << 23)), __int_as_float((k2 + 127) << 23));
 }
 
-// counts the (tile, quad) pairs of the n quads and scans them; the total lands in the scratch's ctrl words
+// counts the (tile, quad) pairs of the n quads and scans them (bin_count_launch); the total lands in the ctrl words
 cudaError_t splat_count_launch(const SplatArgs& a, cudaStream_t stream);
-// emits and sorts the pairs of the longest prefix that fits max_pairs, then draws every tile
+// emits and sorts the pairs of the longest prefix that fits max_pairs (bin_pairs_launch), then draws every tile
 cudaError_t splat_draw_launch(const SplatArgs& a, int sm_count, cudaStream_t stream);
 
 }  // namespace m2s

@@ -82,9 +82,9 @@ def main():
         g = {"setup": 0.0, "binning": 0.0, "tile": 0.0}
         for e in prof.key_averages():
             t = getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0))
-            if "depth_count" in e.key or "depth_scan" in e.key:
+            if "DepthBins" in e.key and ("bin_count" in e.key or "bin_scan" in e.key):
                 g["setup"] += t
-            elif "depth_emit" in e.key or "depth_ranges" in e.key or "sort_" in e.key:
+            elif ("DepthBins" in e.key and ("bin_emit" in e.key or "bin_ranges" in e.key)) or "sort_" in e.key:
                 g["binning"] += t
             elif "depth_tile" in e.key:
                 g["tile"] += t

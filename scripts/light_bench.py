@@ -79,7 +79,7 @@ def main():
             t = getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0))
             if "light_prepass_kernel" in e.key:
                 pre += t
-            elif "shadow_" in e.key or "sort_" in e.key:
+            elif "shadow_" in e.key or "ShadowBins" in e.key or "sort_" in e.key:
                 ras += t
         return pre / args.iters, ras / args.iters
 
