@@ -53,7 +53,7 @@ class m2s_result(C.Structure):
 
 
 class m2s_convert_plan(C.Structure):
-    """ConvertPlan (m2s_api.cu), filled by m2s_debug_convert_plan: the launch a conversion makes and its route."""
+    """ConvertPlan (m2s_convert.cu), filled by m2s_debug_convert_plan: the launch a conversion makes and its route."""
     _fields_ = [(n, C.c_uint64) for n in ("grid", "raster_warps", "unit_tris", "n_units", "item_max", "flush_frags",
                                           "queue_cap", "cap", "multi_round", "direct_ok", "claim_late", "direct_max")]
 

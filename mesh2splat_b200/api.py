@@ -27,6 +27,23 @@ def _torch():
     return torch
 
 
+def _binned_pass(dev, max_pairs, n, draw, draw_enqueue):
+    """The two forms of a binned pass (splat draw, mesh depth, shadow map); returns (drawn, pairs).  max_pairs None:
+    draw(pairs) synchronously, all n items drawn.  Otherwise draw_enqueue(max_pairs, d_pairs, d_drawn, stream) on torch's
+    current stream with that pair budget, then the pair total and the drawn prefix read back."""
+    torch = _torch()
+    if max_pairs is None:
+        torch.cuda.synchronize(dev)   # the buffers torch filled are ready before the context stream reads them
+        pairs = C.c_uint64(0)
+        check(draw(C.byref(pairs)))
+        return n, int(pairs.value)
+    out = torch.zeros(4, dtype=torch.int32, device=dev)   # pairs (uint64) | drawn (uint32)
+    check(draw_enqueue(max_pairs, out.data_ptr(), out[2:].data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+    torch.cuda.synchronize(dev)
+    o = out.cpu().numpy()
+    return int(o[2]), int(o[:2].view(np.uint64)[0])
+
+
 class DeviceScene:
     """Device-resident scene (triangles, primitive table, mip chains): what loadModel leaves on the
     GPU in the reference (VBOs + GL textures)."""
@@ -250,20 +267,12 @@ class Context:
                 gbuffer[name] = torch.empty(width * height * 4, dtype=torch.int16 if dt == np.float16 else torch.uint8, device=dev)
             setattr(g, name, gbuffer[name].data_ptr())
         p = _abi.m2s_splat_params(width, height, render_mode)
-        if max_pairs is None:
-            torch.cuda.synchronize(dev)   # the buffers torch filled are ready before the context stream reads them
-            pairs = C.c_uint64(0)
-            check(lib().m2s_splat_draw(self.handle, sorted_quads.data_ptr(), count, C.byref(p), C.byref(g), C.byref(pairs)))
-            drawn, npairs = count, int(pairs.value)
-        else:
-            out = torch.zeros(4, dtype=torch.int32, device=dev)   # pairs (uint64) | drawn (uint32)
-            check(lib().m2s_splat_draw_enqueue(self.handle, sorted_quads.data_ptr(), count,
-                                               d_draw.data_ptr() if d_draw is not None else None, C.byref(p), C.byref(g),
-                                               max_pairs, out.data_ptr(), out[2:].data_ptr(),
-                                               torch.cuda.current_stream(dev).cuda_stream))
-            torch.cuda.synchronize(dev)
-            o = out.cpu().numpy()
-            npairs, drawn = int(o[:2].view(np.uint64)[0]), int(o[2])
+        drawn, npairs = _binned_pass(
+            dev, max_pairs, count,
+            lambda pairs: lib().m2s_splat_draw(self.handle, sorted_quads.data_ptr(), count, C.byref(p), C.byref(g), pairs),
+            lambda *budget: lib().m2s_splat_draw_enqueue(self.handle, sorted_quads.data_ptr(), count,
+                                                         d_draw.data_ptr() if d_draw is not None else None, C.byref(p),
+                                                         C.byref(g), *budget))
         images = {}
         for name, dt in _abi.GBUFFER_TARGETS:
             if name in targets:
@@ -284,18 +293,10 @@ class Context:
         elif depth.dtype != torch.float32 or depth.device != dev or not depth.is_contiguous() or depth.numel() < width * height:
             raise ValueError("depth must be a contiguous float32 tensor of at least width * height values on the context's device")
         p = _abi.make_mesh_depth_params(world_to_view, view_to_clip, model_to_world, width, height)
-        if max_pairs is None:
-            torch.cuda.synchronize(dev)
-            pairs = C.c_uint64(0)
-            check(lib().m2s_mesh_depth(self.handle, dscene.handle, C.byref(p), depth.data_ptr(), C.byref(pairs)))
-            drawn, npairs = dscene.triangle_count, int(pairs.value)
-        else:
-            out = torch.zeros(4, dtype=torch.int32, device=dev)   # pairs (uint64) | drawn (uint32)
-            check(lib().m2s_mesh_depth_enqueue(self.handle, dscene.handle, C.byref(p), depth.data_ptr(), max_pairs, out.data_ptr(),
-                                               out[2:].data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
-            torch.cuda.synchronize(dev)
-            o = out.cpu().numpy()
-            npairs, drawn = int(o[:2].view(np.uint64)[0]), int(o[2])
+        drawn, npairs = _binned_pass(
+            dev, max_pairs, dscene.triangle_count,
+            lambda pairs: lib().m2s_mesh_depth(self.handle, dscene.handle, C.byref(p), depth.data_ptr(), pairs),
+            lambda *budget: lib().m2s_mesh_depth_enqueue(self.handle, dscene.handle, C.byref(p), depth.data_ptr(), *budget))
         return depth.reshape(-1)[: width * height].cpu().numpy().reshape(height, width).copy(), drawn, npairs
 
     def shadow_map(self, records, count: int, layout: int, model_to_world, light_position, near_far, resolution, std_dev: float,
@@ -312,20 +313,13 @@ class Context:
         if light_quads is None:
             light_quads = torch.empty(max(1, count) * _abi.LIGHT_RECORD_BYTES, dtype=torch.uint8, device=dev)
         p = _abi.make_shadow_params(model_to_world, light_position, near_far, resolution, std_dev, layout, size)
-        if max_pairs is None:
-            torch.cuda.synchronize(dev)   # the buffers torch filled are ready before the context stream reads them
-            pairs = C.c_uint64(0)
-            check(lib().m2s_shadow_map(self.handle, records.data_ptr(), count, C.byref(p), cube.data_ptr(), light_quads.data_ptr(),
-                                       C.byref(pairs)))
-            drawn, npairs = count, int(pairs.value)
-        else:
-            out = torch.zeros(4, dtype=torch.int32, device=dev)   # pairs (uint64) | drawn (uint32)
-            check(lib().m2s_shadow_map_enqueue(self.handle, records.data_ptr(), count, d_count.data_ptr() if d_count is not None else None,
-                                               C.byref(p), cube.data_ptr(), light_quads.data_ptr(), max_pairs, out.data_ptr(),
-                                               out[2:].data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
-            torch.cuda.synchronize(dev)
-            o = out.cpu().numpy()
-            npairs, drawn = int(o[:2].view(np.uint64)[0]), int(o[2])
+        drawn, npairs = _binned_pass(
+            dev, max_pairs, count,
+            lambda pairs: lib().m2s_shadow_map(self.handle, records.data_ptr(), count, C.byref(p), cube.data_ptr(),
+                                               light_quads.data_ptr(), pairs),
+            lambda *budget: lib().m2s_shadow_map_enqueue(self.handle, records.data_ptr(), count,
+                                                         d_count.data_ptr() if d_count is not None else None, C.byref(p),
+                                                         cube.data_ptr(), light_quads.data_ptr(), *budget))
         lq = light_quads.view(torch.uint8)[: count * _abi.LIGHT_RECORD_BYTES].cpu().numpy().view(np.float32).reshape(count, 8).copy()
         return cube[: 6 * size * size].cpu().numpy().reshape(6, size, size).copy(), lq, drawn, npairs
 

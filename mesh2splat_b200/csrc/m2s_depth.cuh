@@ -1,5 +1,5 @@
 // m2s_depth.cuh — arguments and scratch layout of the viewer's mesh depth pre-pass (m2s_depth.cu), shared with the C-ABI
-// host code (m2s_api.cu).
+// host code (m2s_viewer.cu).
 #pragma once
 #include <cstddef>
 #include <cstdint>

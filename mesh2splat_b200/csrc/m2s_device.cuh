@@ -124,4 +124,18 @@ struct ConvertArgs {
     uint32_t* status;                  // context status word (mapped pinned host memory): bit 0/1 = a gather wait timed out
 };
 
+// ---- launchers (m2s_kernels.cu) ----
+int convert_warps_per_cta(int layout);
+size_t tri_frag_bytes(int layout);
+cudaError_t convert_configure(int layout, int* raster_blocks_per_sm, int* fragment_blocks_per_sm);
+cudaError_t convert_launch(int layout, const ConvertArgs& args, int raster_grid, int fragment_grid, cudaStream_t stream, cudaEvent_t mid);
+cudaError_t gather_wait_launch(const unsigned long long* xch, uint32_t world, unsigned long long epoch, unsigned long long gcap,
+                               unsigned long long* total_global, uint32_t* status, cudaStream_t stream);
+cudaError_t mip_groups_launch(uint32_t* arena, const DTexture& t, uint32_t g0, uint32_t g1, cudaStream_t stream);
+cudaError_t vrange_launch(const float4* tris, uint32_t first, uint32_t count, const DRange* ranges, uint32_t nranges, const DPrim* prims,
+                          uint32_t ntex, int* minmax, cudaStream_t stream);
+cudaError_t vrange_publish_launch(int* minmax, uint32_t ntex, int* host, unsigned long long* host_tag, unsigned long long tag, cudaStream_t stream);
+cudaError_t ply_rows_launch(const void* ref96, unsigned long long count, const unsigned long long* d_count,
+                            uint32_t format, float mult, void* rows, cudaStream_t stream);
+
 }  // namespace m2s

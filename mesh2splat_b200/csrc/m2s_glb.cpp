@@ -31,15 +31,7 @@
 #include <string>
 #include <vector>
 
-#include "../../include/m2s.h"
-
-namespace m2s {
-void set_error(const std::string& msg);
-m2s_status write_ply_rows(const char* path, uint32_t format, const void* rows, uint64_t count);
-m2s_status convert_scene_to_ply(m2s_ctx* ctx, const m2s_scene* sc, const m2s_params* p, const char* path, m2s_result* res);
-}
-
-#define M2S_EXPORT extern "C" __attribute__((visibility("default")))
+#include "m2s_host.h"
 
 namespace {
 

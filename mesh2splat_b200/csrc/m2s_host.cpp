@@ -9,14 +9,12 @@
 #include <string>
 #include <vector>
 
-#include "../../include/m2s.h"
+#include "m2s_host.h"
 
 namespace m2s {
 static thread_local std::string g_error;
 void set_error(const std::string& msg) { g_error = msg; }
 }  // namespace m2s
-
-#define M2S_EXPORT extern "C" __attribute__((visibility("default")))
 
 M2S_EXPORT const char* m2s_last_error(void) { return m2s::g_error.c_str(); }
 
@@ -90,22 +88,6 @@ void encode_row(uint32_t format, const float* r, float mult, uint8_t* dst) {
     }
 }
 }  // namespace
-
-namespace m2s {
-// writes header + already-encoded rows
-m2s_status write_ply_rows(const char* path, uint32_t format, const void* rows, uint64_t count) {
-    FILE* f = std::fopen(path, "wb");
-    if (!f) { set_error(std::string("cannot open ") + path); return M2S_E_IO; }
-    char hdr[4096];
-    const size_t n = m2s_ply_header(format, count, hdr, sizeof(hdr));
-    bool ok = std::fwrite(hdr, 1, n, f) == n;
-    const size_t body = (size_t)count * row_bytes(format);
-    if (ok && body) ok = std::fwrite(rows, 1, body, f) == body;
-    ok = (std::fclose(f) == 0) && ok;
-    if (!ok) { set_error(std::string("short write to ") + path); return M2S_E_IO; }
-    return M2S_OK;
-}
-}  // namespace m2s
 
 M2S_EXPORT m2s_status m2s_ply_write(const char* path, const void* h_ref96, uint64_t count, uint32_t format, float mult) {
     if (!path || (count && !h_ref96)) { m2s::set_error("m2s_ply_write: NULL argument"); return M2S_E_INVALID; }

@@ -1850,7 +1850,7 @@ __global__ void ply_rows_kernel(const float4* __restrict__ rec, unsigned long lo
 }
 
 // ------------------------------------------------------------------------------------------
-// launch wrappers used by m2s_api.cu
+// launch wrappers used by the host code (m2s_scene.cu, m2s_convert.cu), declared in m2s_device.cuh
 // ------------------------------------------------------------------------------------------
 static int raster_kind(int layout) { return layout == 0 ? 0 : (layout == 1 ? 1 : 2); }
 static_assert(sizeof(WarpBlock<0>) * RCfg<0>::kWarps + kTableSmemBytes + sizeof(CtaQueue) <= 232448 &&

@@ -1,5 +1,5 @@
 // m2s_light.cuh — arguments and scratch layout of the viewer's shadow pass and deferred lighting (m2s_light.cu), shared
-// with the C-ABI host code (m2s_api.cu).
+// with the C-ABI host code (m2s_viewer.cu).
 #pragma once
 #include <cstddef>
 #include <cstdint>

@@ -1,4 +1,4 @@
-// m2s_prepass.cuh — arguments of the viewer prepass kernel (m2s_prepass.cu), filled by the C-ABI host code (m2s_api.cu).
+// m2s_prepass.cuh — arguments of the viewer prepass kernel (m2s_prepass.cu), filled by the C-ABI host code (m2s_viewer.cu).
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>

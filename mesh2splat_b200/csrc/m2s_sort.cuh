@@ -1,5 +1,5 @@
 // m2s_sort.cuh — arguments and scratch layout of the viewer's depth sort (m2s_sort.cu), shared with the C-ABI host code
-// (m2s_api.cu).
+// (m2s_viewer.cu).
 #pragma once
 #include <cstddef>
 #include <cstdint>

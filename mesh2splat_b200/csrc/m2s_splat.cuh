@@ -1,5 +1,5 @@
 // m2s_splat.cuh — arguments and scratch layout of the viewer's splat draw (m2s_splat.cu), shared with the C-ABI host code
-// (m2s_api.cu).
+// (m2s_viewer.cu).
 #pragma once
 #include <cstddef>
 #include <cstdint>
