@@ -34,6 +34,9 @@
  *     (src/renderer/renderPasses/GaussianRelightingPass.cpp:42-150)
  *   SceneManager::loadModel -> execute -> exportPly             m2s_convert_file
  *     (src/utils/SceneManager.hpp:18-20)
+ *   SceneManager::loadPly + parsers::loadPlyFile                 m2s_ply_parse_header, m2s_ply_decode_enqueue,
+ *     (src/utils/SceneManager.cpp:37-47,                         m2s_ply_read; M2S_VIEW_PLY / M2S_VIEW_PLY_PBR
+ *      src/parsers/parsers.cpp:516-629)                          as the viewer passes' input
  *
  * Plain pointers and sizes only; no C++/torch types.  All functions return an
  * m2s_status; m2s_last_error() gives the thread-local message of the last
@@ -252,6 +255,67 @@ m2s_status m2s_ply_encode(m2s_ctx* ctx, const void* d_ref96, uint64_t count, uin
 m2s_status m2s_ply_write(const char* path, const void* h_ref96, uint64_t count, uint32_t format,
                          float scale_multiplier);
 
+/* ---- inputs of the viewer: replaces SceneManager::loadPly / parsers::loadPlyFile (SURVEY 8 f-10) --------------------
+ * A .ply file -> REF96 records exactly as loadPlyFile fills GaussianDataSSBO (parsers.cpp:577-622):
+ *   position  (x, y, z, 1)
+ *   color     (f_dc * SH_COEFF0 + 0.5f per channel: two fp32 roundings, no FMA,  1 / (1 + (double)expf(-opacity)) in fp64)
+ *   scale     (expf(scale_0), expf(scale_1), expf(scale_2), 1)
+ *   normal    (nx, ny, nz, 0) with has_pbr, else 0
+ *   rotation  glm::normalize(glm::quat(rot_0, rot_1, rot_2, rot_3)) stored (w, x, y, z): each component times
+ *             1 / sqrt((r0 r0 + r1 r1) + (r2 r2 + r3 r3)); (1, 0, 0, 0) when that length is <= 0; NaN propagates
+ *   pbr       (metallicFactor, roughnessFactor, 0, 0) with has_pbr, else 0
+ * expf is evaluated on the device with glibc's own algorithm (the table-driven fp64 expf glibc selects on x86-64 with FMA),
+ * bit-identical to it on all 2^32 inputs; against a glibc that uses its non-FMA variant scale.xyz and color.a may differ
+ * by 1 ulp, every other field is bit-exact.  Denormals are kept.  SH rest coefficients are skipped, as in the reference.
+ * Property rules (happly): the properties are found by name in the first element "vertex" (order and extra properties do
+ * not matter); x y z f_dc_0..2 opacity scale_0..2 rot_0..3 are required; every property read must be float / float32
+ * (happly does not narrow a double); has_pbr = nx ny nz metallicFactor roughnessFactor all present, and 1 for a file of 0
+ * vertices whatever its properties (the reference compares vector sizes: 0 == 0).
+ * Deviations from the reference, each M2S_E_FORMAT with a message naming the cause (the reference prints the error, keeps
+ * the previous gaussians and loadPly still returns true):
+ *   - ascii and binary_big_endian bodies (happly reads them; 3DGS files are binary_little_endian);
+ *   - an element with a list property before "vertex" (fixed-size elements before it are skipped by arithmetic; elements
+ *     after it are ignored);
+ *   - a header without end_header, or a body shorter than body_offset + vertex_count * row_stride (checked with
+ *     overflow-safe arithmetic before anything is allocated; happly reads past the end of the file and keeps garbage);
+ *   - vertex rows longer than M2S_PLY_MAX_STRIDE bytes, or a list property in "vertex";
+ *   - the compressed format (2) of m2s_ply_write is rejected because f_dc_0 is missing, as the reference rejects it. */
+#define M2S_PLY_PROPS 19
+enum {   /* index into m2s_ply_info.offset */
+    M2S_PLY_X = 0, M2S_PLY_Y, M2S_PLY_Z, M2S_PLY_NX, M2S_PLY_NY, M2S_PLY_NZ, M2S_PLY_F_DC_0, M2S_PLY_F_DC_1, M2S_PLY_F_DC_2,
+    M2S_PLY_METALLIC, M2S_PLY_ROUGHNESS, M2S_PLY_OPACITY, M2S_PLY_SCALE_0, M2S_PLY_SCALE_1, M2S_PLY_SCALE_2,
+    M2S_PLY_ROT_0, M2S_PLY_ROT_1, M2S_PLY_ROT_2, M2S_PLY_ROT_3
+};
+#define M2S_PLY_MAX_STRIDE 4096u   /* bytes per vertex row the decoder takes */
+typedef struct m2s_ply_info {
+    uint64_t vertex_count;
+    uint64_t body_offset;            /* file offset of vertex row 0 */
+    uint32_t row_stride;             /* bytes per vertex row: 1..M2S_PLY_MAX_STRIDE */
+    uint32_t has_pbr;                /* loadPlyFile's hasPbr */
+    int32_t offset[M2S_PLY_PROPS];   /* byte offset in the row of x y z nx ny nz f_dc_0..2 metallicFactor roughnessFactor
+                                        opacity scale_0..2 rot_0..3; -1 = absent */
+} m2s_ply_info;
+/* Host only.  bytes/size: the first `size` bytes of the file (the whole file, or any prefix that holds the header);
+ * file_size: the size of the whole file.  Never reads outside [bytes, bytes + size). */
+m2s_status m2s_ply_parse_header(const void* bytes, size_t size, uint64_t file_size, m2s_ply_info* info);
+/* Enqueue-only.  d_rows: `count` rows of info->row_stride bytes (row 0 = the file's vertex row 0 of this block; no
+ * alignment required); d_ref96: count x 96 B, 16-byte aligned.  stream NULL = the context stream. */
+m2s_status m2s_ply_decode_enqueue(m2s_ctx* ctx, const m2s_ply_info* info, const void* d_rows, uint64_t count,
+                                  void* d_ref96, void* stream);
+/* The whole load, synchronous on the context stream: header parsed on the host, the body read in row-aligned blocks
+ * into two pinned buffers, each block copied to a two-slot device staging area and decoded into d_ref96 + first_row * 96
+ * while the next block is read from the file.  d_ref96 == NULL: only fills *info (the probe that sizes the buffer).
+ * capacity < vertex_count: M2S_E_CAPACITY, *info filled, nothing written. */
+m2s_status m2s_ply_read(m2s_ctx* ctx, const char* path, void* d_ref96, uint64_t capacity, m2s_ply_info* info);
+/* Payload bytes m2s_ply_read copied host -> device on this context so far (accounting for benchmarks). */
+uint64_t m2s_ply_h2d_bytes(const m2s_ctx* ctx);
+/* `layout` values of m2s_prepass* and m2s_shadow_map* for REF96 records as loadPlyFile fills them (not conversion
+ * layouts: m2s_record_stride and m2s_convert* do not take them).  The reference's u_format 1: scale multiplier 1, no mesh
+ * depth test (m2s_prepass_mesh_depth gives m2s_prepass's output); the normal through the normal matrix with u_plyHasPbr 1,
+ * the shortest axis with 0 (gaussianSplattingPrepassCS.glsl:93-130, gaussianPointShadowMappingCS.glsl:96). */
+#define M2S_VIEW_PLY     16u   /* u_format 1, u_plyHasPbr 0 */
+#define M2S_VIEW_PLY_PBR 17u   /* u_format 1, u_plyHasPbr 1 */
+
 /* ---- file-level surface: loadModel -> execute -> exportPly --------------------------------- */
 /* .glb -> host scene: SceneManager::parseGltfFile + setupMeshBuffers (bbox rule) + loadTextures
  * (src/utils/SceneManager.cpp:195-459,468-649): scene-graph world transforms, de-indexing, flat
@@ -282,6 +346,7 @@ m2s_status m2s_convert_file(m2s_ctx* ctx, const char* glb_path, uint32_t resolut
  *   M2S_LAYOUT_PACKED56  a standard 3DGS gaussian as the reference loads it from a .ply without PBR values, u_format 1
  *                        (scale = exp(log_scale), colour = SH0 * C0 + 0.5, alpha = sigmoid(opacity), normal = the
  *                        shortest axis, pbr = 0)
+ *   M2S_VIEW_PLY(_PBR)   REF96 records as m2s_ply_read loads them, u_format 1 (u_plyHasPbr 0 / 1; see above)
  * The mesh depth test (u_depthTestMesh 1) is m2s_prepass_mesh_depth below.  Not reproduced: render mode 3 (debug colours
  * from the invocation id).  Output order is unspecified, as in the reference (atomic arrival order). */
 typedef struct m2s_prepass_params {
@@ -292,7 +357,7 @@ typedef struct m2s_prepass_params {
     float near_far[2];
     float std_dev;             /* gaussianStd / resolutionTarget (GaussiansPrepass.cpp:18) */
     uint32_t render_mode;      /* 0 (or 6) colour, 1 depth, 2 normal */
-    uint32_t layout;           /* M2S_LAYOUT_REF96 or M2S_LAYOUT_PACKED56 */
+    uint32_t layout;           /* M2S_LAYOUT_REF96, M2S_LAYOUT_PACKED56, M2S_VIEW_PLY or M2S_VIEW_PLY_PBR */
     uint32_t reserved;
 } m2s_prepass_params;
 #define M2S_QUAD_BYTES 96u
@@ -335,8 +400,8 @@ m2s_status m2s_mesh_depth(m2s_ctx* ctx, const m2s_dscene* scene, const m2s_mesh_
                           uint64_t* pairs);
 /* The prepass with the mesh depth test (gaussianSplattingPrepassCS.glsl:78-91, u_depthTestMesh 1): a REF96 gaussian that
  * passes the frustum cull and has color.a > 0.95f is dropped when (pos2d.z / pos2d.w) 0.5 + 0.5 > depth + 0.00002f,
- * depth = the map's texel at uv = (pos2d.xy / pos2d.w) 0.5 + 0.5, sampled NEAREST with CLAMP_TO_EDGE.  PACKED56 input
- * (u_format 1) never reads the map: the output equals m2s_prepass's.  d_mesh_depth: depth_width x depth_height floats
+ * depth = the map's texel at uv = (pos2d.xy / pos2d.w) 0.5 + 0.5, sampled NEAREST with CLAMP_TO_EDGE.  PACKED56 and
+ * M2S_VIEW_PLY* input (u_format 1) never reads the map: the output equals m2s_prepass's.  d_mesh_depth: depth_width x depth_height floats
  * as m2s_mesh_depth writes them (1..4096 each).  Everything else as m2s_prepass_enqueue / m2s_prepass. */
 m2s_status m2s_prepass_mesh_depth_enqueue(m2s_ctx* ctx, const void* d_records, uint64_t count, const uint64_t* d_count,
                                           const m2s_prepass_params* params, const float* d_mesh_depth, uint32_t depth_width,
@@ -407,7 +472,7 @@ typedef struct m2s_shadow_params {
     float near_far[2];
     float resolution[2];       /* renderContext.rendererResolution (not the face size: sic, the reference's u_resolution) */
     float std_dev;             /* gaussianStd / resolutionTarget */
-    uint32_t layout;           /* M2S_LAYOUT_REF96 or M2S_LAYOUT_PACKED56 */
+    uint32_t layout;           /* M2S_LAYOUT_REF96, M2S_LAYOUT_PACKED56, M2S_VIEW_PLY or M2S_VIEW_PLY_PBR */
     uint32_t size;             /* face size S: 1..1024 (the reference uses 1024) */
 } m2s_shadow_params;
 #define M2S_LIGHT_RECORD_BYTES 32u

@@ -20,6 +20,22 @@ STRIDES = {LAYOUT_REF96: 96, LAYOUT_PACKED56: 56, LAYOUT_PLY_STANDARD: 248, LAYO
            LAYOUT_PLY_COMPRESSED: 48}
 # which .ply format (savePlyVector FORMAT, parsers.cpp:631-651) a row layout corresponds to
 PLY_FORMAT_LAYOUT = {0: LAYOUT_PLY_STANDARD, 1: LAYOUT_PLY_PBR, 2: LAYOUT_PLY_COMPRESSED}
+# viewer-pass input: REF96 records as m2s_ply_read loads them (u_format 1, u_plyHasPbr 0 / 1)
+VIEW_PLY, VIEW_PLY_PBR = 16, 17
+# m2s_ply_info.offset: the properties loadPlyFile reads, in this order
+PLY_PROPS = ("x", "y", "z", "nx", "ny", "nz", "f_dc_0", "f_dc_1", "f_dc_2", "metallicFactor", "roughnessFactor", "opacity",
+             "scale_0", "scale_1", "scale_2", "rot_0", "rot_1", "rot_2", "rot_3")
+PLY_MAX_STRIDE = 4096
+
+
+class m2s_ply_info(C.Structure):
+    """include/m2s.h: what m2s_ply_parse_header reads from a .ply header."""
+    _fields_ = [("vertex_count", C.c_uint64), ("body_offset", C.c_uint64), ("row_stride", C.c_uint32), ("has_pbr", C.c_uint32),
+                ("offset", C.c_int32 * len(PLY_PROPS))]
+
+    def offsets(self) -> dict:
+        """{property name: byte offset in the row} of the properties present."""
+        return {n: int(o) for n, o in zip(PLY_PROPS, self.offset) if o >= 0}
 
 
 class m2s_texture(C.Structure):

@@ -23,6 +23,7 @@ SYMBOLS = [
     "m2s_splat_draw", "m2s_splat_draw_enqueue", "m2s_shadow_map", "m2s_shadow_map_enqueue",
     "m2s_deferred_light", "m2s_deferred_light_enqueue", "m2s_mesh_depth", "m2s_mesh_depth_enqueue",
     "m2s_prepass_mesh_depth", "m2s_prepass_mesh_depth_enqueue",
+    "m2s_ply_parse_header", "m2s_ply_decode_enqueue", "m2s_ply_read", "m2s_ply_h2d_bytes",
 ]
 
 
@@ -133,6 +134,14 @@ def lib() -> C.CDLL:
     L.m2s_prepass_mesh_depth_enqueue.argtypes = [vp, vp, u64, vp, C.POINTER(_abi.m2s_prepass_params), vp, u32, u32, vp, vp, vp, vp]
     L.m2s_prepass_mesh_depth.restype = i32
     L.m2s_prepass_mesh_depth.argtypes = [vp, vp, u64, C.POINTER(_abi.m2s_prepass_params), vp, u32, u32, vp, vp, C.POINTER(u32)]
+    L.m2s_ply_parse_header.restype = i32
+    L.m2s_ply_parse_header.argtypes = [vp, C.c_size_t, u64, C.POINTER(_abi.m2s_ply_info)]
+    L.m2s_ply_decode_enqueue.restype = i32
+    L.m2s_ply_decode_enqueue.argtypes = [vp, C.POINTER(_abi.m2s_ply_info), vp, u64, vp, vp]
+    L.m2s_ply_read.restype = i32
+    L.m2s_ply_read.argtypes = [vp, C.c_char_p, vp, u64, C.POINTER(_abi.m2s_ply_info)]
+    L.m2s_ply_h2d_bytes.restype = u64
+    L.m2s_ply_h2d_bytes.argtypes = [vp]
     _lib = L
     return L
 

@@ -6,6 +6,7 @@ src/renderer/RenderContext.hpp:28-124):
     SceneManager::loadModel(path, parentFolder)      -> SceneManager.loadModel / .setScene
     ConversionPass::execute(RenderContext&)          -> ConversionPass.execute(renderContext)
     SceneManager::exportPly(outPath, exportFormat)   -> SceneManager.exportPly
+    SceneManager::loadPly(filePath)                  -> SceneManager.loadPly (parsers::loadPlyFile on the GPU)
 
 plus the plain functional form `Context.convert(...)`.  torch is used only to own device buffers
 (torch.empty(..., device="cuda")) and pinned host buffers; every computation is a call into
@@ -393,6 +394,38 @@ class Context:
         torch.cuda.synchronize(ref96.device)
         return rows[: count * _abi.STRIDES[layout]]
 
+    # ---- .ply input (loadPlyFile) ----
+    def ply_decode(self, rows, info: _abi.m2s_ply_info, out=None, count: int | None = None):
+        """Decode .ply vertex rows already on the device (a torch uint8 tensor of count * info.row_stride bytes, any
+        alignment) into REF96 records (m2s_ply_decode_enqueue on torch's current stream).  Returns the records as a torch
+        uint8 device tensor of count * 96 bytes (out: optional caller-owned tensor of at least that size)."""
+        torch = _torch()
+        if count is None:
+            count = rows.numel() // info.row_stride
+        if out is None:
+            out = torch.empty(max(1, count) * 96, dtype=torch.uint8, device=rows.device)
+        check(lib().m2s_ply_decode_enqueue(self.handle, C.byref(info), rows.data_ptr(), count, out.data_ptr(),
+                                           torch.cuda.current_stream(rows.device).cuda_stream))
+        torch.cuda.synchronize(rows.device)
+        return out[: count * 96]
+
+    def ply_read(self, path: str, out=None):
+        """SceneManager::loadPly's loadPlyFile on the GPU (m2s_ply_read): returns (records, count, has_pbr), records a
+        torch uint8 device tensor of count * 96 bytes (REF96).  out: optional caller-owned device tensor; M2SError with
+        M2S_E_CAPACITY when it holds fewer than count records."""
+        torch = _torch()
+        info = _abi.m2s_ply_info()
+        check(lib().m2s_ply_read(self.handle, path.encode(), None, 0, C.byref(info)))
+        n = int(info.vertex_count)
+        if out is None:
+            out = torch.empty(max(1, n) * 96, dtype=torch.uint8, device=torch.device("cuda", self.device))
+        torch.cuda.synchronize(out.device)   # the buffer torch hands out is idle before the context stream writes it
+        check(lib().m2s_ply_read(self.handle, path.encode(), out.data_ptr(), out.numel() // 96, C.byref(info)))
+        return out[: n * 96], n, bool(info.has_pbr)
+
+    def ply_h2d_bytes(self) -> int:
+        return int(lib().m2s_ply_h2d_bytes(self.handle))
+
     def convert_file(self, glb_path: str, resolution: int, ply_path: str, gaussian_std: float = 0.65, fmt: int = 0):
         res = _abi.m2s_result()
         check(lib().m2s_convert_file(self.handle, glb_path.encode(), resolution, gaussian_std, fmt, ply_path.encode(),
@@ -412,6 +445,23 @@ def ply_header(fmt: int, count: int) -> bytes:
     buf = C.create_string_buffer(8192)
     n = lib().m2s_ply_header(fmt, count, buf, 8192)
     return buf.raw[:n]
+
+
+def ply_parse_header(data: bytes, file_size: int | None = None) -> _abi.m2s_ply_info:
+    """m2s_ply_parse_header on the first bytes of a .ply file (file_size: the whole file's size, default len(data)).
+    Raises M2SError (M2S_E_FORMAT with the cause) for a file the loader does not take."""
+    info = _abi.m2s_ply_info()
+    buf = C.create_string_buffer(bytes(data), len(data))
+    check(lib().m2s_ply_parse_header(buf, len(data), len(data) if file_size is None else int(file_size), C.byref(info)))
+    return info
+
+
+def ply_parse_file(path: str) -> _abi.m2s_ply_info:
+    """ply_parse_header on a file: its first 1 MB and its size."""
+    import os
+    with open(path, "rb") as f:
+        head = f.read(1 << 20)
+    return ply_parse_header(head, os.path.getsize(path))
 
 
 def ply_write(path: str, ref96: np.ndarray, fmt: int, scale_multiplier: float) -> None:
@@ -435,6 +485,14 @@ class RenderContext:
         self.gaussianBuffer = None           # SSBO: torch.uint8 device tensor of GaussianDataSSBO records
         self.numberOfGaussians = 0           # may exceed the buffer capacity (ConversionPass.cpp:56-59)
         self.lastResult: ConvertOutput | None = None
+        self.format = 0                      # u_format: 0 the conversion's records, 1 a loaded .ply (RenderContext.hpp)
+        self.plyHasPbr = False               # format 1: the .ply carries normals and metallic / roughness
+
+    def viewLayout(self) -> int:
+        """The `layout` the viewer passes (prepass, shadow_map) take for gaussianBuffer."""
+        if self.format == 1:
+            return _abi.VIEW_PLY_PBR if self.plyHasPbr else _abi.VIEW_PLY
+        return _abi.LAYOUT_REF96
 
 
 class SceneManager:
@@ -457,6 +515,20 @@ class SceneManager:
         except (OSError, ValueError) as e:  # the reference prints and returns false
             print(f"Failed to parse GLTF file: {filePath}: {e}")
             return False
+
+    def loadPly(self, filePath: str) -> bool:
+        """SceneManager::loadPly (SceneManager.cpp:37-47) + parsers::loadPlyFile: the file's gaussians become
+        gaussianBuffer (REF96 on the device), format 1, plyHasPbr from the file.  Deviation: a file the loader does not
+        take returns False and leaves the previous gaussians in place (the reference prints the error and returns true)."""
+        rc = self.renderContext
+        try:
+            ply_parse_file(filePath)   # header and size checked on the host before anything reaches the device
+            records, n, has_pbr = rc.ctx.ply_read(filePath)
+        except (OSError, M2SError) as e:
+            print(f"Error loading PLY file: {filePath}: {e}")
+            return False
+        rc.gaussianBuffer, rc.numberOfGaussians, rc.format, rc.plyHasPbr = records, n, 1, has_pbr
+        return True
 
     def exportPly(self, outputFile: str, exportFormat: int = 0) -> None:
         """SceneManager::exportPly (SceneManager.cpp:651-678): read back, scale by std/R, write."""
@@ -491,4 +563,4 @@ class ConversionPass:
 
 
 __all__ = ["Context", "DeviceScene", "ConvertOutput", "RenderContext", "SceneManager", "ConversionPass", "depth_sort_tile",
-           "ply_header", "ply_write", "M2SError"]
+           "ply_header", "ply_write", "ply_parse_header", "ply_parse_file", "M2SError"]

@@ -92,11 +92,13 @@ struct m2s_ctx {
     m2s::Scratch sort;                       // depth sort: control words, alternate key and value buffers (SortLayout, m2s_sort.cuh)
     m2s::BinScratch splat_bins, shadow_bins, depth_bins;  // the binned passes: splat draw, cube raster, mesh depth pre-pass
     m2s::Scratch light_quads;                // shadow pass: light records when the caller passes none
+    m2s::Scratch ply_rows;                   // .ply reader: two slots of one block of raw vertex rows (m2s_ply_read.cu)
     // every Scratch above (m2s_ctx_destroy frees them): a member added above is added here too
     std::vector<m2s::Scratch*> all_scratch() {
-        return {&out, &keys, &trifrag, &items, &sort, &light_quads, &splat_bins.bins, &splat_bins.pairs, &shadow_bins.bins,
+        return {&out, &keys, &trifrag, &items, &sort, &light_quads, &ply_rows, &splat_bins.bins, &splat_bins.pairs, &shadow_bins.bins,
                 &shadow_bins.pairs, &depth_bins.bins, &depth_bins.pairs};
     }
+    uint64_t ply_h2d = 0;                    // row bytes m2s_ply_read copied host -> device
 };
 
 struct m2s_dscene {

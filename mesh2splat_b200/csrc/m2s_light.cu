@@ -84,7 +84,7 @@ __global__ void __launch_bounds__(kLightPrepassThreads) light_prepass_kernel(con
     const float clip = ml(1.05f, c3);   // :89-94
     bool alive = !(c2 < -clip || c0 < -clip || c0 > clip || c1 < -clip || c1 > clip);
     if (alive) {
-        const float mult = a.layout == 0 ? a.std_dev : 1.0f;   // :96-98
+        const float mult = a.fmt == 0 ? a.std_dev : 1.0f;      // :96-98
         const float s[3] = {ml(ml(sx, mult), a.mscale2[0]), ml(ml(sy, mult), a.mscale2[1]), ml(ml(sz, mult), a.mscale2[2])};
         // castQuatToMat3 (common.glsl:22-48): the three "rows" are the columns; quat = (w, x, y, z) in (x, y, z, w)
         const float rot0[9] = {sb(1.f, ml(2.f, ad(ml(qz, qz), ml(qw, qw)))), ml(2.f, sb(ml(qy, qz), ml(qx, qw))), ml(2.f, ad(ml(qy, qw), ml(qx, qz))),

@@ -29,7 +29,8 @@ struct ShadowArgs {
     const unsigned char* records;   // count x 96 B (REF96) or 56 B (PACKED56)
     unsigned long long count;
     const unsigned long long* d_count;   // optional: n = min(count, *d_count)
-    uint32_t layout;                // 0 REF96, 1 PACKED56
+    uint32_t layout;                // record layout: 0 REF96, 1 PACKED56
+    uint32_t fmt;                   // the reference's u_format: 0 conversion, 1 PACKED56 or a loaded .ply
     float M[16];                    // u_modelToWorld
     float V[6][16];                 // u_worldToViews: glm::lookAt per face
     float P[16];                    // u_viewToClip: glm::perspective(90 deg, 1, near, far)

@@ -6,7 +6,8 @@
 // Shape: a streaming kernel, HBM-bound (96 or 56 B in, 100 B out per survivor, ~250 flops).  One thread per gaussian; the
 // survivors of a warp are appended with ONE atomicAdd (the reference: one atomicCounterIncrement per gaussian), staged in
 // shared memory and written as one contiguous span with 16-byte stores.  Consumes the conversion's REF96 records
-// (u_format 0) or its PACKED56 records (a standard 3DGS gaussian: u_format 1 without PBR values).
+// (u_format 0), its PACKED56 records (a standard 3DGS gaussian: u_format 1 without PBR values), or the REF96 records
+// m2s_ply_read loads from a .ply (u_format 1, u_plyHasPbr 0 or 1): the record layout and u_format are separate arguments.
 #include "m2s_prepass.cuh"
 
 namespace m2s {
@@ -111,12 +112,12 @@ __device__ __forceinline__ void prepass_body(const PrepassArgs& a, const float* 
         c3 = a.P[3] * vs0 + a.P[7] * vs1 + a.P[11] * vs2 + a.P[15] * vs3;
         const float clip = 1.05f * c3;                                   // :72-76
         if (c2 < -clip || c0 < -clip || c0 > clip || c1 < -clip || c1 > clip) alive = false;
-        if (kDepth && alive && a.layout == 0 && ca > 0.95f && prepass_behind_mesh(a, map, dw, dh, px, py, pz)) alive = false;
+        if (kDepth && alive && a.fmt == 0 && ca > 0.95f && prepass_behind_mesh(a, map, dw, dh, px, py, pz)) alive = false;
     }
     float4 q0, q1, q2, q3, q4, q5;
     q0 = q1 = q2 = q3 = q4 = q5 = make_float4(0.f, 0.f, 0.f, 0.f);
     if (alive) {
-        const bool fmt0 = a.layout == 0;
+        const bool fmt0 = a.fmt == 0;
         const float mult = fmt0 ? a.std_dev : 1.0f;                     // :95-97
         const float s0 = sx * mult * a.mscale2[0], s1 = sy * mult * a.mscale2[1], s2 = sz * mult * a.mscale2[2];
         // castQuatToMat3 (common.glsl:22-48): the three "rows" are the COLUMNS of the matrix; quat = (w, x, y, z)
@@ -134,7 +135,7 @@ __device__ __forceinline__ void prepass_body(const PrepassArgs& a, const float* 
             for (int k = 0; k < 3; ++k) mmT[c * 3 + k] = mm[k * 3 + c];
         m3mul(mmT, mm, cov3d);
         float n0 = 1.f, n1 = 0.f, n2 = 0.f, n3 = 0.f;
-        if (fmt0) {                                                      // :117-121 normal through the normal matrix
+        if (fmt0 || a.ply_has_pbr) {                                     // :117-121 normal through the normal matrix
             n0 = (a.Nmat[0] * nx + a.Nmat[4] * ny + a.Nmat[8] * nz + a.Nmat[12]) * 0.5f + 0.5f;
             n1 = (a.Nmat[1] * nx + a.Nmat[5] * ny + a.Nmat[9] * nz + a.Nmat[13]) * 0.5f + 0.5f;
             n2 = (a.Nmat[2] * nx + a.Nmat[6] * ny + a.Nmat[10] * nz + a.Nmat[14]) * 0.5f + 0.5f;

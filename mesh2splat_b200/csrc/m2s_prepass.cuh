@@ -12,7 +12,9 @@ struct PrepassArgs {
     float mscale2[3];              // (|M[0]|^2, |M[0]|^2, |M[1]|^2)  (sic, :96)
     float res[2], near_far[2];
     float std_dev;
-    uint32_t render_mode, layout;
+    uint32_t render_mode;
+    uint32_t layout;               // record layout: 0 REF96 (96 B), 1 PACKED56 (56 B)
+    uint32_t fmt, ply_has_pbr;     // the reference's u_format (0 conversion, 1 loaded .ply) and u_plyHasPbr
     unsigned long long count;
     const unsigned long long* d_count;
     const unsigned char* records;

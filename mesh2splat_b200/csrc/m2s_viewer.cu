@@ -49,12 +49,25 @@ static bool invert4(const double m[16], double inv[16]) {   // column-major, cof
     return true;
 }
 
+// the `layout` of m2s_prepass* / m2s_shadow_map*: the record layout and the reference's u_format / u_plyHasPbr it stands for
+struct ViewInput { uint32_t layout, fmt, ply_has_pbr; };
+static bool view_input(uint32_t layout, ViewInput& v) {
+    switch (layout) {
+        case M2S_LAYOUT_REF96: v = {0u, 0u, 0u}; return true;     // a conversion's records
+        case M2S_LAYOUT_PACKED56: v = {1u, 1u, 0u}; return true;  // a standard 3DGS gaussian, u_format 1 without PBR values
+        case M2S_VIEW_PLY: v = {0u, 1u, 0u}; return true;         // REF96 records as m2s_ply_read loads them
+        case M2S_VIEW_PLY_PBR: v = {0u, 1u, 1u}; return true;
+        default: return false;
+    }
+}
+
 // d_valid: the enqueue forms' counter (the synchronous forms use the context's, never NULL)
 static m2s_status prepass_check(const m2s_ctx* ctx, const void* d_records, uint64_t count, const m2s_prepass_params* p, const void* d_quads,
                                 const float* d_depths, bool has_valid) {
     const char* fn = "m2s_prepass";
     if (!ctx || !p || !has_valid || (count && (!d_records || !d_quads || !d_depths))) return invalid(fn, "NULL argument");
-    if (p->layout != M2S_LAYOUT_REF96 && p->layout != M2S_LAYOUT_PACKED56) return invalid(fn, "layouts REF96 and PACKED56 only");
+    ViewInput v;
+    if (!view_input(p->layout, v)) return invalid(fn, "layouts REF96, PACKED56, VIEW_PLY and VIEW_PLY_PBR only");
     if (p->render_mode == 3 || (p->render_mode > 2 && p->render_mode != 6)) return invalid(fn, "render modes 0 (6), 1 and 2 only");
     if (count >= (1ull << 32)) return invalid(fn, "too many gaussians (< 2^32 supported)");
     return aligned_ok(fn, "the record and quad buffers must be 16-byte aligned", {{d_quads, 16}, {d_records, 16}}) ? M2S_OK : M2S_E_INVALID;
@@ -81,7 +94,9 @@ static m2s_status prepass_fill(const void* d_records, uint64_t count, const uint
     const double l0 = M[0] * M[0] + M[1] * M[1] + M[2] * M[2] + M[3] * M[3], l1 = M[4] * M[4] + M[5] * M[5] + M[6] * M[6] + M[7] * M[7];
     a.mscale2[0] = (float)l0; a.mscale2[1] = (float)l0; a.mscale2[2] = (float)l1;   // (|M[0]|, |M[0]|, |M[1]|) squared — sic (:96)
     a.res[0] = p->resolution[0]; a.res[1] = p->resolution[1]; a.near_far[0] = p->near_far[0]; a.near_far[1] = p->near_far[1];
-    a.std_dev = p->std_dev; a.render_mode = p->render_mode; a.layout = p->layout == M2S_LAYOUT_REF96 ? 0u : 1u;
+    ViewInput v;
+    view_input(p->layout, v);   // checked by prepass_check
+    a.std_dev = p->std_dev; a.render_mode = p->render_mode; a.layout = v.layout; a.fmt = v.fmt; a.ply_has_pbr = v.ply_has_pbr;
     a.count = count; a.d_count = (const unsigned long long*)d_count;
     a.records = (const unsigned char*)d_records; a.quads = (float4*)d_quads; a.depths = d_depths; a.valid = d_valid;
     return M2S_OK;
@@ -344,7 +359,10 @@ static void shadow_uniforms(const m2s_shadow_params* p, ShadowArgs& a) {
     a.res[0] = p->resolution[0]; a.res[1] = p->resolution[1];
     a.near_far[0] = n; a.near_far[1] = fa;
     a.std_dev = p->std_dev;
-    a.layout = p->layout == M2S_LAYOUT_REF96 ? 0u : 1u;
+    ViewInput v;
+    view_input(p->layout, v);   // checked by shadow_pass
+    a.layout = v.layout;
+    a.fmt = v.fmt;
     a.size = p->size;
 }
 
@@ -356,7 +374,8 @@ static m2s_status shadow_pass(m2s_ctx* ctx, const void* d_records, uint64_t coun
     const char* fn = "m2s_shadow_map";
     if (!ctx || !p || !d_cube) return invalid(fn, "NULL argument");
     if (count && !d_records) return invalid(fn, "NULL records");
-    if (p->layout != M2S_LAYOUT_REF96 && p->layout != M2S_LAYOUT_PACKED56) return invalid(fn, "layouts REF96 and PACKED56 only");
+    ViewInput v;
+    if (!view_input(p->layout, v)) return invalid(fn, "layouts REF96, PACKED56, VIEW_PLY and VIEW_PLY_PBR only");
     if (!aligned_ok(fn, "the record and light-record buffers must be 16-byte aligned, the cube 4-byte aligned",
                     {{d_records, 16}, {d_light_quads, 16}, {d_cube, 4}}))
         return M2S_E_INVALID;
