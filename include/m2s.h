@@ -265,8 +265,10 @@ m2s_status m2s_ply_write(const char* path, const void* h_ref96, uint64_t count, 
  *             1 / sqrt((r0 r0 + r1 r1) + (r2 r2 + r3 r3)); (1, 0, 0, 0) when that length is <= 0; NaN propagates
  *   pbr       (metallicFactor, roughnessFactor, 0, 0) with has_pbr, else 0
  * expf is evaluated on the device with glibc's own algorithm (the table-driven fp64 expf glibc selects on x86-64 with FMA),
- * bit-identical to it on all 2^32 inputs; against a glibc that uses its non-FMA variant scale.xyz and color.a may differ
- * by 1 ulp, every other field is bit-exact.  Denormals are kept.  SH rest coefficients are skipped, as in the reference.
+ * bit-identical to it on all 2^32 inputs (tests/test_gpu_codec.py); against a glibc that uses its non-FMA variant
+ * scale.xyz and color.a may differ by 1 ulp, every other field is bit-exact.  The writers' encodings are exact the same
+ * way: SH0 = (c - 0.5f) / SH_COEFF0 (the IEEE quotient), the opacity logit and the log-scale with glibc's logf, in the
+ * conversion's .ply and PACKED56 layouts, m2s_ply_encode and m2s_convert_file.  Denormals are kept.  SH rest coefficients are skipped, as in the reference.
  * Property rules (happly): the properties are found by name in the first element "vertex" (order and extra properties do
  * not matter); x y z f_dc_0..2 opacity scale_0..2 rot_0..3 are required; every property read must be float / float32
  * (happly does not narrow a double); has_pbr = nx ny nz metallicFactor roughnessFactor all present, and 1 for a file of 0

@@ -26,6 +26,8 @@ VIEW_PLY, VIEW_PLY_PBR = 16, 17
 PLY_PROPS = ("x", "y", "z", "nx", "ny", "nz", "f_dc_0", "f_dc_1", "f_dc_2", "metallicFactor", "roughnessFactor", "opacity",
              "scale_0", "scale_1", "scale_2", "rot_0", "rot_1", "rot_2", "rot_3")
 PLY_MAX_STRIDE = 4096
+# m2s_debug_codec_eval function ids (m2s_codec.cu; not in m2s.h)
+CODEC_SH0, CODEC_LOGIT, CODEC_LOG_SCALE, CODEC_EXPF, CODEC_SIGMOID = range(5)
 
 
 class m2s_ply_info(C.Structure):

@@ -185,6 +185,20 @@ class Context:
         check(fn(self.handle, dscene.handle, C.byref(p), capacity, C.byref(plan)))
         return plan
 
+    def codec_eval(self, fn: int, x, arg: float = 1.0, out=None):
+        """One function of m2s_codec.cuh (_abi.CODEC_*) applied elementwise to a float32 device tensor on torch's current
+        stream (m2s_debug_codec_eval): the encodings the conversion and the .ply writer use, the decodings the loader
+        uses.  arg: the scale multiplier of CODEC_LOG_SCALE."""
+        torch = _torch()
+        fn_c = lib().m2s_debug_codec_eval
+        fn_c.restype = C.c_int
+        fn_c.argtypes = [C.c_void_p, C.c_uint32, C.c_float, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]
+        x = x.contiguous()
+        if out is None:
+            out = torch.empty_like(x)
+        check(fn_c(self.handle, fn, arg, x.data_ptr(), x.numel(), out.data_ptr(), torch.cuda.current_stream(x.device).cuda_stream))
+        return out
+
     def convert_enqueue(self, dscene: DeviceScene, params: _abi.m2s_params, out, capacity: int, keys=None,
                         total=None, stream: int = 0) -> None:
         """Enqueue only (no synchronisation); out/keys/total are torch device tensors."""

@@ -14,9 +14,9 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libm2s.so")
-SOURCES = ["m2s_kernels.cu", "m2s_prepass.cu", "m2s_sort.cu", "m2s_splat.cu", "m2s_light.cu", "m2s_depth.cu", "m2s_ply_read.cu", "m2s_api.cu", "m2s_scene.cu", "m2s_convert.cu",
+SOURCES = ["m2s_kernels.cu", "m2s_prepass.cu", "m2s_sort.cu", "m2s_splat.cu", "m2s_light.cu", "m2s_depth.cu", "m2s_ply_read.cu", "m2s_codec.cu", "m2s_api.cu", "m2s_scene.cu", "m2s_convert.cu",
            "m2s_viewer.cu", "m2s_host.cpp", "m2s_glb.cpp"]
-HEADERS = ["m2s_host.h", "m2s_ctx.cuh", "m2s_device.cuh", "m2s_prepass.cuh", "m2s_sort.cuh", "m2s_bin.cuh", "m2s_splat.cuh", "m2s_light.cuh", "m2s_depth.cuh", os.path.join("..", "..", "include", "m2s.h")]
+HEADERS = ["m2s_host.h", "m2s_ctx.cuh", "m2s_device.cuh", "m2s_prepass.cuh", "m2s_sort.cuh", "m2s_bin.cuh", "m2s_splat.cuh", "m2s_light.cuh", "m2s_depth.cuh", "m2s_codec.cuh", os.path.join("..", "..", "include", "m2s.h")]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 

@@ -12,6 +12,7 @@
 #include <string>
 #include <vector>
 
+#include "m2s_codec.cuh"
 #include "m2s_ctx.cuh"
 
 namespace m2s {
@@ -197,40 +198,6 @@ __device__ __forceinline__ float ld_f32(const unsigned char* p) {
     if ((reinterpret_cast<uintptr_t>(p) & 3u) == 0) return *reinterpret_cast<const float*>(p);
     return __uint_as_float((uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24));
 }
-// expf as glibc evaluates it on x86-64 with FMA (the table-driven fp64 algorithm of ARM's optimized-routines that glibc
-// uses since 2.28): x N / ln2 = k + r, exp(x) = 2^(k/N) (C0 r^3 + C1 r^2 + C2 r + 1), N = 32, the reduction and the
-// polynomial fused, one rounding to fp32 at the end (denormal results kept).  Bit-identical to that glibc's expf on all
-// 2^32 inputs; CUDA's own expf is not (up to 2 ulp).  tab: the shared copy of kExp2Tab.
-__constant__ unsigned long long kExp2Tab[32] = {   // the bits of 2^(i/32) rounded to fp64, minus i << 47
-    0x3ff0000000000000ULL, 0x3fefd9b0d3158574ULL, 0x3fefb5586cf9890fULL, 0x3fef9301d0125b51ULL,
-    0x3fef72b83c7d517bULL, 0x3fef54873168b9aaULL, 0x3fef387a6e756238ULL, 0x3fef1e9df51fdee1ULL,
-    0x3fef06fe0a31b715ULL, 0x3feef1a7373aa9cbULL, 0x3feedea64c123422ULL, 0x3feece086061892dULL,
-    0x3feebfdad5362a27ULL, 0x3feeb42b569d4f82ULL, 0x3feeab07dd485429ULL, 0x3feea47eb03a5585ULL,
-    0x3feea09e667f3bcdULL, 0x3fee9f75e8ec5f74ULL, 0x3feea11473eb0187ULL, 0x3feea589994cce13ULL,
-    0x3feeace5422aa0dbULL, 0x3feeb737b0cdc5e5ULL, 0x3feec49182a3f090ULL, 0x3feed503b23e255dULL,
-    0x3feee89f995ad3adULL, 0x3feeff76f2fb5e47ULL, 0x3fef199bdd85529cULL, 0x3fef3720dcef9069ULL,
-    0x3fef5818dcfba487ULL, 0x3fef7c97337b9b5fULL, 0x3fefa4afa2a490daULL, 0x3fefd0765b6e4540ULL};
-__device__ __forceinline__ float ref_expf(float x, const unsigned long long* tab) {
-    const uint32_t ux = __float_as_uint(x), abstop = (ux >> 20) & 0x7ffu;
-    if (abstop >= 0x42bu) {                            // |x| >= 88 or NaN
-        if (ux == 0xff800000u) return 0.0f;            // -inf
-        if (abstop >= 0x7f8u) return x + x;            // +inf, NaN
-        if (x > 0x1.62e42ep6f) return __int_as_float(0x7f800000);   // overflow
-        if (x < -0x1.9fe368p6f) return 0.0f;           // underflow
-    }
-    const double kInvLn2N = 0x1.71547652b82fep+0 * 32, kShift = 0x1.8p+52;
-    const double kC0 = 0x1.c6af84b912394p-5 / (32.0 * 32.0 * 32.0), kC1 = 0x1.ebfce50fac4f3p-3 / (32.0 * 32.0), kC2 = 0x1.62e42ff0c52d6p-1 / 32.0;
-    const double xd = (double)x;
-    double kd = __dadd_rn(__dmul_rn(kInvLn2N, xd), kShift);
-    const unsigned long long ki = (unsigned long long)__double_as_longlong(kd);
-    kd = __dsub_rn(kd, kShift);
-    const double r = __fma_rn(kInvLn2N, xd, -kd);
-    const double s = __longlong_as_double((long long)(tab[ki & 31u] + (ki << 47)));
-    const double z = __fma_rn(kC0, r, kC1), r2 = __dmul_rn(r, r);
-    const double y = __fma_rn(z, r2, __fma_rn(kC2, r, 1.0));
-    return __double2float_rn(__dmul_rn(y, s));
-}
-
 __global__ void __launch_bounds__(kDecodeThreads) ply_decode_kernel(const __grid_constant__ PlyDecodeArgs a) {
     __shared__ uint4 stage[kDecodeThreads / 32][kWarpStage / 16 + 2];   // + 32 B: the span's 16-byte-aligned cover
     __shared__ unsigned long long tab[32];
@@ -260,12 +227,9 @@ __global__ void __launch_bounds__(kDecodeThreads) ply_decode_kernel(const __grid
     if ((uint32_t)lane < nrows) {
         const unsigned char* row = reinterpret_cast<const unsigned char*>(stage[warp]) + (s - lo) + (size_t)lane * a.stride;
         auto f = [&](int k) { return ld_f32(row + a.off[k]); };
-        const float kC0 = 0.28209479177387814f;   // SH_COEFF0 (params.hpp:17)
         q0 = make_float4(f(M2S_PLY_X), f(M2S_PLY_Y), f(M2S_PLY_Z), 1.0f);
-        // utils::sigmoid (utils.hpp:269): 1.0 / (1.0 + std::exp(-opacity)), the exp in fp32, the rest in fp64
-        const float ex = ref_expf(-f(M2S_PLY_OPACITY), tab);
-        q1 = make_float4(__fadd_rn(__fmul_rn(f(M2S_PLY_F_DC_0), kC0), 0.5f), __fadd_rn(__fmul_rn(f(M2S_PLY_F_DC_1), kC0), 0.5f),
-                         __fadd_rn(__fmul_rn(f(M2S_PLY_F_DC_2), kC0), 0.5f), __double2float_rn(__ddiv_rn(1.0, __dadd_rn(1.0, (double)ex))));
+        q1 = make_float4(sh0_decode(f(M2S_PLY_F_DC_0)), sh0_decode(f(M2S_PLY_F_DC_1)), sh0_decode(f(M2S_PLY_F_DC_2)),
+                         opacity_sigmoid(f(M2S_PLY_OPACITY), tab));
         q2 = make_float4(ref_expf(f(M2S_PLY_SCALE_0), tab), ref_expf(f(M2S_PLY_SCALE_1), tab), ref_expf(f(M2S_PLY_SCALE_2), tab), 1.0f);
         q3 = a.has_pbr ? make_float4(f(M2S_PLY_NX), f(M2S_PLY_NY), f(M2S_PLY_NZ), 0.0f) : make_float4(0.f, 0.f, 0.f, 0.f);
         // glm::normalize(glm::quat(w = rot_0, x = rot_1, y = rot_2, z = rot_3)), stored (w, x, y, z)

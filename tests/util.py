@@ -25,6 +25,24 @@ NORMAL_OUTLIER_FRACTION = 2e-4
 NORMAL_TOL_OUTLIER = 1e-2
 
 
+def glibc_uses_the_fma_variant() -> bool:
+    """Whether this host's glibc evaluates logf / expf with its FMA variant, the one the device ports (m2s_codec.cuh):
+    glibc selects it on an x86-64 CPU with FMA and AVX2, and aarch64 has no other.  Against that glibc the device's
+    values are bit-identical; against the other variant they are within 1 ulp."""
+    import platform
+    if platform.machine() in ("aarch64", "arm64"):
+        return True
+    try:
+        with open("/proc/cpuinfo") as f:
+            flags = set(f.read().split())
+    except OSError:
+        return False
+    return "fma" in flags and "avx2" in flags
+
+
+GLIBC_MAX_ULP = 0 if glibc_uses_the_fma_variant() else 1
+
+
 def scene_diag(scene: _abi.Scene) -> float:
     pos = scene.triangles.reshape(-1, 3, 12)[:, :, :3].reshape(-1, 3)
     if len(pos) == 0:
