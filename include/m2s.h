@@ -248,7 +248,8 @@ m2s_status m2s_convert_gather_enqueue(m2s_ctx* ctx, const m2s_dscene* scene, con
 /* ASCII header of format 0/1/2 for `count` vertices; returns bytes written (excl. NUL) or the
  * needed size if dst is too small. */
 size_t m2s_ply_header(uint32_t format, uint64_t count, char* dst, size_t dst_size);
-/* GPU encoder: REF96 device records -> .ply body rows on the device (format 0/1/2). */
+/* GPU encoder: REF96 device records -> .ply body rows on the device (format 0/1/2).  Both buffers must be
+ * 16-byte aligned (M2S_E_INVALID otherwise). */
 m2s_status m2s_ply_encode(m2s_ctx* ctx, const void* d_ref96, uint64_t count, uint32_t format,
                           float scale_multiplier, void* d_rows, void* stream);
 /* Host writer: REF96 host records -> file, byte-identical to parsers::savePlyVector. */

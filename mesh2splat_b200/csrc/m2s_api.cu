@@ -69,7 +69,8 @@ static m2s_status ctx_init(m2s_ctx* c) {
     CUDA_TRY(cudaHostAlloc(&c->h_chunk_tot, 2 * m2s_ctx::kMaxChunks * sizeof(unsigned long long), cudaHostAllocMapped));
     std::memset(c->h_chunk_tot, 0, 2 * m2s_ctx::kMaxChunks * sizeof(unsigned long long));
     for (int l = 0; l < m2s_ctx::kLayouts; ++l) {
-        CUDA_TRY(convert_configure(l, &c->blocks_per_sm[l], &c->frag_blocks_per_sm[l]));
+        CUDA_TRY(raster_configure(l, &c->blocks_per_sm[l]));
+        CUDA_TRY(fragment_configure(l, &c->frag_blocks_per_sm[l]));
         if (c->blocks_per_sm[l] < 1 || c->frag_blocks_per_sm[l] < 1) { set_error("conversion kernel does not fit on this device"); return M2S_E_CUDA; }
     }
     return M2S_OK;

@@ -1,7 +1,7 @@
-// m2s_codec.cuh — the per-value encodings of the .ply and PACKED56 outputs and the decodings of the .ply loader, in one
-// place: the conversion's shading (raster and fragment kernels), ply_rows_kernel (m2s_ply_encode) and the .ply decode
-// kernel include this header and nothing else computes these values.  m2s_debug_codec_eval evaluates each function
-// elementwise, so the tests compare them with glibc on every input bit pattern.
+// m2s_codec.cuh — the per-value encodings of the .ply and PACKED56 outputs, the .ply row layouts, and the decodings of
+// the .ply loader, in one place: the conversion's shading (raster and fragment kernels), ply_rows_kernel (m2s_ply_encode)
+// and the .ply decode kernel include this header and nothing else computes these values.  m2s_debug_codec_eval evaluates
+// each function elementwise, so the tests compare them with glibc on every input bit pattern.
 //
 // Every function returns what the reference computes on x86-64 with glibc (2.28 or later, the FMA variant of expf /
 // logf that glibc selects on a CPU with FMA and AVX2), bit for bit, NaN as NaN:
@@ -106,6 +106,58 @@ __device__ __forceinline__ float opacity_logit(float a) {
     return -ref_logf(__fsub_rn(__frcp_rn(__fadd_rn(a, 1e-8f)), 1.0f));
 }
 __device__ __forceinline__ float log_scale(float s, float mult) { return ref_logf(__fmul_rn(s, mult)); }
+
+// ---- the writer's rows (parsers.cpp:431-514 standard, 232-316 PBR, 339-428 compressed) ----
+__device__ __forceinline__ unsigned char to_byte(float v) {
+    v = fminf(fmaxf(v, 0.0f), 1.0f);
+    return (unsigned char)roundf(v * 255.0f);
+}
+// One body row of .ply format FMT at `row`: 0 = standard, 248 bytes, 8-byte aligned (62 floats: xyz n f_dc f_rest(45 x 0)
+// opacity scale rot); 1 = PBR, 76 bytes, 4-byte aligned (19 floats); 2 = compressed, 48 bytes, 4-byte aligned.
+// rgba: linear colour and alpha; q: quaternion (w, x, y, z) and ls: the first two log scales, both read where they are
+// stored (the fragment kernel: its staged record); ls3: the third log scale, the caller's; metal / rough: unused by the
+// standard row.
+template <int FMT>
+__device__ __forceinline__ void ply_row(unsigned char* __restrict__ row, float3 p, float3 n, float4 rgba, const float* q,
+                                        const float* ls, float ls3, float metal, float rough) {
+    if constexpr (FMT == 0) {
+        float2* s2 = reinterpret_cast<float2*>(row);
+        s2[0] = make_float2(p.x, p.y); s2[1] = make_float2(p.z, n.x); s2[2] = make_float2(n.y, n.z);
+        s2[3] = make_float2(sh0_encode(rgba.x), sh0_encode(rgba.y));
+        s2[4] = make_float2(sh0_encode(rgba.z), 0.0f);
+#pragma unroll
+        for (int k = 5; k < 27; ++k) s2[k] = make_float2(0.0f, 0.0f);
+        s2[27] = make_float2(opacity_logit(rgba.w), ls[0]);
+        s2[28] = make_float2(ls[1], ls3);
+        s2[29] = make_float2(q[0], q[1]);
+        s2[30] = make_float2(q[2], q[3]);
+    } else if constexpr (FMT == 1) {
+        float* f = reinterpret_cast<float*>(row);
+        f[0] = p.x; f[1] = p.y; f[2] = p.z; f[3] = n.x; f[4] = n.y; f[5] = n.z;
+        f[6] = sh0_encode(rgba.x); f[7] = sh0_encode(rgba.y); f[8] = sh0_encode(rgba.z);
+        f[9] = metal; f[10] = rough; f[11] = opacity_logit(rgba.w);
+        f[12] = ls[0]; f[13] = ls[1]; f[14] = ls3;
+        f[15] = q[0]; f[16] = q[1]; f[17] = q[2]; f[18] = q[3];
+    } else {
+        float* f = reinterpret_cast<float*>(row);
+        f[0] = p.x; f[1] = p.y; f[2] = p.z;
+        *reinterpret_cast<uchar4*>(row + 12) = make_uchar4(to_byte(rgba.x), to_byte(rgba.y), to_byte(rgba.z), to_byte(rgba.w));
+        f[4] = q[0]; f[5] = q[1]; f[6] = q[2]; f[7] = q[3];
+        f[8] = ls[0]; f[9] = ls[1]; f[10] = ls3;
+        // octahedral normal (parsers.cpp:318-337), without contraction: the bytes equal the writer's on the same normal
+        const float s = __fadd_rn(__fadd_rn(__fadd_rn(fabsf(n.x), fabsf(n.y)), fabsf(n.z)), 1e-8f);
+        const float ox = __fdiv_rn(n.x, s), oy = __fdiv_rn(n.y, s), oz = __fdiv_rn(n.z, s);
+        float rx, ry;
+        if (oz >= 0.0f) { rx = ox; ry = oy; }
+        else {
+            const float m = (ox >= 0.0f && oy >= 0.0f) ? 1.0f : -1.0f;
+            rx = __fmul_rn(__fsub_rn(1.0f, fabsf(oy)), m); ry = __fmul_rn(__fsub_rn(1.0f, fabsf(ox)), m);
+        }
+        const float qx = fminf(fmaxf(roundf(__fmul_rn(__fadd_rn(__fmul_rn(rx, 0.5f), 0.5f), 255.0f)), 0.0f), 255.0f);
+        const float qy = fminf(fmaxf(roundf(__fmul_rn(__fadd_rn(__fmul_rn(ry, 0.5f), 0.5f), 255.0f)), 0.0f), 255.0f);
+        *reinterpret_cast<uchar4*>(row + 44) = make_uchar4((unsigned char)qx, (unsigned char)qy, to_byte(rough), to_byte(metal));
+    }
+}
 
 // ---- the loader's decodings ----
 __device__ __forceinline__ float sh0_decode(float f) { return __fadd_rn(__fmul_rn(f, kShC0), 0.5f); }

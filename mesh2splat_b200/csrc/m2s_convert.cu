@@ -71,11 +71,7 @@ static void convert_plan(const m2s_ctx* ctx, const m2s_dscene* s, const m2s_para
     pl->queue_cap = std::min<uint64_t>(2 * pl->n_units + pl->cap / 32 + pl->cap / pl->flush_frags + pl->cap / pl->item_max +
                                        warps * (2ull * kMaxSplit + kStashItems) + 64, (1u << 24) - 1);
     pl->multi_round = pl->n_units > warps;
-#ifndef M2S_EXP_NODIRECT
     pl->direct_ok = klayout == M2S_LAYOUT_PACKED56 && pl->multi_round && world <= 1;
-#else
-    pl->direct_ok = 0;
-#endif
     // the late claim evens out the weights of the direct units when each warp gets only two of them; with more units
     // per warp they average out anyway and the claim's exposed atomic round trip is not worth it (DESIGN §4)
     pl->claim_late = pl->direct_ok && pl->n_units < 3 * warps;
@@ -91,6 +87,15 @@ M2S_EXPORT m2s_status m2s_debug_convert_plan(m2s_ctx* ctx, const m2s_dscene* s, 
     convert_plan(ctx, s, p, out_capacity, 1u, &pl);
     std::memcpy(plan, &pl, sizeof(pl));
     return M2S_OK;
+}
+
+// The two kernels of one conversion on one stream.  mid != nullptr: recorded between them (measurement of the per-kernel
+// shares); the fragment kernel then launches without programmatic dependent launch, so the kernels do not overlap.
+static cudaError_t convert_launch(int layout, const ConvertArgs& a, int raster_grid, int fragment_grid, cudaStream_t stream, cudaEvent_t mid) {
+    cudaError_t e = raster_launch(layout, a, raster_grid, stream);
+    if (e != cudaSuccess) return e;
+    if (mid) { e = cudaEventRecord(mid, stream); if (e != cudaSuccess) return e; }
+    return fragment_launch(layout, a, fragment_grid, mid == nullptr, stream);
 }
 
 m2s_status m2s::convert_enqueue_impl(m2s_ctx* ctx, const m2s_dscene* s, const m2s_params* p, void* d_out, uint64_t out_capacity,
@@ -170,7 +175,7 @@ m2s_status m2s::convert_enqueue_impl(m2s_ctx* ctx, const m2s_dscene* s, const m2
     cudaError_t e = convert_launch(klayout, a, (int)pl.grid, fgrid, stream, mid);
     if (e != cudaSuccess) { ctx->dirty = true; set_error(std::string("convert launch: ") + cudaGetErrorString(e)); return M2S_E_CUDA; }
     if (peers && peers->world > 1)
-        CUDA_TRY(gather_wait_launch((const unsigned long long*)peers->xch[peers->rank], peers->world, a.epoch, out_capacity,
+        CUDA_TRY(gather_wait_launch((const unsigned long long*)peers->xch[peers->rank], peers->world, a.epoch,
                                     (unsigned long long*)d_total, ctx->d_status, stream));
     return M2S_OK;
 }
@@ -479,9 +484,11 @@ m2s_status m2s::convert_scene_to_ply(m2s_ctx* ctx, const m2s_scene* sc, const m2
 // ---- outputs ----------------------------------------------------------------------------------
 M2S_EXPORT m2s_status m2s_ply_encode(m2s_ctx* ctx, const void* d_ref96, uint64_t count, uint32_t format, float mult, void* d_rows,
                                      void* stream_) {
-    if (!ctx || (count && (!d_ref96 || !d_rows))) { set_error("m2s_ply_encode: NULL argument"); return M2S_E_INVALID; }
+    const char* fn = "m2s_ply_encode";
+    if (!ctx || (count && (!d_ref96 || !d_rows))) return invalid(fn, "NULL argument");
+    if (!aligned_ok(fn, "the record and row buffers must be 16-byte aligned", {{d_ref96, 16}, {d_rows, 16}})) return M2S_E_INVALID;
     if (format > 2) format = 0;  // savePlyVector default branch (parsers.cpp:646-648)
     CUDA_TRY(cudaSetDevice(ctx->device));
-    CUDA_TRY(ply_rows_launch(d_ref96, count, nullptr, format, mult, d_rows, pick_stream(ctx, stream_)));
+    CUDA_TRY(ply_rows_launch(d_ref96, count, format, mult, d_rows, pick_stream(ctx, stream_)));
     return M2S_OK;
 }

@@ -175,7 +175,7 @@ m2s_status vrange_enqueue(m2s_ctx* ctx, m2s_dscene* d, uint64_t lo, uint64_t hi,
 m2s_status upload_texture_groups(m2s_ctx* ctx, m2s_dscene* d, uint32_t t, uint32_t g0, uint32_t g1, std::vector<MipRun>* deferred = nullptr);
 
 // Which texture rows can the triangles [lo, hi) sample?  The v-range per texture is reduced ON THE GPU from the triangles
-// already uploaded (vrange_launch: the host would have to stream the same 144 B/triangle through one core — ~1 ms for
+// already uploaded (vrange_kernel, m2s_scene.cu: the host would have to stream the same 144 B/triangle through one core — ~1 ms for
 // the bench scene), copied back (8 bytes per texture) and turned into 16-row groups here: +-3 groups cover the
 // footprints of all five mip levels (level l reaches 2^(l+1) level-0 rows beyond the sample point, plus the drift of
 // non-power-of-two chains) and the REPEAT wrap at both ends; a range whose v spans a whole period (or is not finite)

@@ -23,7 +23,7 @@ constexpr float kGuard = 8192.0f;        // window-coordinate guard band (|xw| b
 #endif
 
 // ---- raster_kernel -> fragment_kernel interface (context-owned scratch, L2-resident at the sizes of interest) ----
-// The raster kernel only COUNTS: per triangle it leaves a record (TriRec, m2s_kernels.cu) holding the exact edge
+// The raster kernel only COUNTS: per triangle it leaves a record (TriRec, m2s_shade.cuh) holding the exact edge
 // functions, the shading constants and — for small triangles — the 64-bit coverage mask of the candidate box; the
 // fragment kernel enumerates the covered pixels itself (mask rows / exact row spans, m2s_span.cuh).
 // Work of the fragment kernel = the queued FragItems: the small triangles of one work unit, or up to 32 row blocks of
@@ -41,6 +41,11 @@ struct FragItem {               // 288 B
     BlockRef blocks[kItemBlocks];
 };
 static_assert(sizeof(FragItem) == 288, "FragItem layout");
+// FragItem::nblocks flags (the raster kernel's stash carries the same bits)
+constexpr uint32_t kItUnit = 0x80000000u;   // item = the unit's small triangles (one implicit block per triangle)
+constexpr uint32_t kItSplit = 0x40000000u;  // item = one oversized row block, cut into several queue slots
+constexpr uint32_t kItMicro = 0x20000000u;  // unit item of <= 32 fragments: the block area holds the fragments themselves
+                                            // (slot | x << 5 | y << 11, box-relative), one warp shades it with direct loads
 
 // RGBA8 mip chain of one texture inside the texture arena (one allocation for all textures).
 // Levels are pitch-linear, tightly packed, row 0 first; off[] are TEXEL offsets from the arena base.
@@ -124,18 +129,20 @@ struct ConvertArgs {
     uint32_t* status;                  // context status word (mapped pinned host memory): bit 0/1 = a gather wait timed out
 };
 
-// ---- launchers (m2s_kernels.cu) ----
+// ---- launchers ----
+// m2s_raster.cu
 int convert_warps_per_cta(int layout);
 size_t tri_frag_bytes(int layout);
-cudaError_t convert_configure(int layout, int* raster_blocks_per_sm, int* fragment_blocks_per_sm);
-cudaError_t convert_launch(int layout, const ConvertArgs& args, int raster_grid, int fragment_grid, cudaStream_t stream, cudaEvent_t mid);
-cudaError_t gather_wait_launch(const unsigned long long* xch, uint32_t world, unsigned long long epoch, unsigned long long gcap,
-                               unsigned long long* total_global, uint32_t* status, cudaStream_t stream);
+cudaError_t raster_configure(int layout, int* blocks_per_sm);
+cudaError_t raster_launch(int layout, const ConvertArgs& args, int grid, cudaStream_t stream);
+// m2s_fragment.cu; pdl: launched with programmatic dependent launch, overlapping the raster kernel's tail
+cudaError_t fragment_configure(int layout, int* blocks_per_sm);
+cudaError_t fragment_launch(int layout, const ConvertArgs& args, int grid, bool pdl, cudaStream_t stream);
+cudaError_t gather_wait_launch(const unsigned long long* xch, uint32_t world, unsigned long long epoch, unsigned long long* total_global,
+                               uint32_t* status, cudaStream_t stream);
+// m2s_scene.cu
 cudaError_t mip_groups_launch(uint32_t* arena, const DTexture& t, uint32_t g0, uint32_t g1, cudaStream_t stream);
-cudaError_t vrange_launch(const float4* tris, uint32_t first, uint32_t count, const DRange* ranges, uint32_t nranges, const DPrim* prims,
-                          uint32_t ntex, int* minmax, cudaStream_t stream);
-cudaError_t vrange_publish_launch(int* minmax, uint32_t ntex, int* host, unsigned long long* host_tag, unsigned long long tag, cudaStream_t stream);
-cudaError_t ply_rows_launch(const void* ref96, unsigned long long count, const unsigned long long* d_count,
-                            uint32_t format, float mult, void* rows, cudaStream_t stream);
+// m2s_codec.cu
+cudaError_t ply_rows_launch(const void* ref96, unsigned long long count, uint32_t format, float mult, void* rows, cudaStream_t stream);
 
 }  // namespace m2s

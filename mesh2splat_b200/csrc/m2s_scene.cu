@@ -4,6 +4,127 @@
 
 using namespace m2s;
 
+namespace {
+
+// ---- mip chain: 2x2 box, round half up (matches oracle orc_mip_down; GL_TEXTURE_MAX_LEVEL 4, glUtils.cpp:313) ----------
+__device__ __forceinline__ uint32_t box4(uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+    uint32_t o = 0;
+#pragma unroll
+    for (int s = 0; s < 32; s += 8) {
+        const uint32_t sum = ((a >> s) & 0xff) + ((b >> s) & 0xff) + ((c >> s) & 0xff) + ((d >> s) & 0xff);
+        o |= ((sum + 2) >> 2) << s;
+    }
+    return o;
+}
+// ALL levels of the 16-row groups [g0, g0 + gridDim.y) of one texture in one launch: a CTA takes 64 columns x 16 rows of
+// level 0 and produces 32x8, 16x4, 8x2 and 4x1 texels of levels 1..4 (level l row j needs level l-1 rows 2j, 2j+1
+// clamped to the last row: a 16-row group, and a 64-column tile, is closed under the filter).
+__global__ void __launch_bounds__(256) mip_groups_kernel(uint32_t* __restrict__ arena, const DTexture t, uint32_t g0) {
+    __shared__ uint32_t lv[3][8][32];  // levels 1..3 of this tile
+    const uint32_t gx = blockIdx.x, g = g0 + blockIdx.y, tid = threadIdx.x;
+    uint32_t cols = 32, rows = 8;
+#pragma unroll
+    for (uint32_t l = 1; l <= 4; ++l) {
+        if (l < t.nlevels && tid < cols * rows) {
+            const uint32_t lx = tid % cols, ly = tid / cols;
+            const uint32_t x = gx * cols + lx, y = g * rows + ly;
+            const uint32_t dw = t.w[l], dh = t.h[l], sw = t.w[l - 1], sh = t.h[l - 1];
+            if (x < dw && y < dh) {
+                const uint32_t x0 = min(2 * x, sw - 1), x1 = min(2 * x + 1, sw - 1), y0 = min(2 * y, sh - 1), y1 = min(2 * y + 1, sh - 1);
+                uint32_t a, b, c, d;
+                if (l == 1) {
+                    const uint32_t* src = arena + t.off[0];
+                    a = src[(size_t)y0 * sw + x0]; b = src[(size_t)y0 * sw + x1]; c = src[(size_t)y1 * sw + x0]; d = src[(size_t)y1 * sw + x1];
+                } else {  // the source texels are this tile's own texels of the level above
+                    const uint32_t bx = gx * cols * 2, by = g * rows * 2;
+                    a = lv[l - 2][y0 - by][x0 - bx]; b = lv[l - 2][y0 - by][x1 - bx]; c = lv[l - 2][y1 - by][x0 - bx]; d = lv[l - 2][y1 - by][x1 - bx];
+                }
+                const uint32_t o = box4(a, b, c, d);
+                arena[t.off[l] + (size_t)y * dw + x] = o;
+                if (l < 4) lv[l - 1][ly][lx] = o;
+            }
+        }
+        __syncthreads();
+        cols >>= 1; rows >>= 1;
+    }
+}
+
+// ---- v-range of a triangle range per texture (host pipeline: which texture rows must be uploaded before these triangles
+// can be shaded).  minmax: [ntex] sortable-int minima | [ntex] maxima | 1 flag (non-finite or absurd v seen). -----------
+__device__ __forceinline__ int float_key(float f) { const int i = __float_as_int(f); return i ^ ((i >> 31) & 0x7fffffff); }
+__global__ void __launch_bounds__(256) vrange_kernel(const float4* __restrict__ tris, uint32_t first, uint32_t count,
+                                                     const DRange* __restrict__ ranges, uint32_t nranges, const DPrim* __restrict__ prims,
+                                                     uint32_t ntex, int* __restrict__ minmax) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int lane = threadIdx.x & 31;
+    int prim = -1;
+    float vmin = 3.0e38f, vmax = -3.0e38f;
+    bool bad = false;
+    if (i < count) {
+        const uint32_t t = first + i;
+        int lo = 0, hi = (int)nranges - 1;
+        while (lo <= hi) {
+            const int mid = (lo + hi) >> 1;
+            const DRange r = ranges[mid];
+            if (t < r.first) hi = mid - 1;
+            else if (t >= r.end) lo = mid + 1;
+            else { prim = (int)r.prim; break; }
+        }
+        if (prim >= 0) {
+            const float v0 = __ldg(&tris[(size_t)t * 9 + 2]).w, v1 = __ldg(&tris[(size_t)t * 9 + 5]).w, v2 = __ldg(&tris[(size_t)t * 9 + 8]).w;
+            vmin = fminf(v0, fminf(v1, v2)); vmax = fmaxf(v0, fmaxf(v1, v2));
+            bad = !(fabsf(v0) <= 1e30f) || !(fabsf(v1) <= 1e30f) || !(fabsf(v2) <= 1e30f);
+        }
+    }
+    const unsigned full = 0xffffffffu;
+    if (__any_sync(full, bad) && lane == 0) atomicOr(minmax + 2 * ntex, 1);
+    const int p0 = __shfl_sync(full, prim, 0);
+    if (__all_sync(full, prim == p0)) {  // the usual case: the whole warp is inside one primitive
+        if (p0 < 0) return;
+#pragma unroll
+        for (int d = 16; d > 0; d >>= 1) {
+            vmin = fminf(vmin, __shfl_xor_sync(full, vmin, d));
+            vmax = fmaxf(vmax, __shfl_xor_sync(full, vmax, d));
+        }
+        if (lane != 0) return;
+    } else if (prim < 0) return;
+    for (int m = 0; m < 3; ++m) {
+        const int ti = prims[prim].tex[m];
+        if (ti >= 0 && (uint32_t)ti < ntex) {
+            atomicMin(minmax + ti, float_key(vmin));
+            atomicMax(minmax + ntex + ti, float_key(vmax));
+        }
+    }
+}
+
+// The v-ranges of one chunk -> mapped pinned host memory, then a tag the host polls; the device copy is re-armed for its
+// next use (min <- 0x7f7f7f7f, max <- 0x80808080, flag <- 0).  No copy engine: the download engine is busy with records,
+// an 8-byte copy queued behind them reached the host 100-200 us late.
+__global__ void vrange_publish_kernel(int* __restrict__ minmax, uint32_t ntex, volatile int* __restrict__ host, unsigned long long* host_tag,
+                                      unsigned long long tag) {
+    const uint32_t n = 2 * ntex + 1;
+    for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
+        host[i] = minmax[i];
+        minmax[i] = i < ntex ? 0x7f7f7f7f : (i < 2 * ntex ? (int)0x80808080 : 0);
+    }
+    __threadfence_system();
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence_system();
+        *reinterpret_cast<volatile unsigned long long*>(host_tag) = tag;
+    }
+}
+
+}  // namespace
+
+// levels 1.. of the 16-row groups [g0, g1) of one texture (level 0 must be resident), one launch
+cudaError_t m2s::mip_groups_launch(uint32_t* arena, const DTexture& t, uint32_t g0, uint32_t g1, cudaStream_t stream) {
+    if (t.nlevels <= 1 || g1 <= g0) return cudaSuccess;
+    dim3 grd((t.w[0] + 63) / 64, g1 - g0);
+    mip_groups_kernel<<<grd, 256, 0, stream>>>(arena, t, g0);
+    return cudaGetLastError();
+}
+
 // ---- inputs ---------------------------------------------------------------------------------
 M2S_EXPORT m2s_status m2s_compute_bboxes(const float* tris, m2s_primitive* prims, uint32_t nprim, int cumulative) {
     if ((!tris && nprim) || (!prims && nprim)) { set_error("m2s_compute_bboxes: NULL input"); return M2S_E_INVALID; }
@@ -94,10 +215,14 @@ m2s_status m2s::vrange_enqueue(m2s_ctx* ctx, m2s_dscene* d, uint64_t lo, uint64_
         }
         ctx->vr_dirty = false;
     }
-    if (hi > lo)
-        CUDA_TRY(vrange_launch(d->d_tris, (uint32_t)lo, (uint32_t)(hi - lo), d->d_ranges, d->nranges, d->d_prims, nt, v.d_minmax, ctx->aux));
+    if (hi > lo) {
+        vrange_kernel<<<(uint32_t)(hi - lo + 255) / 256, 256, 0, ctx->aux>>>(d->d_tris, (uint32_t)lo, (uint32_t)(hi - lo), d->d_ranges,
+                                                                           d->nranges, d->d_prims, nt, v.d_minmax);
+        CUDA_TRY(cudaGetLastError());
+    }
     v.tag = ++ctx->host_seq;
-    CUDA_TRY(vrange_publish_launch(v.d_minmax, nt, v.h_minmax_dev, v.h_tag_dev, v.tag, ctx->aux));
+    vrange_publish_kernel<<<1, 128, 0, ctx->aux>>>(v.d_minmax, nt, v.h_minmax_dev, v.h_tag_dev, v.tag);
+    CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaEventRecord(v.ev, ctx->aux));
     return M2S_OK;
 }

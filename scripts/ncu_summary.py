@@ -41,13 +41,6 @@ def num(k):
 traffic = num("dram__bytes_read.sum") + num("dram__bytes_write.sum")
 lines += ["", f"DRAM traffic per launch: {traffic/1e6:.2f} MB (read {num('dram__bytes_read.sum')/1e6:.2f} + write {num('dram__bytes_write.sum')/1e6:.2f}); "
           "the 126 MB L2 absorbs most of the record writes of one launch, so this is below the algorithmic bytes."]
-# per-source-region instruction split (needs the same build's .so)
-try:
-    sect = ("raster_kernel" if "raster" in kname else "fragment_kernel") + ("ILi0" if layout == "ref96" else "ILi1")
-    by = subprocess.run([sys.executable, os.path.join(root, "scripts", "ncu_by_line.py"), rep, sect, "25"], capture_output=True, text=True).stdout
-    lines += ["", "## hottest source lines (executed warp-instructions, stall samples)", "", "```", by.strip(), "```"]
-except Exception as e:  # noqa: BLE001
-    lines += ["", f"(source-line join unavailable: {e})"]
 open(out, "w").write("\n".join(lines) + "\n")
 tj = os.path.join(root, "profiles", "traffic.json")
 t = json.load(open(tj)) if os.path.exists(tj) else {}

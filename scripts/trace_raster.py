@@ -24,7 +24,7 @@ for i in range(5):
     out = ctx.convert(ds, R, layout, flags=_abi.FLAG_UNCAPPED, capacity=6 * R * R, out=out.data if out else None)
 t = tr.cpu().numpy().reshape(nw, 16).astype(np.float64)
 _lib.lib().m2s_debug_set_trace(None)
-# slots: enum TraceSlot in m2s_kernels.cu
+# slots: enum TraceSlot in m2s_raster.cu
 PHASES = ["triangle-load wait", "set-up", "walk + scan", "larger tris + flush", "reservation wait", "listing",
           "direct shading", "unit end (stores)", "tail (help, last CTA)"]
 UNITS, DUNITS, GROUPS, CYC, NS, ENTRY = 9, 10, 11, 12, 13, 14

@@ -239,6 +239,18 @@ def test_ply_encode_equals_the_writer_byte_for_byte(gpu_ctx, tmp_path, fmt):
         _same_bits(rows.reshape(n, -1), want, f"format {fmt}, mult {mult:.9g}", byte_lanes=(3, 11) if fmt == 2 else ())
 
 
+def test_ply_encode_rejects_misaligned_buffers(gpu_ctx):
+    """The encoder's wide loads and stores need 16-byte aligned buffers: a misaligned one is an argument error, not a
+    fault.  count = 0: nothing is ever launched, whatever the check does."""
+    import torch
+    from mesh2splat_b200._lib import lib
+    buf = torch.zeros(64, dtype=torch.uint8, device="cuda")
+    p = buf.data_ptr()
+    assert lib().m2s_ply_encode(gpu_ctx.handle, p, 0, 0, 1.0, p + 16, None) == _abi.M2S_OK
+    for ref96, rows in ((p + 4, p), (p, p + 4)):
+        assert lib().m2s_ply_encode(gpu_ctx.handle, ref96, 0, 0, 1.0, rows, None) == _abi.M2S_E_INVALID
+
+
 # ---- export -> import ----------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("fmt", [0, 1])
 def test_convert_file_then_ply_read_equals_the_writer_then_the_loader(gpu_ctx, tmp_path, fmt):
