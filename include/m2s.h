@@ -134,7 +134,8 @@ typedef struct m2s_params {
     uint32_t layout;        /* m2s_layout */
     uint32_t flags;
     /* shard of the flattened triangle list this call converts (multi-GPU: one contiguous range
-     * per rank); triangle_count == 0 means "to the end" */
+     * per rank); triangle_count == 0 means "to the end", so an empty range is first_triangle = the scene's
+     * triangle count */
     uint64_t first_triangle;
     uint64_t triangle_count;
     /* pixel-row band of the R x R grid this call rasterises: rows [row_begin, row_end); row_end == 0 means
@@ -185,7 +186,8 @@ m2s_status m2s_scene_upload(m2s_ctx* ctx, const m2s_scene* scene, m2s_dscene** o
 /* One shard of a scene (multi-GPU: one contiguous triangle range per rank): copies the triangles
  * [first_triangle, first_triangle + triangle_count) to their global positions and, of the maps `layout` consumes, only
  * the texture rows those triangles can sample (16-row groups incl. their mip rows, REPEAT wrap and all five levels'
- * footprints considered).  Converting any triangle outside the range with the returned scene is undefined. */
+ * footprints considered).  Converting any triangle outside the range with the returned scene is undefined.  The empty
+ * range (first_triangle = the scene's triangle count) uploads no triangles and no texture rows. */
 m2s_status m2s_scene_upload_range(m2s_ctx* ctx, const m2s_scene* scene, uint32_t layout, uint64_t first_triangle,
                                   uint64_t triangle_count, m2s_dscene** out);
 /* Payload bytes copied host -> device for this scene so far (triangles + texture rows); accounting for benchmarks. */
@@ -232,8 +234,11 @@ m2s_status m2s_convert_host(m2s_ctx* ctx, const m2s_scene* scene, const m2s_para
  * that maps peer memory into each process (torch symmetric memory, cudaIpc*, cuMem*).
  * xch[p]: rank p's exchange block, M2S_MAX_PEERS*4 uint64, zeroed once before first use.
  * Every rank must make the same sequence of calls (an epoch counter pairs them up).  Layouts REF96 and
- * PACKED56.  d_total_global (device, optional) receives the number of records in the final buffer
- * once all ranks' records have landed; work enqueued after this call on `stream` sees the full buffer. */
+ * PACKED56.  d_total_global (device, optional), once all ranks' records have landed: with world > 1 the number
+ * of records in the final buffer, min(sum over the ranks of min(generated, the rank's cap), out_capacity); with
+ * world == 1 (a plain m2s_convert_enqueue into out[0]) the generated total, which may exceed out_capacity.  Work
+ * enqueued after this call on `stream` sees the full buffer.  A rank with no triangles passes first_triangle =
+ * the scene's triangle count (triangle_count 0 alone means "to the end"); it still takes part, with 0 records. */
 #define M2S_MAX_PEERS 8
 typedef struct m2s_peers {
     uint32_t world, rank;

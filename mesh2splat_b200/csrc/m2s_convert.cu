@@ -175,7 +175,7 @@ m2s_status m2s::convert_enqueue_impl(m2s_ctx* ctx, const m2s_dscene* s, const m2
     cudaError_t e = convert_launch(klayout, a, (int)pl.grid, fgrid, stream, mid);
     if (e != cudaSuccess) { ctx->dirty = true; set_error(std::string("convert launch: ") + cudaGetErrorString(e)); return M2S_E_CUDA; }
     if (peers && peers->world > 1)
-        CUDA_TRY(gather_wait_launch((const unsigned long long*)peers->xch[peers->rank], peers->world, a.epoch,
+        CUDA_TRY(gather_wait_launch((const unsigned long long*)peers->xch[peers->rank], peers->world, a.epoch, out_capacity,
                                     (unsigned long long*)d_total, ctx->d_status, stream));
     return M2S_OK;
 }

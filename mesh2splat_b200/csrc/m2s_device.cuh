@@ -138,8 +138,8 @@ cudaError_t raster_launch(int layout, const ConvertArgs& args, int grid, cudaStr
 // m2s_fragment.cu; pdl: launched with programmatic dependent launch, overlapping the raster kernel's tail
 cudaError_t fragment_configure(int layout, int* blocks_per_sm);
 cudaError_t fragment_launch(int layout, const ConvertArgs& args, int grid, bool pdl, cudaStream_t stream);
-cudaError_t gather_wait_launch(const unsigned long long* xch, uint32_t world, unsigned long long epoch, unsigned long long* total_global,
-                               uint32_t* status, cudaStream_t stream);
+cudaError_t gather_wait_launch(const unsigned long long* xch, uint32_t world, unsigned long long epoch, unsigned long long gcap,
+                               unsigned long long* total_global, uint32_t* status, cudaStream_t stream);
 // m2s_scene.cu
 cudaError_t mip_groups_launch(uint32_t* arena, const DTexture& t, uint32_t g0, uint32_t g1, cudaStream_t stream);
 // m2s_codec.cu

@@ -267,15 +267,16 @@ __global__ void __launch_bounds__(kFragThreads, (LAYOUT == 1 ? M2S_FRAG_THREADS_
 }
 
 // waits until every rank's records of this epoch have landed in THIS rank's final buffer, publishes the
-// total; one thread — the data path never returns to the host
+// number of records it holds: the ranks' stored counts summed, cut at the buffer's capacity gcap (emit_records
+// clips every span there); one thread — the data path never returns to the host
 __global__ void gather_wait_kernel(const unsigned long long* xch, uint32_t world, unsigned long long epoch,
-                                   unsigned long long* total_global, uint32_t* status) {
+                                   unsigned long long gcap, unsigned long long* total_global, uint32_t* status) {
     unsigned long long tot = 0;
     for (uint32_t r = 0; r < world; ++r) {
         wait_epoch(xch + r * 4 + 2, epoch, status, 2u);
         tot += *reinterpret_cast<const volatile unsigned long long*>(xch + r * 4);
     }
-    if (total_global) *total_global = tot;
+    if (total_global) *total_global = tot < gcap ? tot : gcap;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -317,9 +318,9 @@ cudaError_t fragment_launch(int layout, const ConvertArgs& args, int grid, bool 
     });
 }
 
-cudaError_t gather_wait_launch(const unsigned long long* xch, uint32_t world, unsigned long long epoch, unsigned long long* total_global,
-                               uint32_t* status, cudaStream_t stream) {
-    gather_wait_kernel<<<1, 1, 0, stream>>>(xch, world, epoch, total_global, status);
+cudaError_t gather_wait_launch(const unsigned long long* xch, uint32_t world, unsigned long long epoch, unsigned long long gcap,
+                               unsigned long long* total_global, uint32_t* status, cudaStream_t stream) {
+    gather_wait_kernel<<<1, 1, 0, stream>>>(xch, world, epoch, gcap, total_global, status);
     return cudaGetLastError();
 }
 

@@ -22,7 +22,10 @@ import numpy as np
 
 def plan_shards(triangle_count: int, world: int, cost: np.ndarray | None = None) -> list:
     """Contiguous (first, count) per rank.  With `cost` (per-triangle estimated work, e.g. bbox pixel
-    area) the cuts balance cumulative cost; otherwise triangle counts."""
+    area) the cuts balance cumulative cost; otherwise triangle counts.  The non-empty ranges go to the first ranks,
+    in triangle order.  The ranks left without triangles (fewer triangles than ranks, or one heavy triangle) come
+    last, each with (triangle_count, 0): m2s_params reads a count of 0 as "to the end", so that is the only range it
+    converts as empty, and it keeps every range starting where the previous one ends."""
     if world < 1:
         raise ValueError("world must be >= 1")
     if cost is None or triangle_count == 0:
@@ -36,7 +39,8 @@ def plan_shards(triangle_count: int, world: int, cost: np.ndarray | None = None)
         cuts = np.searchsorted(cum, targets, side="left").astype(np.int64)
         cuts[0], cuts[-1] = 0, triangle_count
         cuts = np.maximum.accumulate(np.clip(cuts, 0, triangle_count)).tolist()
-    return [(int(cuts[r]), int(cuts[r + 1] - cuts[r])) for r in range(world)]
+    ranges = [(int(cuts[r]), int(cuts[r + 1] - cuts[r])) for r in range(world) if cuts[r + 1] > cuts[r]]
+    return ranges + [(int(triangle_count), 0)] * (world - len(ranges))
 
 
 def plan_work(triangle_count: int, world: int, resolution: int, cost: np.ndarray | None = None) -> list:

@@ -86,6 +86,48 @@ def test_plan_shards_properties():
         plan_shards(10, 0)
 
 
+def _assert_partition(sh, T, w):
+    """The non-empty ranges are contiguous in rank order, come first and partition [0, T); every empty range is
+    (T, 0), the only (first, count) m2s_params reads as no triangles (a count of 0 means "to the end")."""
+    assert len(sh) == w and sum(c for _, c in sh) == T
+    full = [r for r in sh if r[1] > 0]
+    assert sh[len(full):] == [(T, 0)] * (w - len(full)), sh
+    if full:
+        assert full[0][0] == 0 and full[-1][0] + full[-1][1] == T
+        assert all(full[i][0] + full[i][1] == full[i + 1][0] for i in range(len(full) - 1)), sh
+
+
+def test_plan_shards_empty_ranges():
+    """Fewer triangles than ranks, or one triangle heavier than a rank's share, leave ranks without triangles: they
+    get (T, 0), after the ranks that have triangles, and the oracle converts no record for them."""
+    sys.path.insert(0, ROOT)
+    import oracle
+    from mesh2splat_b200 import synth
+    from mesh2splat_b200.shard import estimate_cost, plan_shards, plan_work
+    for T in (0, 1, 2, 3, 7, 1000):
+        for w in (1, 2, 3, 8):
+            sh = plan_shards(T, w)
+            _assert_partition(sh, T, w)
+            assert sum(c == 0 for _, c in sh) == max(0, w - T)
+    heavy = np.ones(5); heavy[2] = 1000.0   # one triangle outweighs every other
+    for w in (2, 4, 8):
+        sh = plan_shards(5, w, heavy)
+        _assert_partition(sh, 5, w)
+        assert (w > 2) == any(c == 0 for _, c in sh), sh
+    assert plan_shards(3, 8) == [(0, 1), (1, 1), (2, 1)] + [(3, 0)] * 5
+    assert plan_shards(2, 3) == [(0, 1), (1, 1), (2, 0)]
+    # plan_work without a cost, or with one when there are fewer rows than ranks, hands out triangle ranges
+    assert plan_work(2, 4, 512, None) == [(0, 1, 0, 0), (1, 1, 0, 0), (2, 0, 0, 0), (2, 0, 0, 0)]
+    q = synth.unit_quad()
+    plan = plan_work(q.triangle_count, 4, 2, estimate_cost(q.triangles, q.primitives[0].bbox_min, q.primitives[0].bbox_max, 2))
+    assert plan == [(0, 1, 0, 0), (1, 1, 0, 0), (2, 0, 0, 0), (2, 0, 0, 0)]
+    # the oracle reads the range as m2s_params does: an empty range converts 0 records, the others their triangles
+    for R, ranges in ((2, [p[:2] for p in plan]), (64, plan_shards(2, 3)), (64, plan_shards(2, 8))):
+        totals = [oracle.convert(q, R, first_triangle=a, triangle_count=n)[2] for a, n in ranges]
+        assert all((t == 0) == (n == 0) for t, (_, n) in zip(totals, ranges)), (ranges, totals)
+        assert sum(totals) == oracle.convert(q, R)[2] == R * R
+
+
 def test_plan_work_switches_to_row_bands_for_huge_triangles():
     """A 2-triangle quad cannot be balanced by triangle ranges: plan_work hands every rank all triangles and a
     band of pixel rows; the bands partition the grid and the per-band oracle outputs add up to the whole."""
