@@ -24,7 +24,8 @@ constexpr float kShC0 = 0.28209479177387814f;  // SH_COEFF0 (params.hpp:17)
 // ---- glibc's logf and expf (the table-driven fp64 algorithms of ARM's optimized-routines, glibc >= 2.28) ----
 // logf: x = 2^k z, z in [0x3f330000, 2 * that) split into 16 subintervals with c near each centre; log(x) =
 // log1p(z / c - 1) + log(c) + k ln2, log1p by a degree-3 polynomial in fp64, one rounding to fp32 at the end.
-// kLogfTab: (1 / c, log(c)) of each subinterval, as the bits of glibc's __logf_data.tab.
+// kLogfTab: (1 / c, log(c)) of each subinterval, as the bits of glibc's __logf_data.tab.  tab: kLogfTab or a copy of it
+// (the raster kernel keeps one in shared memory: two dependent global loads fewer in every fragment's opacity).
 static __device__ const double kLogfTab[32] = {
     0x1.661ec79f8f3bep+0, -0x1.57bf7808caadep-2, 0x1.571ed4aaf883dp+0, -0x1.2bef0a7c06ddbp-2,
     0x1.49539f0f010bp+0,  -0x1.01eae7f513a67p-2, 0x1.3c995b0b80385p+0, -0x1.b31d8a68224e9p-3,
@@ -34,7 +35,7 @@ static __device__ const double kLogfTab[32] = {
     0x1.e608cfd9a47acp-1, 0x1.aa5aa5df25984p-5,  0x1.ca4b31f026aap-1,  0x1.c5e53aa362eb4p-4,
     0x1.b2036576afce6p-1, 0x1.526e57720db08p-3,  0x1.9c2d163a1aa2dp-1, 0x1.bc2860d22477p-3,
     0x1.886e6037841edp-1, 0x1.1058bc8a07ee1p-2,  0x1.767dcf5534862p-1, 0x1.4043057b6ee09p-2};
-__device__ __forceinline__ float ref_logf(float x) {
+__device__ __forceinline__ float ref_logf(float x, const double* tab) {
     uint32_t ix = __float_as_uint(x);
     if (ix == 0x3f800000u) return 0.0f;
     if (ix - 0x00800000u >= 0x7f800000u - 0x00800000u) {   // subnormal, zero, negative, inf or NaN
@@ -46,7 +47,7 @@ __device__ __forceinline__ float ref_logf(float x) {
     const uint32_t tmp = ix - 0x3f330000u;
     const int i = (int)((tmp >> 19) & 15u), k = (int32_t)tmp >> 23;
     const double z = (double)__uint_as_float(ix - (tmp & 0xff800000u));
-    const double invc = __ldg(kLogfTab + 2 * i), logc = __ldg(kLogfTab + 2 * i + 1);
+    const double invc = tab[2 * i], logc = tab[2 * i + 1];
     const double kLn2 = 0x1.62e42fefa39efp-1, kA0 = -0x1.00ea348b88334p-2, kA1 = 0x1.5575b0be00b6ap-2, kA2 = -0x1.ffffef20a4123p-2;
     const double r = __fma_rn(z, invc, -1.0);
     const double y0 = __dadd_rn(logc, __dmul_rn((double)k, kLn2));
@@ -56,6 +57,7 @@ __device__ __forceinline__ float ref_logf(float x) {
     y = __fma_rn(y, r2, __dadd_rn(y0, r));
     return __double2float_rn(y);
 }
+__device__ __forceinline__ float ref_logf(float x) { return ref_logf(x, kLogfTab); }
 
 // expf: x N / ln2 = k + r, exp(x) = 2^(k/N) (C0 r^3 + C1 r^2 + C2 r + 1), N = 32, the reduction and the polynomial fused,
 // one rounding to fp32 at the end (denormal results kept).  tab: kExp2Tab or a copy of it (the .ply decoder keeps one in
@@ -101,10 +103,11 @@ __device__ __forceinline__ float sh0_encode(float c) {
 }
 // std::clamp keeps a NaN alpha (NaN < 0 and 1 < NaN are false), so NaN encodes to NaN; alpha 1 encodes to +inf.
 // __frcp_rn is the IEEE 1.0f / x.
-__device__ __forceinline__ float opacity_logit(float a) {
+__device__ __forceinline__ float opacity_logit(float a, const double* logtab) {
     a = a < 0.0f ? 0.0f : (1.0f < a ? 1.0f : a);
-    return -ref_logf(__fsub_rn(__frcp_rn(__fadd_rn(a, 1e-8f)), 1.0f));
+    return -ref_logf(__fsub_rn(__frcp_rn(__fadd_rn(a, 1e-8f)), 1.0f), logtab);
 }
+__device__ __forceinline__ float opacity_logit(float a) { return opacity_logit(a, kLogfTab); }
 __device__ __forceinline__ float log_scale(float s, float mult) { return ref_logf(__fmul_rn(s, mult)); }
 
 // ---- the writer's rows (parsers.cpp:431-514 standard, 232-316 PBR, 339-428 compressed) ----

@@ -48,7 +48,15 @@ __device__ __forceinline__ void tma_store_1d(void* dst_gmem, const void* src_sme
 }
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// the bulk groups of this thread but the most recent one have finished reading their sources
+__device__ __forceinline__ void tma_store_wait_read_but_last() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
+// 8 bytes global -> shared without a register round trip (LDGSTS): the copy flies while the thread goes on
+__device__ __forceinline__ void cp_async_8(void* dst_smem, const void* src_gmem) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(dst_smem)), "l"(src_gmem) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 __device__ __forceinline__ void st_release_sys(unsigned long long* p, unsigned long long v) {
     asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");

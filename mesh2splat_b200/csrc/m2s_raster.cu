@@ -16,7 +16,7 @@
 //     pixel-row band); the triangle's resolved sampler state (mip level pair, blend fraction, level offsets)
 //   coverage is only COUNTED here:
 //     small triangles (box <= 64 pixels, <= 32 rows, int32-safe): lane-per-triangle lock-step walk of the box
-//       with incremental edge functions -> 64-bit coverage mask, stored in the record; a warp scan gives every
+//       with incremental edge functions (box_mask, m2s_span.cuh) -> 64-bit coverage mask, stored in the record; a warp scan gives every
 //       triangle its offset inside the unit; ONE global atomicAdd per unit reserves the output range
 //       (the reference: one atomicCounterIncrement per fragment)
 //     all other triangles: lane-per-ROW exact interval (m2s_span.cuh: three estimated divisions + exact int64
@@ -28,7 +28,8 @@
 //   PACKED56 records also carry the varyings the layout needs (position, uv) as PLANES over the pixel grid (fp64
 //     coefficients from the exact edge functions): the fragment stage needs neither the vertices nor 64-bit arithmetic
 //   DIRECT path (PACKED56, launches where the warps take several units each): the small triangles of a light unit are
-//     shaded by the warp that rasterised them, straight from the records in its shared-memory slice (direct_run)
+//     shaded by the warp that rasterised them, straight from the records in its shared-memory slice (direct_run); each
+//     group of 32 records leaves through one bulk async copy
 //
 // Bit-exactness: every float operation of the per-triangle stage is written with __f*_rn intrinsics in the
 // operation order of the oracle (and of GLM, which the reference's GLSL-as-C++ build uses): coverage is
@@ -82,6 +83,7 @@ struct __align__(128) WarpBlock {
     uint32_t itN[kStashItems];                    // blocks per item | kItUnit / kItSplit
     uint32_t itTotal[kStashItems];                // fragments per item
     uint64_t bar;
+    double logtab[RK == 1 ? 32 : 1];              // PACKED56: the direct path's copy of ref_logf's table (kLogfTab)
 };
 
 // The scene's descriptor tables as the set-up sees them: in shared memory when they fit (each CTA copies
@@ -480,27 +482,40 @@ struct CtaQueue {
 // warps of an SM are too few to hide the latency of the shading chain and the unit goes to the fragment kernel (that was
 // faster than the direct path, also with CTA-level group stealing and software pipelining, when measured during
 // development).
-// The worker: the `total` listed fragments of this warp's unit, 32 at a time.  Out of line: its registers are not the
-// raster loop's.
+// The worker: the `total` listed fragments of this warp's unit, 32 at a time (PACKED56).  Out of line: its registers are
+// not the raster loop's.  It takes the few per-launch values it needs as arguments (through a ConvertArgs reference every
+// group re-loaded them).  tri0: the unit's first triangle of the scene; base / room: OutRange; logtab: ref_logf's table.
+// A group's records leave the stage as one bulk async copy issued by lane 0 (bulk_span, with emit_records' capacity cut);
+// the groups alternate between the two halves of the stage, so a group is shaded while the previous one's copy reads.
 // ------------------------------------------------------------------------------------------
-template <int RK>
-__device__ __noinline__ void direct_run(const ConvertArgs& a, WarpBlock<RK>& wb, uint32_t total, unsigned long long dfirst, uint32_t t0,
-                                        unsigned long long base_prev, unsigned long long room, int lane) {
-    constexpr int kStride = Cfg<RK>::kStride;   // layout == raster kind for REF96 / PACKED56
-    static_assert(32 * kStride <= kUnitTris * kTriBytes, "the output stage lives in the triangle staging area");
-    unsigned char* stage = reinterpret_cast<unsigned char*>(wb.tri);   // dead since the set-up of the unit
+__device__ __noinline__ void direct_run(WarpBlock<1>& wb, uint32_t total, unsigned long long dfirst, uint32_t tri0, uint8_t* out,
+                                        unsigned long long* keys, const uint32_t* __restrict__ texb, const double* logtab, float log_sz,
+                                        unsigned long long base, unsigned long long room, int lane) {
+    constexpr int kStride = Cfg<1>::kStride;
+    constexpr uint32_t kHalf = kUnitTris * kTriBytes / 2;
+    static_assert(8 + 32 * kStride <= kHalf && kHalf % 16 == 0, "two output stages (32 records + the shift) in the triangle staging area");
+    unsigned char* const stage0 = reinterpret_cast<unsigned char*>(wb.tri);   // dead since the set-up of the unit
     const unsigned short* list = reinterpret_cast<const unsigned short*>(wb.pend);
     for (uint32_t g0 = 0; g0 < total; g0 += 32) {
         const uint32_t nfr = min(32u, total - g0);
         const uint32_t e = list[g0 + min((uint32_t)lane, nfr - 1u)];  // idle lanes shadow the last fragment
         const uint32_t slot = e & 31u;
         const int dxi = (int)((e >> 5) & 63u), dyi = (int)(e >> 11);
-        const unsigned long long idx0 = dfirst + g0;
-        shade<RK>(a, wb.rec[slot], nullptr, dxi, dyi, a.tex_base, stage + stage_shift<kStride>(base_prev + idx0) + lane * kStride);
+        const unsigned long long idx = dfirst + g0;
+        unsigned char* const stage = stage0 + ((g0 >> 5) & 1u) * kHalf;
+        Frag1 s;
+        shade1_fetch(wb.rec[slot], dxi, dyi, texb, s);
+        if (lane == 0) tma_store_wait_read_but_last();   // the copy from this half, two groups ago
         __syncwarp();
-        emit_records<kStride>(a, stage, nfr, idx0, base_prev, room, false, 0ull, 0u,
-                              [&] { return fragment_key(a.tri_first + t0 + slot, wb.rec[slot].meta, (uint32_t)dxi, (uint32_t)dyi); }, lane);
+        shade1_finish(log_sz, logtab, wb.rec[slot], s, stage + stage_shift<kStride>(base + idx) + lane * kStride);
+        fence_proxy_async();   // the stage's writes, before the bulk copy reads them
         __syncwarp();
+        const uint32_t nval = idx < room ? (uint32_t)min((unsigned long long)nfr, room - idx) : 0u;
+        if (lane == 0) {   // one bulk group per group of records, empty past the cut: "two groups ago" stays exact
+            bulk_span<kStride>(out, (base + idx) * (unsigned long long)kStride, stage, nval * kStride);
+            tma_store_commit();
+        }
+        if (keys != nullptr && (uint32_t)lane < nval) keys[base + idx + lane] = fragment_key(tri0 + slot, wb.rec[slot].meta, (uint32_t)dxi, (uint32_t)dyi);
     }
 }
 
@@ -515,6 +530,7 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     WarpBlock<RK>& wb = *reinterpret_cast<WarpBlock<RK>*>(smem + (size_t)warp * sizeof(WarpBlock<RK>));
     const unsigned char* tri_bytes = reinterpret_cast<const unsigned char*>(a.tris);
+    constexpr bool kDirectOK = (RK == 1);   // PACKED56: the records carry everything the shading needs
 #ifdef M2S_TRACE
     long long tr_prev_ = clock64();
     const long long tr_c0_ = tr_prev_;
@@ -538,6 +554,10 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         tma_load_1d(wb.tri, tri_bytes + ((size_t)a.tri_first + t0) * kTriBytes, bytes, &wb.bar);
     };
     if (lane == 0 && unit < a.n_units) issue_load(unit);
+    // ref_logf's table for the direct path's opacities -> the warp's slice, as an asynchronous copy that lands while the
+    // first unit is set up (waited for before the first shading; a CTA-wide copy would wait at the barrier below: ~1 us
+    // more per warp, measured on the H100)
+    if constexpr (kDirectOK) cp_async_8(wb.logtab + lane, kLogfTab + lane);
 
     // descriptor tables -> shared memory (once per CTA) when they fit
     Tables tabs{a.ranges, a.prims, a.texs, a.nranges};
@@ -562,7 +582,6 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
     if (threadIdx.x < kCtaQueueCap) cq.q[threadIdx.x].ready = 0u;
     __syncthreads();  // tables + help queue: the only CTA-wide barrier before the end of the kernel
     const OutRange out = out_range(a);   // the direct path's records
-    constexpr bool kDirectOK = (RK == 1);   // PACKED56: the records carry everything the shading needs
     uint32_t phase = 0;
     Stash st;
     st.n_it = 0; st.cur_nb = 0; st.cur_total = 0; st.frags = 0; st.slots = 0; st.seen = 0;
@@ -601,13 +620,13 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         next = __shfl_sync(0xffffffffu, next, 0);
 
         // ---- small triangles: lane-per-triangle lock-step walk of the candidate box -> coverage mask ----
-        int e0 = 0, e1 = 0, e2 = 0, a0 = 0, a1 = 0, a2 = 0, r0 = 0, r1 = 0, r2 = 0, w = 1;
+        int e0 = 0, e1 = 0, e2 = 0, a0 = 0, a1 = 0, a2 = 0, b0 = 0, b1 = 0, b2 = 0, w = 1;
         bool small = false;
         if (cnt) {
             w = ts.w;
             const int h = ts.h;
             a0 = ts.A[0]; a1 = ts.A[1]; a2 = ts.A[2];
-            const int b0 = ts.B[0], b1 = ts.B[1], b2 = ts.B[2];
+            b0 = ts.B[0]; b1 = ts.B[1]; b2 = ts.B[2];
             // E at the box origin, with the ownership bias folded in: inside <=> all E' >= 0
             const long long E0 = ts.E0[0] - ((ts.incl & 1u) ? 0 : 1);
             const long long E1 = ts.E0[1] - ((ts.incl & 2u) ? 0 : 1);
@@ -617,23 +636,10 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
             const long long s1 = llabs(E1) + (long long)(w - 1) * abs(a1) + (long long)(h - 1) * abs(b1);
             const long long s2 = llabs(E2) + (long long)(w - 1) * abs(a2) + (long long)(h - 1) * abs(b2);
             small = cnt <= kSmallCand && h <= 32 && s0 < lim && s1 < lim && s2 < lim;
-            if (small) {
-                e0 = (int)E0; e1 = (int)E1; e2 = (int)E2;
-                r0 = b0 - (w - 1) * a0; r1 = b1 - (w - 1) * a1; r2 = b2 - (w - 1) * a2;  // step to the next row's first pixel
-            }
+            if (small) { e0 = (int)E0; e1 = (int)E1; e2 = (int)E2; }
         }
-        unsigned long long hits = 0;
-        {
-            const uint32_t mine = small ? cnt : 0u;
-            const uint32_t maxc = __reduce_max_sync(0xffffffffu, mine);
-            int col = 0, f0 = e0, f1 = e1, f2 = e2;
-            for (uint32_t it = 0; it < maxc; ++it) {
-                const bool inside = it < mine && (f0 | f1 | f2) >= 0;
-                hits |= (unsigned long long)inside << it;
-                if (++col == w) { col = 0; f0 += r0; f1 += r1; f2 += r2; }
-                else { f0 += a0; f1 += a1; f2 += a2; }
-            }
-        }
+        const uint32_t mine = small ? cnt : 0u;
+        const unsigned long long hits = box_mask(e0, e1, e2, a0, a1, a2, b0, b1, b2, w, mine, __reduce_max_sync(0xffffffffu, mine));
         const uint32_t nh = (uint32_t)__popcll(hits);
         uint32_t incl_scan = nh;  // inclusive warp scan
 #pragma unroll
@@ -719,15 +725,17 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
                 TR_ADD(a, kTrDirectUnits, 1);
                 // every lane lists the covered pixels of its triangle at their place in the unit
                 list_pixels(reinterpret_cast<unsigned short*>(wb.pend), incl_scan - nh, hits, (uint32_t)w, (uint32_t)lane);
+                cp_async_wait_all();   // wb.logtab has landed (a no-op after the first direct unit)
                 __syncwarp();
                 TR_PHASE(a, kTrList);
-                direct_run<RK>(a, wb, total_small, dfirst, t0, out.base, out.room, lane);
+                direct_run(wb, total_small, dfirst, a.tri_first + t0, a.out, a.keys, a.tex_base, wb.logtab, a.log_sz, out.base, out.room, lane);
                 TR_PHASE(a, kTrShade);
                 TR_ADD(a, kTrGroups, (total_small + 31) / 32);
                 // the stage was written through the generic proxy: every writer fences before the TMA engine writes there again
                 fence_proxy_async();
                 __syncwarp();
                 if (claim_late) claim();
+                if (lane == 0) tma_store_wait_read();   // the last groups' copies have read the stage
                 if (lane == 0 && next < a.n_units) issue_load(next);
             }
         }
@@ -776,6 +784,7 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         stash_flush<RK>(a, wb, eu, st, lane);
     }
     if (lane == 0) tma_store_wait_all();  // record stores are complete (not just read) before the kernel ends
+    if constexpr (kDirectOK) cp_async_wait_all();   // a warp without a direct unit never waited for its wb.logtab
     // ---- last CTA out publishes the counts and re-arms the scheduler for the next launch ---------
     __syncthreads();
     if (warp == 0) {

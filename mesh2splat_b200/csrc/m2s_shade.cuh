@@ -6,6 +6,7 @@
 #include <cstddef>
 #include "m2s_codec.cuh"
 #include "m2s_device.cuh"
+#include "m2s_ptx.cuh"
 #include "m2s_span.cuh"
 
 // resident raster warps per SM per raster kind (a multiple of 4: register allocation granularity)
@@ -236,7 +237,9 @@ __device__ __forceinline__ void shade1_fetch(const TriRec<1>& tf, int dxi, int d
     s.w = bl.w;
     s.has = fetch_footprint(texb, ref, f, bl, s.tx);
 }
-__device__ __forceinline__ void shade1_finish(const ConvertArgs& a, const TriRec<1>& tf, const Frag1& s, unsigned char* __restrict__ srec_bytes) {
+// log_sz: ConvertArgs::log_sz; logtab: kLogfTab or a copy of it (ref_logf)
+__device__ __forceinline__ void shade1_finish(float log_sz, const double* logtab, const TriRec<1>& tf, const Frag1& s,
+                                              unsigned char* __restrict__ srec_bytes) {
     // converterFS.glsl:55-62,99; parsers.cpp:484-499: SH0, opacity logit, log scale (per triangle)
     const uint32_t k4b = opaque_4b();
     float cr = 1.f, cg = 1.f, cb = 1.f, ca = 1.f;
@@ -248,9 +251,12 @@ __device__ __forceinline__ void shade1_finish(const ConvertArgs& a, const TriRec
     s2[1] = make_float2(s.Pz, q.x);
     s2[2] = make_float2(q.y, q.z);
     s2[3] = make_float2(q.w, tf.sx);
-    s2[4] = make_float2(s.sy, a.log_sz);
+    s2[4] = make_float2(s.sy, log_sz);
     s2[5] = make_float2(sh0_encode(cr), sh0_encode(cg));
-    s2[6] = make_float2(sh0_encode(cb), opacity_logit(ca));
+    s2[6] = make_float2(sh0_encode(cb), opacity_logit(ca, logtab));
+}
+__device__ __forceinline__ void shade1_finish(const ConvertArgs& a, const TriRec<1>& tf, const Frag1& s, unsigned char* __restrict__ srec_bytes) {
+    shade1_finish(a.log_sz, kLogfTab, tf, s, srec_bytes);
 }
 
 // One fragment: pixel (dx, dy) relative to the box origin of the triangle whose record is `tf`; v: its 9 float4 of vertex
@@ -393,6 +399,23 @@ __device__ __forceinline__ void copy_span(uint8_t* dstbase, unsigned long long b
             if (c < nw) dst[c] = src[c];
         }
     }
+}
+
+// copy_span for strides that are 8 mod 16, issued by ONE lane: the 16-byte body as one bulk async copy (cp.async.bulk,
+// SASS UBLKCP), the 8-byte head and tail as plain stores.  The caller fences the stage's generic-proxy writes
+// (fence_proxy_async) before, commits the bulk group after (tma_store_commit; an empty group when nothing was copied), and
+// waits for the copy's reads (tma_store_wait_read) before the stage is written again.
+template <int STRIDE>
+__device__ __forceinline__ void bulk_span(uint8_t* dstbase, unsigned long long boff, const unsigned char* stage, uint32_t nbytes) {
+    static_assert(STRIDE % 16 == 8, "the stage shift aligns source and destination of 8-mod-16 strides only");
+    if (nbytes == 0) return;
+    const uint32_t head = (uint32_t)(boff & 8ull);   // == stage_shift of the first record
+    stage += head;
+    if (head) *reinterpret_cast<float2*>(dstbase + boff) = *reinterpret_cast<const float2*>(stage);
+    const uint32_t body = (nbytes - head) & ~15u;
+    if (body) tma_store_1d(dstbase + boff + head, stage + head, body);
+    const uint32_t pos = head + body;
+    if (pos < nbytes) *reinterpret_cast<float2*>(dstbase + boff + pos) = *reinterpret_cast<const float2*>(stage + pos);
 }
 
 // fragment identity: global triangle << 24 | y << 12 | x (meta: the triangle's box origin, TriRec::meta)
