@@ -4,7 +4,7 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
 import oracle
-from test_abi_host import _glb_with_image
+from util import write_image_glb
 from mesh2splat_b200.gltf import load_glb
 from PIL import Image
 
@@ -12,7 +12,7 @@ d = tempfile.mkdtemp(); rng = np.random.default_rng(5)
 worst = 0
 def cmp(blob, tag):
     global worst
-    p = os.path.join(d, "t.glb"); _glb_with_image(p, blob, "image/jpeg")
+    p = os.path.join(d, "t.glb"); write_image_glb(p, blob, "image/jpeg")
     ok, meshes = oracle.ref_load_glb(p)
     ours = load_glb(p).textures[0]
     t = meshes[0]["textures"].get(0)

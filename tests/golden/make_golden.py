@@ -137,8 +137,7 @@ def loader_vectors():
     import tempfile
     from PIL import Image
     sys.path.insert(0, os.path.join(ROOT, "tests"))
-    from test_abi_host import _glb_with_image, _make_glb
-    from util import png_encode
+    from util import png_encode, write_image_glb, write_quad_glb
     if oracle.ref_loader_lib() is None:
         raise SystemExit("oracle/_ref/libm2s_refloader.so is not built (no /root/reference here)")
     rng = np.random.default_rng(424242)
@@ -182,7 +181,7 @@ def loader_vectors():
                             q = rng.normal(size=4); q /= np.linalg.norm(q)
                             kw["trs"] = ([float(v) for v in rng.normal(size=3) * 3], [float(v) for v in q], [float(v) for v in rng.random(3) * 3 + 0.1])
                         path = os.path.join(d, f"g{k}.glb")
-                        _make_glb(path, **kw)
+                        write_quad_glb(path, **kw)
                         add(f"geom{k:02d}", path)
                         k += 1
         # images: every 8-bit-or-less PNG type (plain + Adam7), JPEG baseline/progressive x subsampling, gray
@@ -200,7 +199,7 @@ def loader_vectors():
                 trns = b"".join(int(v).to_bytes(2, "big") for v in smp[4, 5])
             for il in (False, True):
                 path = os.path.join(d, "p.glb")
-                _glb_with_image(path, png_encode(smp, ctype, depth, il, plte, trns), "image/png")
+                write_image_glb(path, png_encode(smp, ctype, depth, il, plte, trns), "image/png")
                 add(f"png_c{ctype}_d{depth}_i{int(il)}", path)
         for (w, h) in [(64, 48), (37, 70), (17, 9), (1, 1)]:
             yy, xx = np.mgrid[0:h, 0:w].astype(np.float32)
@@ -211,12 +210,12 @@ def loader_vectors():
                     b = io.BytesIO()
                     Image.fromarray(img).save(b, "JPEG", quality=80, subsampling=ss, progressive=prog)
                     path = os.path.join(d, "j.glb")
-                    _glb_with_image(path, b.getvalue(), "image/jpeg")
+                    write_image_glb(path, b.getvalue(), "image/jpeg")
                     add(f"jpeg_{w}x{h}_p{int(prog)}_s{ss}", path)
             b = io.BytesIO()
             Image.fromarray(img[..., 0]).save(b, "JPEG", quality=80)
             path = os.path.join(d, "j.glb")
-            _glb_with_image(path, b.getvalue(), "image/jpeg")
+            write_image_glb(path, b.getvalue(), "image/jpeg")
             add(f"jpeg_{w}x{h}_gray", path)
         # random multi-mesh scene graphs (nested matrix / TRS nodes, instancing, several materials sharing images,
         # u8 / u16 / u32 / no indices, skipped LINES and POSITION-less primitives, two scenes)

@@ -14,7 +14,7 @@ import pytest
 import oracle
 from mesh2splat_b200 import _abi, _lib, synth
 from mesh2splat_b200._abi import Primitive, Scene
-from util import png_bytes
+from util import write_glb, write_image_glb, write_quad_glb
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -131,75 +131,10 @@ def test_ply_writer_matches_reference_savePlyVector_golden(tmp_path, fmt):
 
 
 # ---- .glb loader ------------------------------------------------------------------------------------
-def _make_glb(path, *, indexed=True, with_normals=True, with_tangents=True, with_uv=True, with_texture=True,
-              matrix=None, trs=None, two_prims=False):
-    rng = np.random.default_rng(5)
-    pos = np.array([[0, 0, 0], [1, 0, 0], [1, 1, 0], [0, 1, 0.5]], np.float32)
-    nrm = np.tile(np.array([0, 0, 1], np.float32), (4, 1))
-    tan = np.tile(np.array([1, 0, 0, -1], np.float32), (4, 1))
-    uv = pos[:, :2].copy()
-    idx = np.array([0, 1, 2, 0, 2, 3], np.uint16)
-    img = rng.integers(0, 256, size=(5, 7, 4), dtype=np.uint8)
-    img_rgb = rng.integers(0, 256, size=(4, 4, 3), dtype=np.uint8)
-    blobs, views, accessors = [], [], []
-
-    def add_view(b):
-        off = sum(len(x) for x in blobs)
-        pad = (-len(b)) % 4
-        blobs.append(b + b"\x00" * pad)
-        views.append({"buffer": 0, "byteOffset": off, "byteLength": len(b)})
-        return len(views) - 1
-
-    def add_acc(arr, ctype, typ):
-        v = add_view(arr.tobytes())
-        accessors.append({"bufferView": v, "componentType": ctype, "count": len(arr), "type": typ})
-        return len(accessors) - 1
-
-    if not indexed:
-        pos_, nrm_, tan_, uv_ = pos[idx], nrm[idx], tan[idx], uv[idx]
-    else:
-        pos_, nrm_, tan_, uv_ = pos, nrm, tan, uv
-    attrs = {"POSITION": add_acc(pos_, 5126, "VEC3")}
-    if with_normals: attrs["NORMAL"] = add_acc(nrm_, 5126, "VEC3")
-    if with_tangents: attrs["TANGENT"] = add_acc(tan_, 5126, "VEC4")
-    if with_uv: attrs["TEXCOORD_0"] = add_acc(uv_, 5126, "VEC2")
-    prim = {"attributes": attrs, "material": 0}
-    if indexed: prim["indices"] = add_acc(idx, 5123, "SCALAR")
-    prims = [prim]
-    if two_prims:
-        prims.append({"attributes": {"POSITION": add_acc(pos_ + np.float32(3.0), 5126, "VEC3")}, "mode": 4})
-        prims.append({"attributes": {"POSITION": attrs["POSITION"]}, "mode": 1})   # lines: skipped
-    gltf = {"asset": {"version": "2.0"}, "scene": 0, "scenes": [{"nodes": [0]}],
-            "nodes": [{"children": [1], "name": "root"}, {"mesh": 0}],
-            "meshes": [{"name": "quad", "primitives": prims}],
-            "materials": [{"pbrMetallicRoughness": {"baseColorFactor": [0.5, 0.6, 0.7, 0.8]}}]}
-    if matrix is not None: gltf["nodes"][0]["matrix"] = [float(x) for x in np.asarray(matrix, np.float32).T.reshape(-1)]
-    if trs is not None:
-        gltf["nodes"][1].update({"translation": trs[0], "rotation": trs[1], "scale": trs[2]})
-    if with_texture:
-        iv = add_view(png_bytes(img)); iv2 = add_view(png_bytes(img_rgb))
-        gltf["images"] = [{"bufferView": iv, "mimeType": "image/png"}, {"bufferView": iv2, "mimeType": "image/png"}]
-        gltf["textures"] = [{"source": 0}, {"source": 1}]
-        gltf["materials"][0]["pbrMetallicRoughness"]["baseColorTexture"] = {"index": 0}
-        gltf["materials"][0]["pbrMetallicRoughness"]["metallicRoughnessTexture"] = {"index": 1}
-        gltf["materials"][0]["normalTexture"] = {"index": 0, "scale": 2.0}
-    gltf["bufferViews"] = views; gltf["accessors"] = accessors
-    binblob = b"".join(blobs)
-    gltf["buffers"] = [{"byteLength": len(binblob)}]
-    js = json.dumps(gltf).encode()
-    js += b" " * ((-len(js)) % 4)
-    total = 12 + 8 + len(js) + 8 + len(binblob)
-    with open(path, "wb") as f:
-        f.write(struct.pack("<4sII", b"glTF", 2, total))
-        f.write(struct.pack("<I4s", len(js), b"JSON")); f.write(js)
-        f.write(struct.pack("<I4s", len(binblob), b"BIN\x00")); f.write(binblob)
-    return dict(pos=pos, nrm=nrm, tan=tan, uv=uv, idx=idx, img=img, img_rgb=img_rgb)
-
-
 def test_glb_loader_basic(tmp_path):
     from mesh2splat_b200.gltf import load_glb
     p = tmp_path / "a.glb"
-    src = _make_glb(str(p))
+    src = write_quad_glb(str(p))
     s = load_glb(str(p))
     assert s.triangle_count == 2 and len(s.primitives) == 1 and s.primitives[0].name == "quad_0"
     v = s.triangles.reshape(2, 3, 12)
@@ -220,7 +155,7 @@ def test_glb_loader_fallbacks_and_transforms(tmp_path):
     from mesh2splat_b200.gltf import load_glb
     p = tmp_path / "b.glb"
     M = np.eye(4, dtype=np.float32); M[:3, :3] = np.diag([2.0, 1.0, 0.5]); M[:3, 3] = (1, 2, 3)
-    src = _make_glb(str(p), indexed=False, with_normals=False, with_tangents=False, with_texture=False, matrix=M,
+    src = write_quad_glb(str(p), indexed=False, with_normals=False, with_tangents=False, with_texture=False, matrix=M,
                     trs=([0.5, 0.0, 0.0], [0.0, 0.0, 0.70710678, 0.70710678], [1.0, 1.0, 2.0]), two_prims=True)
     s = load_glb(str(p))
     assert [q.name for q in s.primitives] == ["quad_0", "quad_1"]     # the LINES primitive is skipped, no counter bump
@@ -265,11 +200,8 @@ def _rewrite_glb_json(src: str, dst: str, edit) -> None:
     jlen = struct.unpack_from("<I", raw, 12)[0]
     g = json.loads(raw[20:20 + jlen])
     edit(g)
-    js = json.dumps(g).encode(); js += b" " * ((-len(js)) % 4)
-    rest = raw[20 + jlen:]
-    with open(dst, "wb") as f:
-        f.write(struct.pack("<4sII", b"glTF", 2, 12 + 8 + len(js) + len(rest)))
-        f.write(struct.pack("<I4s", len(js), b"JSON")); f.write(js); f.write(rest)
+    blen = struct.unpack_from("<I", raw, 20 + jlen)[0]
+    write_glb(dst, g, raw[28 + jlen:28 + jlen + blen])
 
 
 _HOSTILE = [-1, -3, -1000000, 2**31, 2**40, 2**63, 1e300, 0.5, -0.5]
@@ -282,7 +214,7 @@ def test_glb_loader_rejects_hostile_sizes(tmp_path):
     import subprocess
     import sys as _sys
     base = tmp_path / "base.glb"
-    _make_glb(str(base))
+    write_quad_glb(str(base))
     cases = []
     for i, bad in enumerate(_HOSTILE):
         def e_img_off(g, bad=bad): g["bufferViews"][g["images"][0]["bufferView"]]["byteOffset"] = bad
@@ -312,25 +244,6 @@ def test_glb_loader_rejects_hostile_sizes(tmp_path):
     r = subprocess.run([_sys.executable, "-c", child, *cases], capture_output=True, text=True, timeout=300)
     assert r.returncode == 0, f"loader crashed (rc {r.returncode}): {r.stderr[-400:]}"
     assert r.stdout.strip() == f"rejected {len(cases)} of {len(cases)}", r.stdout
-
-
-def _glb_with_image(path, blob: bytes, mime: str):
-    """Single-triangle .glb whose baseColorTexture is `blob`."""
-    pos = np.array([[0, 0, 0], [1, 0, 0], [0, 1, 0]], np.float32).tobytes()
-    views = [{"buffer": 0, "byteOffset": 0, "byteLength": len(pos)}, {"buffer": 0, "byteOffset": len(pos), "byteLength": len(blob)}]
-    gltf = {"asset": {"version": "2.0"}, "scenes": [{"nodes": [0]}], "nodes": [{"mesh": 0}],
-            "meshes": [{"primitives": [{"attributes": {"POSITION": 0}, "material": 0}]}],
-            "materials": [{"pbrMetallicRoughness": {"baseColorTexture": {"index": 0}}}],
-            "textures": [{"source": 0}], "images": [{"bufferView": 1, "mimeType": mime}],
-            "accessors": [{"bufferView": 0, "componentType": 5126, "count": 3, "type": "VEC3"}], "bufferViews": views}
-    binblob = pos + blob
-    binblob += b"\x00" * ((-len(binblob)) % 4)
-    gltf["buffers"] = [{"byteLength": len(binblob)}]
-    js = json.dumps(gltf).encode(); js += b" " * ((-len(js)) % 4)
-    with open(path, "wb") as f:
-        f.write(struct.pack("<4sII", b"glTF", 2, 12 + 8 + len(js) + 8 + len(binblob)))
-        f.write(struct.pack("<I4s", len(js), b"JSON")); f.write(js)
-        f.write(struct.pack("<I4s", len(binblob), b"BIN\x00")); f.write(binblob)
 
 
 def _loader_golden():
@@ -390,7 +303,7 @@ def test_glb_loader_decodes_baseline_jpeg(tmp_path, mode, subsampling, size):
     pil.save(buf, "JPEG", **kw)
     want = np.asarray(Image.open(io.BytesIO(buf.getvalue())).convert("RGB")).astype(np.int32)
     p = tmp_path / "j.glb"
-    _glb_with_image(str(p), buf.getvalue(), "image/jpeg")
+    write_image_glb(str(p), buf.getvalue(), "image/jpeg")
     s = load_glb(str(p))
     got = s.textures[0]
     assert got.shape == (h, w, 4) and np.all(got[..., 3] == 255)
@@ -444,7 +357,7 @@ def test_glb_loader_decodes_every_png_type(tmp_path, ctype, depth, interlace):
         want[...] = to8(smp)
     blob = png_encode(smp, ctype, depth, interlace, plte, trns)
     p = tmp_path / "p.glb"
-    _glb_with_image(str(p), blob, "image/png")
+    write_image_glb(str(p), blob, "image/png")
     got = load_glb(str(p)).textures[0]
     assert got.shape == (h, w, 4)
     assert np.array_equal(got.astype(np.int64), want)
@@ -483,7 +396,7 @@ def test_glb_loader_decodes_progressive_jpeg(tmp_path, mode, subsampling, size, 
             assert b"\xff\xc2" in buf.getvalue()
             want = np.asarray(Image.open(io.BytesIO(buf.getvalue())).convert("RGB")).astype(np.int32)
         p = tmp_path / f"j{int(prog)}.glb"
-        _glb_with_image(str(p), buf.getvalue(), "image/jpeg")
+        write_image_glb(str(p), buf.getvalue(), "image/jpeg")
         outs[prog] = load_glb(str(p)).textures[0]
     got = outs[True]
     assert got.shape == (h, w, 4) and np.all(got[..., 3] == 255)
@@ -504,7 +417,7 @@ def test_glb_loader_rejects_arithmetic_jpeg(tmp_path):
     Image.fromarray(np.full((16, 16, 3), 90, np.uint8)).save(buf, "JPEG")
     blob = buf.getvalue().replace(b"\xff\xc0", b"\xff\xc9", 1)
     p = tmp_path / "p.glb"
-    _glb_with_image(str(p), blob, "image/jpeg")
+    write_image_glb(str(p), blob, "image/jpeg")
     with pytest.raises(ValueError, match="arithmetic"):
         load_glb(str(p))
 

@@ -257,9 +257,9 @@ def test_convert_file_then_ply_read_equals_the_writer_then_the_loader(gpu_ctx, t
     """m2s_convert_file then m2s_ply_read equals orc_ply_load of m2s_ply_write's bytes of the REF96 conversion of the same
     .glb, bit for bit (as multisets of records: both files are in atomic arrival order)."""
     from mesh2splat_b200.gltf import load_glb
-    from test_abi_host import _make_glb
+    from util import write_quad_glb
     glb, ply, ref_ply = tmp_path / "m.glb", tmp_path / f"m{fmt}.ply", tmp_path / f"r{fmt}.ply"
-    _make_glb(str(glb), two_prims=True)
+    write_quad_glb(str(glb), two_prims=True)
     R, std = 96, 0.65
     res = gpu_ctx.convert_file(str(glb), R, str(ply), std, fmt)
     ds = gpu_ctx.upload(load_glb(str(glb)))

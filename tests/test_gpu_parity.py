@@ -315,10 +315,10 @@ def test_convert_host_pipelined_capacity(gpu_ctx):
 def test_convert_file_glb_to_ply(gpu_ctx, tmp_path, fmt):
     """m2s_convert_file = loadModel -> ConversionPass::execute -> exportPly: the file must be the oracle's file
     (same header bytes, same rows as a multiset; rows are ordered by atomic arrival in both)."""
-    from test_abi_host import _make_glb
+    from util import write_quad_glb
     from mesh2splat_b200.gltf import load_glb
     glb, ply = tmp_path / "m.glb", tmp_path / f"m{fmt}.ply"
-    _make_glb(str(glb), two_prims=True)
+    write_quad_glb(str(glb), two_prims=True)
     R, std = 96, 0.65
     res = gpu_ctx.convert_file(str(glb), R, str(ply), std, fmt)
     s = load_glb(str(glb))

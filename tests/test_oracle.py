@@ -87,7 +87,7 @@ def live_transform_glbs(directory):
     """24 single-mesh .glb files with random node transforms and attribute combinations: [(k, path)]."""
     import sys
     sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-    from test_abi_host import _make_glb
+    from util import write_quad_glb
     rng = np.random.default_rng(99)
     out = []
     for k in range(24):
@@ -99,7 +99,7 @@ def live_transform_glbs(directory):
             kw = dict(trs=([float(v) for v in rng.normal(size=3)], [float(v) for v in q], [float(v) for v in rng.random(3) * 2 + 0.2]))
         kw.update(with_normals=bool(k % 3), with_tangents=bool(k % 5), indexed=bool(k % 4))
         p = os.path.join(str(directory), f"c{k}.glb")
-        _make_glb(p, **kw)
+        write_quad_glb(p, **kw)
         out.append((k, p))
     return out
 

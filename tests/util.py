@@ -10,6 +10,10 @@ Tolerances (stated once, used everywhere):
 """
 from __future__ import annotations
 
+import json
+import struct
+import zlib
+
 import numpy as np
 
 from mesh2splat_b200 import _abi
@@ -128,11 +132,12 @@ def assert_records_match(scene: _abi.Scene, layout: int, got, got_keys, want, wa
         raise ValueError(layout)
 
 
+def _png_chunk(t: bytes, d: bytes) -> bytes:
+    return struct.pack(">I", len(d)) + t + d + struct.pack(">I", zlib.crc32(t + d) & 0xffffffff)
+
+
 def png_bytes(img: np.ndarray) -> bytes:
     """Minimal PNG writer (RGBA8 / RGB8 / gray8, filter 0) for loader tests."""
-    import struct
-    import zlib
-
     img = np.ascontiguousarray(img, np.uint8)
     if img.ndim == 2:
         ctype, ch = 0, 1
@@ -141,12 +146,8 @@ def png_bytes(img: np.ndarray) -> bytes:
         ctype = {1: 0, 2: 4, 3: 2, 4: 6}[ch]
     h, w = img.shape[:2]
     raw = b"".join(b"\x00" + img[y].tobytes() for y in range(h))
-
-    def chunk(t, d):
-        return struct.pack(">I", len(d)) + t + d + struct.pack(">I", zlib.crc32(t + d) & 0xffffffff)
-
-    return (b"\x89PNG\r\n\x1a\n" + chunk(b"IHDR", struct.pack(">IIBBBBB", w, h, 8, ctype, 0, 0, 0))
-            + chunk(b"IDAT", zlib.compress(raw, 6)) + chunk(b"IEND", b""))
+    return (b"\x89PNG\r\n\x1a\n" + _png_chunk(b"IHDR", struct.pack(">IIBBBBB", w, h, 8, ctype, 0, 0, 0))
+            + _png_chunk(b"IDAT", zlib.compress(raw, 6)) + _png_chunk(b"IEND", b""))
 
 
 def planar_triangulation(n_points: int, seed: int) -> _abi.Scene:
@@ -262,57 +263,122 @@ class GuardedHost:
         assert len(holes) == 0, f"{self.what}: {len(holes)} records below `written` never written, first {int(holes[0])}"
 
 
-def write_soup_glb(path: str, triangles: np.ndarray, texture: np.ndarray | None = None,
-                   base_color=(1.0, 1.0, 1.0, 1.0)) -> None:
-    """A .glb of one mesh with one non-indexed primitive: POSITION, NORMAL, TANGENT and TEXCOORD_0 straight from the
-    (T, 36) triangle array (3 x {pos3 nrm3 tan4 uv2}), optionally with a PNG base-colour texture (RGBA8)."""
-    import json
-    import struct
-    v = np.ascontiguousarray(triangles, np.float32).reshape(-1, 12)
-    blobs, views, accessors = [], [], []
+class GlbBin:
+    """The BIN chunk of a .glb being built, with its bufferViews and accessors; every view starts 4-byte aligned."""
 
-    def add_view(b):
-        off = sum(len(x) for x in blobs)
-        blobs.append(b + b"\x00" * ((-len(b)) % 4))
-        views.append({"buffer": 0, "byteOffset": off, "byteLength": len(b)})
-        return len(views) - 1
+    def __init__(self):
+        self.blobs, self.views, self.accessors = [], [], []
 
-    def add_acc(arr, typ, minmax=False):
-        a = np.ascontiguousarray(arr, np.float32)
-        acc = {"bufferView": add_view(a.tobytes()), "componentType": 5126, "count": len(a), "type": typ}
-        if minmax:
-            acc["min"] = [float(x) for x in a.min(axis=0)]; acc["max"] = [float(x) for x in a.max(axis=0)]
-        accessors.append(acc)
-        return len(accessors) - 1
+    def add_view(self, b: bytes) -> int:
+        self.views.append({"buffer": 0, "byteOffset": sum(len(x) for x in self.blobs), "byteLength": len(b)})
+        self.blobs.append(b + b"\x00" * ((-len(b)) % 4))
+        return len(self.views) - 1
 
-    attrs = {"POSITION": add_acc(v[:, 0:3], "VEC3", True), "NORMAL": add_acc(v[:, 3:6], "VEC3"),
-             "TANGENT": add_acc(v[:, 6:10], "VEC4"), "TEXCOORD_0": add_acc(v[:, 10:12], "VEC2")}
-    pbr = {"baseColorFactor": [float(x) for x in base_color]}
-    gltf = {"asset": {"version": "2.0"}, "scene": 0, "scenes": [{"nodes": [0]}], "nodes": [{"mesh": 0}],
-            "meshes": [{"name": "soup", "primitives": [{"attributes": attrs, "material": 0}]}],
-            "materials": [{"pbrMetallicRoughness": pbr}]}
-    if texture is not None:
-        gltf["images"] = [{"bufferView": add_view(png_bytes(texture)), "mimeType": "image/png"}]
-        gltf["textures"] = [{"source": 0}]
-        pbr["baseColorTexture"] = {"index": 0}
-    gltf["bufferViews"] = views
-    gltf["accessors"] = accessors
-    binblob = b"".join(blobs)
+    def add_accessor(self, arr, ctype: int, typ: str, **extra) -> int:
+        arr = np.ascontiguousarray(arr)
+        self.accessors.append({"bufferView": self.add_view(arr.tobytes()), "componentType": ctype, "count": len(arr),
+                               "type": typ, **extra})
+        return len(self.accessors) - 1
+
+    def bytes(self) -> bytes:
+        return b"".join(self.blobs)
+
+
+def write_glb(path: str, gltf: dict, binblob: bytes) -> None:
+    """Writes a .glb: the glTF JSON chunk (`buffers` set to the BIN chunk, padded with spaces), then the BIN chunk."""
     gltf["buffers"] = [{"byteLength": len(binblob)}]
     js = json.dumps(gltf).encode()
     js += b" " * ((-len(js)) % 4)
     with open(path, "wb") as f:
         f.write(struct.pack("<4sII", b"glTF", 2, 12 + 8 + len(js) + 8 + len(binblob)))
-        f.write(struct.pack("<I4s", len(js), b"JSON")); f.write(js)
-        f.write(struct.pack("<I4s", len(binblob), b"BIN\x00")); f.write(binblob)
+        f.write(struct.pack("<I4s", len(js), b"JSON") + js)
+        f.write(struct.pack("<I4s", len(binblob), b"BIN\x00") + binblob)
+
+
+def write_soup_glb(path: str, triangles: np.ndarray, texture: np.ndarray | None = None,
+                   base_color=(1.0, 1.0, 1.0, 1.0)) -> None:
+    """A .glb of one mesh with one non-indexed primitive: POSITION, NORMAL, TANGENT and TEXCOORD_0 straight from the
+    (T, 36) triangle array (3 x {pos3 nrm3 tan4 uv2}), optionally with a PNG base-colour texture (RGBA8)."""
+    v = np.ascontiguousarray(triangles, np.float32).reshape(-1, 12)
+    b = GlbBin()
+    pos = v[:, 0:3]
+    attrs = {"POSITION": b.add_accessor(pos, 5126, "VEC3", min=[float(x) for x in pos.min(axis=0)],
+                                        max=[float(x) for x in pos.max(axis=0)]),
+             "NORMAL": b.add_accessor(v[:, 3:6], 5126, "VEC3"), "TANGENT": b.add_accessor(v[:, 6:10], 5126, "VEC4"),
+             "TEXCOORD_0": b.add_accessor(v[:, 10:12], 5126, "VEC2")}
+    pbr = {"baseColorFactor": [float(x) for x in base_color]}
+    gltf = {"asset": {"version": "2.0"}, "scene": 0, "scenes": [{"nodes": [0]}], "nodes": [{"mesh": 0}],
+            "meshes": [{"name": "soup", "primitives": [{"attributes": attrs, "material": 0}]}],
+            "materials": [{"pbrMetallicRoughness": pbr}]}
+    if texture is not None:
+        gltf["images"] = [{"bufferView": b.add_view(png_bytes(texture)), "mimeType": "image/png"}]
+        gltf["textures"] = [{"source": 0}]
+        pbr["baseColorTexture"] = {"index": 0}
+    gltf["bufferViews"] = b.views
+    gltf["accessors"] = b.accessors
+    write_glb(path, gltf, b.bytes())
+
+
+def write_quad_glb(path, *, indexed=True, with_normals=True, with_tangents=True, with_uv=True, with_texture=True,
+                   matrix=None, trs=None, two_prims=False):
+    """A .glb of one quad (two triangles, mesh "quad") under a parent node, with the given attributes, node transform
+    and textures; two_prims adds a shifted POSITION-only copy and a LINES primitive.  Returns the source arrays."""
+    rng = np.random.default_rng(5)
+    pos = np.array([[0, 0, 0], [1, 0, 0], [1, 1, 0], [0, 1, 0.5]], np.float32)
+    nrm = np.tile(np.array([0, 0, 1], np.float32), (4, 1))
+    tan = np.tile(np.array([1, 0, 0, -1], np.float32), (4, 1))
+    uv = pos[:, :2].copy()
+    idx = np.array([0, 1, 2, 0, 2, 3], np.uint16)
+    img = rng.integers(0, 256, size=(5, 7, 4), dtype=np.uint8)
+    img_rgb = rng.integers(0, 256, size=(4, 4, 3), dtype=np.uint8)
+    b = GlbBin()
+    pos_, nrm_, tan_, uv_ = (pos, nrm, tan, uv) if indexed else (pos[idx], nrm[idx], tan[idx], uv[idx])
+    attrs = {"POSITION": b.add_accessor(pos_, 5126, "VEC3")}
+    if with_normals: attrs["NORMAL"] = b.add_accessor(nrm_, 5126, "VEC3")
+    if with_tangents: attrs["TANGENT"] = b.add_accessor(tan_, 5126, "VEC4")
+    if with_uv: attrs["TEXCOORD_0"] = b.add_accessor(uv_, 5126, "VEC2")
+    prim = {"attributes": attrs, "material": 0}
+    if indexed: prim["indices"] = b.add_accessor(idx, 5123, "SCALAR")
+    prims = [prim]
+    if two_prims:
+        prims.append({"attributes": {"POSITION": b.add_accessor(pos_ + np.float32(3.0), 5126, "VEC3")}, "mode": 4})
+        prims.append({"attributes": {"POSITION": attrs["POSITION"]}, "mode": 1})   # lines: skipped
+    gltf = {"asset": {"version": "2.0"}, "scene": 0, "scenes": [{"nodes": [0]}],
+            "nodes": [{"children": [1], "name": "root"}, {"mesh": 0}],
+            "meshes": [{"name": "quad", "primitives": prims}],
+            "materials": [{"pbrMetallicRoughness": {"baseColorFactor": [0.5, 0.6, 0.7, 0.8]}}]}
+    if matrix is not None: gltf["nodes"][0]["matrix"] = [float(x) for x in np.asarray(matrix, np.float32).T.reshape(-1)]
+    if trs is not None:
+        gltf["nodes"][1].update({"translation": trs[0], "rotation": trs[1], "scale": trs[2]})
+    if with_texture:
+        iv = b.add_view(png_bytes(img)); iv2 = b.add_view(png_bytes(img_rgb))
+        gltf["images"] = [{"bufferView": iv, "mimeType": "image/png"}, {"bufferView": iv2, "mimeType": "image/png"}]
+        gltf["textures"] = [{"source": 0}, {"source": 1}]
+        gltf["materials"][0]["pbrMetallicRoughness"]["baseColorTexture"] = {"index": 0}
+        gltf["materials"][0]["pbrMetallicRoughness"]["metallicRoughnessTexture"] = {"index": 1}
+        gltf["materials"][0]["normalTexture"] = {"index": 0, "scale": 2.0}
+    gltf["bufferViews"] = b.views; gltf["accessors"] = b.accessors
+    write_glb(path, gltf, b.bytes())
+    return dict(pos=pos, nrm=nrm, tan=tan, uv=uv, idx=idx, img=img, img_rgb=img_rgb)
+
+
+def write_image_glb(path, blob: bytes, mime: str):
+    """Single-triangle .glb whose baseColorTexture is `blob`."""
+    b = GlbBin()
+    b.add_accessor(np.array([[0, 0, 0], [1, 0, 0], [0, 1, 0]], np.float32), 5126, "VEC3")
+    b.add_view(blob)
+    gltf = {"asset": {"version": "2.0"}, "scenes": [{"nodes": [0]}], "nodes": [{"mesh": 0}],
+            "meshes": [{"primitives": [{"attributes": {"POSITION": 0}, "material": 0}]}],
+            "materials": [{"pbrMetallicRoughness": {"baseColorTexture": {"index": 0}}}],
+            "textures": [{"source": 0}], "images": [{"bufferView": 1, "mimeType": mime}],
+            "accessors": b.accessors, "bufferViews": b.views}
+    write_glb(path, gltf, b.bytes())
 
 
 def png_encode(samples: np.ndarray, ctype: int, depth: int, interlace: bool = False, plte: bytes | None = None,
                trns: bytes | None = None) -> bytes:
     """General PNG writer for loader tests.  samples: (h, w, channels) integers < 2**depth (channels: 1 gray/palette,
     2 gray+alpha, 3 rgb, 4 rgba).  Rows cycle through the five filter types; Adam7 when interlace."""
-    import struct
-    import zlib
     smp = np.asarray(samples)
     h, w, ch = smp.shape
     assert ch == {0: 1, 2: 3, 3: 1, 4: 2, 6: 4}[ctype]
@@ -361,17 +427,14 @@ def png_encode(samples: np.ndarray, ctype: int, depth: int, interlace: bool = Fa
             continue
         raw += filt([pack_row(sub[y]) for y in range(sub.shape[0])])
 
-    def chunk(t, d):
-        return struct.pack(">I", len(d)) + t + d + struct.pack(">I", zlib.crc32(t + d) & 0xffffffff)
-
-    out = b"\x89PNG\r\n\x1a\n" + chunk(b"IHDR", struct.pack(">IIBBBBB", w, h, depth, ctype, 0, 0, 1 if interlace else 0))
+    out = b"\x89PNG\r\n\x1a\n" + _png_chunk(b"IHDR", struct.pack(">IIBBBBB", w, h, depth, ctype, 0, 0, 1 if interlace else 0))
     if plte is not None:
-        out += chunk(b"PLTE", plte)
+        out += _png_chunk(b"PLTE", plte)
     if trns is not None:
-        out += chunk(b"tRNS", trns)
+        out += _png_chunk(b"tRNS", trns)
     half = len(raw) // 2 or 1
     z = zlib.compress(raw, 6)
-    return out + chunk(b"IDAT", z[:half]) + chunk(b"IDAT", z[half:]) + chunk(b"IEND", b"")
+    return out + _png_chunk(b"IDAT", z[:half]) + _png_chunk(b"IDAT", z[half:]) + _png_chunk(b"IEND", b"")
 
 
 def make_complex_glb(path: str, seed: int) -> None:
@@ -379,27 +442,15 @@ def make_complex_glb(path: str, seed: int) -> None:
     nodes, 2-4 meshes of 1-3 primitives (index types u8 / u16 / u32 / none; optional NORMAL / TANGENT / TEXCOORD_0;
     a LINES primitive and a POSITION-less one that must be skipped), several materials sharing images, a primitive
     without a material, a mesh instanced by two nodes, an unnamed mesh, optionally two scenes with `scene` set."""
-    import json
-    import struct
     rng = np.random.default_rng(seed)
-    blobs, views, accessors = [], [], []
-
-    def add_view(b):
-        off = sum(len(x) for x in blobs)
-        blobs.append(b + b"\x00" * ((-len(b)) % 4))
-        views.append({"buffer": 0, "byteOffset": off, "byteLength": len(b)})
-        return len(views) - 1
-
-    def add_acc(arr, ctype, typ):
-        accessors.append({"bufferView": add_view(np.ascontiguousarray(arr).tobytes()), "componentType": ctype, "count": len(arr), "type": typ})
-        return len(accessors) - 1
+    b = GlbBin()
 
     nimg = int(rng.integers(1, 4))
     images = []
     for i in range(nimg):
         w, h = int(rng.integers(2, 9)), int(rng.integers(2, 9))
         ch = int(rng.choice([3, 4]))
-        images.append({"bufferView": add_view(png_bytes(rng.integers(0, 256, size=(h, w, ch), dtype=np.uint8))), "mimeType": "image/png"})
+        images.append({"bufferView": b.add_view(png_bytes(rng.integers(0, 256, size=(h, w, ch), dtype=np.uint8))), "mimeType": "image/png"})
     textures = [{"source": int(rng.integers(0, nimg))} for _ in range(int(rng.integers(1, 5)))]
     materials = []
     for m in range(int(rng.integers(1, 4))):
@@ -417,24 +468,24 @@ def make_complex_glb(path: str, seed: int) -> None:
         for pi in range(int(rng.integers(1, 4))):
             nv = int(rng.integers(3, 12))
             pos = (rng.normal(size=(nv, 3)) * 2).astype(np.float32)
-            attrs = {"POSITION": add_acc(pos, 5126, "VEC3")}
+            attrs = {"POSITION": b.add_accessor(pos, 5126, "VEC3")}
             if rng.random() < 0.6:
-                n = rng.normal(size=(nv, 3)); attrs["NORMAL"] = add_acc((n / np.linalg.norm(n, axis=1, keepdims=True)).astype(np.float32), 5126, "VEC3")
+                n = rng.normal(size=(nv, 3)); attrs["NORMAL"] = b.add_accessor((n / np.linalg.norm(n, axis=1, keepdims=True)).astype(np.float32), 5126, "VEC3")
             if rng.random() < 0.5:
                 t = rng.normal(size=(nv, 3)); t /= np.linalg.norm(t, axis=1, keepdims=True)
-                attrs["TANGENT"] = add_acc(np.concatenate([t, np.where(rng.random((nv, 1)) < 0.5, -1.0, 1.0)], axis=1).astype(np.float32), 5126, "VEC4")
+                attrs["TANGENT"] = b.add_accessor(np.concatenate([t, np.where(rng.random((nv, 1)) < 0.5, -1.0, 1.0)], axis=1).astype(np.float32), 5126, "VEC4")
             if rng.random() < 0.7:
-                attrs["TEXCOORD_0"] = add_acc(rng.random((nv, 2)).astype(np.float32), 5126, "VEC2")
+                attrs["TEXCOORD_0"] = b.add_accessor(rng.random((nv, 2)).astype(np.float32), 5126, "VEC2")
             prim = {"attributes": attrs}
             kind = int(rng.integers(0, 4))
             ntri = int(rng.integers(1, 6))
             if kind < 3:
                 idx = rng.integers(0, nv, size=ntri * 3)
                 dt, ct = [(np.uint8, 5121), (np.uint16, 5123), (np.uint32, 5125)][kind]
-                prim["indices"] = add_acc(idx.astype(dt), ct, "SCALAR")
+                prim["indices"] = b.add_accessor(idx.astype(dt), ct, "SCALAR")
             elif nv % 3:   # non-indexed needs a multiple of 3 vertices, else the reference skips the primitive: keep both cases
                 if rng.random() < 0.5:
-                    prim["attributes"]["POSITION"] = add_acc(pos[: nv - nv % 3], 5126, "VEC3")
+                    prim["attributes"]["POSITION"] = b.add_accessor(pos[: nv - nv % 3], 5126, "VEC3")
                     for k in ("NORMAL", "TANGENT", "TEXCOORD_0"):
                         prim["attributes"].pop(k, None)
             if rng.random() < 0.8: prim["material"] = int(rng.integers(0, len(materials)))
@@ -470,20 +521,14 @@ def make_complex_glb(path: str, seed: int) -> None:
     roots = [add_node(1) for _ in range(int(rng.integers(1, 3)))]
     scenes = [{"nodes": roots}]
     gltf = {"asset": {"version": "2.0"}, "scenes": scenes, "nodes": nodes, "meshes": meshes, "materials": materials,
-            "textures": textures, "images": images, "bufferViews": views, "accessors": accessors}
+            "textures": textures, "images": images, "bufferViews": b.views, "accessors": b.accessors}
     if rng.random() < 0.3:
         other = add_node(1)
         gltf["scenes"] = [{"nodes": [other]}, {"nodes": roots}]
         gltf["scene"] = 1
     elif rng.random() < 0.7:
         gltf["scene"] = 0
-    binblob = b"".join(blobs)
-    gltf["buffers"] = [{"byteLength": len(binblob)}]
-    js = json.dumps(gltf).encode(); js += b" " * ((-len(js)) % 4)
-    with open(path, "wb") as f:
-        f.write(struct.pack("<4sII", b"glTF", 2, 12 + 8 + len(js) + 8 + len(binblob)))
-        f.write(struct.pack("<I4s", len(js), b"JSON")); f.write(js)
-        f.write(struct.pack("<I4s", len(binblob), b"BIN\x00")); f.write(binblob)
+    write_glb(path, gltf, b.bytes())
 
 
 # ---- viewer prepass (SURVEY 8 f-4) --------------------------------------------------------------------------------
