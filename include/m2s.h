@@ -29,9 +29,13 @@
  *     + gaussianPointShadowMappingCS.glsl
  *     + gaussianPointLightCubeMapShadowVS/PS.glsl
  *     (src/renderer/renderPasses/GaussianShadowPass.cpp:83-236)
+ *   MeshRenderPass::execute + meshRenderVS/PS.glsl              m2s_mesh_render, m2s_mesh_render_enqueue
+ *     (src/renderer/renderPasses/MeshRenderPass.cpp:8-73)
  *   GaussianRelightingPass::execute                             m2s_deferred_light, m2s_deferred_light_enqueue
  *     + gaussianSplattingDeferredVS/PS.glsl
  *     (src/renderer/renderPasses/GaussianRelightingPass.cpp:42-150)
+ *   GaussianRelightingPass::execute, split screen               m2s_deferred_light_split,
+ *     (src/renderer/renderPasses/GaussianRelightingPass.cpp:90-135) m2s_deferred_light_split_enqueue
  *   SceneManager::loadModel -> execute -> exportPly             m2s_convert_file
  *     (src/utils/SceneManager.hpp:18-20)
  *   SceneManager::loadPly + parsers::loadPlyFile                 m2s_ply_parse_header, m2s_ply_decode_enqueue,
@@ -511,7 +515,7 @@ m2s_status m2s_shadow_map(m2s_ctx* ctx, const void* d_records, uint64_t count, c
  *                       Reinhard, pow 1/2.2 — with the shader's quirks kept (DESIGN §6)
  * Required: albedo (every mode), metallic_roughness (modes 5, 6), position, normal and d_cube (mode 6); the rest may
  * be NULL.  d_cube as m2s_shadow_map writes it, with shadow_size = S.  The pow, sampling and format rules are DESIGN §2.
- * Not built: split screen and the mesh G-buffer (GaussianRelightingPass.cpp:90-135). */
+ * Split screen with the mesh G-buffer (m2s_mesh_render) is m2s_deferred_light_split below. */
 typedef struct m2s_light_params {
     uint32_t width, height;    /* renderContext.rendererResolution: 1..4096 each */
     uint32_t render_mode;      /* 0..6 */
@@ -529,6 +533,47 @@ m2s_status m2s_deferred_light_enqueue(m2s_ctx* ctx, const m2s_gbuffer* gbuffer, 
 /* Synchronous form on the context stream. */
 m2s_status m2s_deferred_light(m2s_ctx* ctx, const m2s_gbuffer* gbuffer, const float* d_cube,
                               const m2s_light_params* params, uint8_t* d_image);
+
+/* ---- the mesh G-buffer pass (SURVEY 8 row 14) and the split-screen lighting -------------------------------------------
+ * MeshRenderPass::execute (src/renderer/renderPasses/MeshRenderPass.cpp:8-73) + meshRenderVS.glsl + meshRenderPS.glsl
+ * (+ common.glsl): every triangle of every primitive (base colour alpha plays no part), primitive table order then
+ * triangle order, into the five targets of an m2s_gbuffer cleared to 0, back faces culled (counter-clockwise front faces
+ * in window space, y up: a model matrix with a negative determinant culls the other side), depth test LESS on a D24
+ * buffer cleared to 1, no blending.  gl_Position = P (V (M p)), a different association from m2s_mesh_depth's (P V) M.
+ * Targets: position (worldPos, 1), normal (encodeNormal(N), 1), albedo (colour.rgb, 1), depth (d, d, d, 1) with d =
+ * computeExponentialDepth(viewDepth, near_far), metallic_roughness (metallic, roughness, 0, 1); colour by render mode:
+ * 0, 5, 6 albedo, 1 depth, 2 encoded normal, 3 a colour per triangle from gl_PrimitiveID (restarting at 0 for each
+ * primitive), 4 (0.01, 0.005, 0).  The fixed-function choices (clipping, rasteriser, perspective-correct
+ * interpolation, the LOD from 2 x 2 quad derivatives, the sampler, the sin of mode 3, the formats) are DESIGN §2.  Row 0
+ * of every target is the bottom row.  The scene must come from m2s_scene_upload (all triangles and maps resident). */
+typedef struct m2s_mesh_render_params {
+    float world_to_view[16], view_to_clip[16], model_to_world[16];  /* column-major, as m2s_mesh_depth_params */
+    float near_far[2];                                              /* u_nearFar */
+    uint32_t width, height;                                         /* 1..4096 each */
+    uint32_t render_mode;                                           /* 0..6 */
+} m2s_mesh_render_params;
+/* Enqueue-only.  Every pixel of every non-NULL target is written exactly once, clear included; a NULL target changes
+ * nothing in the others.  max_pairs (< 2^30) is the budget of (16 x 16 tile, clipped triangle) pairs: when the triangles
+ * need more, the longest prefix of source triangles (scene order) whose pairs fit is drawn.  d_drawn (optional, device
+ * uint32) receives the prefix length, d_pairs (optional, device uint64) the pairs all triangles need.  A singular
+ * model_to_world is M2S_E_INVALID.  Scratch is stream-ordered context memory grown on `stream` (NULL = context stream);
+ * nothing is synchronised. */
+m2s_status m2s_mesh_render_enqueue(m2s_ctx* ctx, const m2s_dscene* scene, const m2s_mesh_render_params* params,
+                                   const m2s_gbuffer* gbuffer, uint64_t max_pairs, uint64_t* d_pairs, uint32_t* d_drawn,
+                                   void* stream);
+/* Synchronous form on the context stream: every triangle drawn; *pairs (optional, host) receives the pair count. */
+m2s_status m2s_mesh_render(m2s_ctx* ctx, const m2s_dscene* scene, const m2s_mesh_render_params* params,
+                           const m2s_gbuffer* gbuffer, uint64_t* pairs);
+/* The relighting pass's split screen: splitPixelX = (int)(split_position * width) (fp32 product, truncated); the columns
+ * x < splitPixelX are m2s_deferred_light of `mesh`, the others m2s_deferred_light of `splat`, with the same params and
+ * cube; then the columns [max(0, splitPixelX - 1), +2) clipped to the image are set to (255, 255, 255, 255).
+ * split_position in [0, 1].  Both G-buffers must hold what the render mode needs (as m2s_deferred_light).  Every pixel
+ * is written; nothing is synchronised by the enqueue form. */
+m2s_status m2s_deferred_light_split_enqueue(m2s_ctx* ctx, const m2s_gbuffer* splat, const m2s_gbuffer* mesh, const float* d_cube,
+                                            const m2s_light_params* params, float split_position, uint8_t* d_image,
+                                            void* stream);
+m2s_status m2s_deferred_light_split(m2s_ctx* ctx, const m2s_gbuffer* splat, const m2s_gbuffer* mesh, const float* d_cube,
+                                    const m2s_light_params* params, float split_position, uint8_t* d_image);
 
 #ifdef __cplusplus
 }

@@ -165,6 +165,21 @@ def make_mesh_depth_params(world_to_view, view_to_clip, model_to_world, width: i
     return p
 
 
+class m2s_mesh_render_params(C.Structure):
+    """include/m2s.h: the uniforms of MeshRenderPass::execute; matrices column-major (glm::mat4)."""
+    _fields_ = [("world_to_view", C.c_float * 16), ("view_to_clip", C.c_float * 16), ("model_to_world", C.c_float * 16),
+                ("near_far", C.c_float * 2), ("width", C.c_uint32), ("height", C.c_uint32), ("render_mode", C.c_uint32)]
+
+
+def make_mesh_render_params(world_to_view, view_to_clip, model_to_world, width: int, height: int, near_far, render_mode: int = 0):
+    p = m2s_mesh_render_params()
+    for name, m in (("world_to_view", world_to_view), ("view_to_clip", view_to_clip), ("model_to_world", model_to_world)):
+        setattr(p, name, (C.c_float * 16)(*[float(v) for v in np.asarray(m, np.float32).ravel()]))
+    p.near_far = (C.c_float * 2)(float(near_far[0]), float(near_far[1]))
+    p.width, p.height, p.render_mode = int(width), int(height), int(render_mode)
+    return p
+
+
 class m2s_peers(C.Structure):
     _fields_ = [("world", C.c_uint32), ("rank", C.c_uint32), ("out", C.c_void_p * MAX_PEERS), ("xch", C.c_void_p * MAX_PEERS)]
 

@@ -22,7 +22,8 @@ SYMBOLS = [
     "m2s_prepass", "m2s_prepass_enqueue", "m2s_depth_sort", "m2s_depth_sort_enqueue",
     "m2s_splat_draw", "m2s_splat_draw_enqueue", "m2s_shadow_map", "m2s_shadow_map_enqueue",
     "m2s_deferred_light", "m2s_deferred_light_enqueue", "m2s_mesh_depth", "m2s_mesh_depth_enqueue",
-    "m2s_prepass_mesh_depth", "m2s_prepass_mesh_depth_enqueue",
+    "m2s_prepass_mesh_depth", "m2s_prepass_mesh_depth_enqueue", "m2s_mesh_render", "m2s_mesh_render_enqueue",
+    "m2s_deferred_light_split", "m2s_deferred_light_split_enqueue",
     "m2s_ply_parse_header", "m2s_ply_decode_enqueue", "m2s_ply_read", "m2s_ply_h2d_bytes",
 ]
 
@@ -134,6 +135,16 @@ def lib() -> C.CDLL:
     L.m2s_prepass_mesh_depth_enqueue.argtypes = [vp, vp, u64, vp, C.POINTER(_abi.m2s_prepass_params), vp, u32, u32, vp, vp, vp, vp]
     L.m2s_prepass_mesh_depth.restype = i32
     L.m2s_prepass_mesh_depth.argtypes = [vp, vp, u64, C.POINTER(_abi.m2s_prepass_params), vp, u32, u32, vp, vp, C.POINTER(u32)]
+    L.m2s_mesh_render_enqueue.restype = i32
+    L.m2s_mesh_render_enqueue.argtypes = [vp, vp, C.POINTER(_abi.m2s_mesh_render_params), C.POINTER(_abi.m2s_gbuffer), u64, vp, vp, vp]
+    L.m2s_mesh_render.restype = i32
+    L.m2s_mesh_render.argtypes = [vp, vp, C.POINTER(_abi.m2s_mesh_render_params), C.POINTER(_abi.m2s_gbuffer), C.POINTER(u64)]
+    L.m2s_deferred_light_split_enqueue.restype = i32
+    L.m2s_deferred_light_split_enqueue.argtypes = [vp, C.POINTER(_abi.m2s_gbuffer), C.POINTER(_abi.m2s_gbuffer), vp,
+                                                   C.POINTER(_abi.m2s_light_params), C.c_float, vp, vp]
+    L.m2s_deferred_light_split.restype = i32
+    L.m2s_deferred_light_split.argtypes = [vp, C.POINTER(_abi.m2s_gbuffer), C.POINTER(_abi.m2s_gbuffer), vp,
+                                           C.POINTER(_abi.m2s_light_params), C.c_float, vp]
     L.m2s_ply_parse_header.restype = i32
     L.m2s_ply_parse_header.argtypes = [vp, C.c_size_t, u64, C.POINTER(_abi.m2s_ply_info)]
     L.m2s_ply_decode_enqueue.restype = i32

@@ -45,6 +45,31 @@ def _binned_pass(dev, max_pairs, n, draw, draw_enqueue):
     return int(o[2]), int(o[:2].view(np.uint64)[0])
 
 
+def _gbuffer(dev, width: int, height: int, targets, gbuffer):
+    """The m2s_gbuffer of the named targets, each the caller's tensor in `gbuffer` or a new one; (struct, {name: tensor})."""
+    torch = _torch()
+    gbuffer = dict(gbuffer or {})
+    g = _abi.m2s_gbuffer()
+    for name, dt in _abi.GBUFFER_TARGETS:
+        if name not in targets:
+            continue
+        if name not in gbuffer:
+            gbuffer[name] = torch.empty(width * height * 4, dtype=torch.int16 if dt == np.float16 else torch.uint8, device=dev)
+        setattr(g, name, gbuffer[name].data_ptr())
+    return g, gbuffer
+
+
+def _gbuffer_images(gbuffer: dict, width: int, height: int, targets) -> dict:
+    """The drawn targets as {name: numpy array (height, width, 4)}, float16 or uint8."""
+    torch = _torch()
+    images = {}
+    for name, dt in _abi.GBUFFER_TARGETS:
+        if name in targets:
+            raw = gbuffer[name].view(torch.uint8)[: width * height * 4 * np.dtype(dt).itemsize]
+            images[name] = raw.cpu().numpy().view(dt).reshape(height, width, 4).copy()
+    return images
+
+
 class DeviceScene:
     """Device-resident scene (triangles, primitive table, mip chains): what loadModel leaves on the
     GPU in the reference (VBOs + GL textures)."""
@@ -271,16 +296,8 @@ class Context:
         max_pairs None: m2s_splat_draw (all quads drawn).  Otherwise m2s_splat_draw_enqueue on torch's current stream with
         that pair budget, d_draw (optional int32 device tensor, the sort's draw command) limiting n.  gbuffer: optional
         {name: caller-owned device tensor of width * height * 4 elements} for the drawn targets."""
-        torch = _torch()
         dev = sorted_quads.device
-        gbuffer = dict(gbuffer or {})
-        g = _abi.m2s_gbuffer()
-        for name, dt in _abi.GBUFFER_TARGETS:
-            if name not in targets:
-                continue
-            if name not in gbuffer:
-                gbuffer[name] = torch.empty(width * height * 4, dtype=torch.int16 if dt == np.float16 else torch.uint8, device=dev)
-            setattr(g, name, gbuffer[name].data_ptr())
+        g, gbuffer = _gbuffer(dev, width, height, targets, gbuffer)
         p = _abi.m2s_splat_params(width, height, render_mode)
         drawn, npairs = _binned_pass(
             dev, max_pairs, count,
@@ -288,12 +305,7 @@ class Context:
             lambda *budget: lib().m2s_splat_draw_enqueue(self.handle, sorted_quads.data_ptr(), count,
                                                          d_draw.data_ptr() if d_draw is not None else None, C.byref(p),
                                                          C.byref(g), *budget))
-        images = {}
-        for name, dt in _abi.GBUFFER_TARGETS:
-            if name in targets:
-                raw = gbuffer[name].view(torch.uint8)[: width * height * 4 * np.dtype(dt).itemsize]
-                images[name] = raw.cpu().numpy().view(dt).reshape(height, width, 4).copy()
-        return images, drawn, npairs
+        return _gbuffer_images(gbuffer, width, height, targets), drawn, npairs
 
     def mesh_depth(self, dscene: DeviceScene, world_to_view, view_to_clip, model_to_world, width: int, height: int,
                    max_pairs: int | None = None, depth=None):
@@ -313,6 +325,24 @@ class Context:
             lambda pairs: lib().m2s_mesh_depth(self.handle, dscene.handle, C.byref(p), depth.data_ptr(), pairs),
             lambda *budget: lib().m2s_mesh_depth_enqueue(self.handle, dscene.handle, C.byref(p), depth.data_ptr(), *budget))
         return depth.reshape(-1)[: width * height].cpu().numpy().reshape(height, width).copy(), drawn, npairs
+
+    def mesh_render(self, dscene: DeviceScene, world_to_view, view_to_clip, model_to_world, width: int, height: int, near_far,
+                    render_mode: int = 0, targets=tuple(name for name, _ in _abi.GBUFFER_TARGETS), max_pairs: int | None = None,
+                    gbuffer=None):
+        """MeshRenderPass::execute on an uploaded scene: the mesh G-buffer as {target name: numpy array (height, width, 4)}
+        (float16 for position / normal / depth, uint8 for albedo / metallic_roughness, row 0 = the bottom row), plus
+        (drawn, pairs).  targets: the names to draw.  max_pairs None: m2s_mesh_render (every triangle drawn).  Otherwise
+        m2s_mesh_render_enqueue on torch's current stream with that pair budget.  gbuffer: optional {name: caller-owned
+        device tensor of width * height * 4 elements} for the drawn targets (pass them on to deferred_light_split)."""
+        torch = _torch()
+        dev = torch.device("cuda", self.device)
+        g, gbuffer = _gbuffer(dev, width, height, targets, gbuffer)
+        p = _abi.make_mesh_render_params(world_to_view, view_to_clip, model_to_world, width, height, near_far, render_mode)
+        drawn, npairs = _binned_pass(
+            dev, max_pairs, dscene.triangle_count,
+            lambda pairs: lib().m2s_mesh_render(self.handle, dscene.handle, C.byref(p), C.byref(g), pairs),
+            lambda *budget: lib().m2s_mesh_render_enqueue(self.handle, dscene.handle, C.byref(p), C.byref(g), *budget))
+        return _gbuffer_images(gbuffer, width, height, targets), drawn, npairs
 
     def shadow_map(self, records, count: int, layout: int, model_to_world, light_position, near_far, resolution, std_dev: float,
                    size: int = 1024, max_pairs: int | None = None, d_count=None, cube=None, light_quads=None):
@@ -362,6 +392,34 @@ class Context:
         else:
             torch.cuda.synchronize(dev)
             check(lib().m2s_deferred_light(self.handle, C.byref(g), cp, C.byref(p), image.data_ptr()))
+        torch.cuda.synchronize(dev)
+        return image.view(torch.uint8)[: width * height * 4].cpu().numpy().reshape(height, width, 4).copy()
+
+    def deferred_light_split(self, splat_gbuffer: dict, mesh_gbuffer: dict, cube, width: int, height: int, split_position: float,
+                             render_mode: int = 6, light_position=(0.0, 0.0, 0.0), light_color=(1.0, 1.0, 1.0),
+                             light_intensity: float = 1.0, cam_pos=(0.0, 0.0, 0.0), far_plane: float = 100.0, shadow_size: int = 1024,
+                             image=None, enqueue: bool = False):
+        """GaussianRelightingPass::execute in split screen: the mesh G-buffer lit left of int(split_position * width),
+        the splat G-buffer right of it, the two divider columns white; the RGBA8 image (height, width, 4) as numpy.
+        Everything else as deferred_light."""
+        torch = _torch()
+        dev = next(t.device for t in list(splat_gbuffer.values()) + list(mesh_gbuffer.values()) if t is not None)
+        gs, gm = _abi.m2s_gbuffer(), _abi.m2s_gbuffer()
+        for g, gb in ((gs, splat_gbuffer), (gm, mesh_gbuffer)):
+            for name, t in gb.items():
+                if t is not None:
+                    setattr(g, name, t.data_ptr())
+        if image is None:
+            image = torch.empty(width * height * 4, dtype=torch.uint8, device=dev)
+        p = _abi.make_light_params(width, height, render_mode, light_position, light_color, light_intensity, cam_pos, far_plane, shadow_size)
+        cp = cube.data_ptr() if cube is not None else None
+        if enqueue:
+            check(lib().m2s_deferred_light_split_enqueue(self.handle, C.byref(gs), C.byref(gm), cp, C.byref(p), float(split_position),
+                                                         image.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+        else:
+            torch.cuda.synchronize(dev)
+            check(lib().m2s_deferred_light_split(self.handle, C.byref(gs), C.byref(gm), cp, C.byref(p), float(split_position),
+                                                 image.data_ptr()))
         torch.cuda.synchronize(dev)
         return image.view(torch.uint8)[: width * height * 4].cpu().numpy().reshape(height, width, 4).copy()
 

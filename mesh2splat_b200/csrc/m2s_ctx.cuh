@@ -90,13 +90,14 @@ struct m2s_ctx {
     m2s::Scratch out, keys;                  // convert_host output and keys
     m2s::Scratch trifrag, items;             // between the raster and the fragment kernel: TriRec per triangle, FragItem queue
     m2s::Scratch sort;                       // depth sort: control words, alternate key and value buffers (SortLayout, m2s_sort.cuh)
-    m2s::BinScratch splat_bins, shadow_bins, depth_bins;  // the binned passes: splat draw, cube raster, mesh depth pre-pass
+    m2s::BinScratch splat_bins, shadow_bins, depth_bins, mesh_bins;  // the binned passes: splat draw, cube raster, mesh depth
+                                                                  // pre-pass, mesh G-buffer pass
     m2s::Scratch light_quads;                // shadow pass: light records when the caller passes none
     m2s::Scratch ply_rows;                   // .ply reader: two slots of one block of raw vertex rows (m2s_ply_read.cu)
     // every Scratch above (m2s_ctx_destroy frees them): a member added above is added here too
     std::vector<m2s::Scratch*> all_scratch() {
         return {&out, &keys, &trifrag, &items, &sort, &light_quads, &ply_rows, &splat_bins.bins, &splat_bins.pairs, &shadow_bins.bins,
-                &shadow_bins.pairs, &depth_bins.bins, &depth_bins.pairs};
+                &shadow_bins.pairs, &depth_bins.bins, &depth_bins.pairs, &mesh_bins.bins, &mesh_bins.pairs};
     }
     uint64_t ply_h2d = 0;                    // row bytes m2s_ply_read copied host -> device
 };

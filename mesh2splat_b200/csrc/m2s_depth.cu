@@ -14,41 +14,12 @@
 // the map is round-to-nearest fp32 / fp64 with no contraction (__f*_rn, __d*_rn), integer, or a conversion of DESIGN
 // §2, so the map equals the oracle's (oracle/m2s_depth_oracle.c) bit for bit.
 #include "m2s_bin.cuh"
+#include "m2s_clip.cuh"
 #include "m2s_depth.cuh"
 
 namespace m2s {
 
 namespace {
-__device__ __forceinline__ float ad(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ float sb(float a, float b) { return __fsub_rn(a, b); }
-__device__ __forceinline__ float ml(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ float dv(float a, float b) { return __fdiv_rn(a, b); }
-
-// GLM mat4 * vec4(x, y, z, 1): (m0 x + m1 y) + (m2 z + m3)
-__device__ __forceinline__ float depth_row(const float* m, int row, float x, float y, float z) {
-    return ad(ad(ml(m[row], x), ml(m[4 + row], y)), ad(ml(m[8 + row], z), ml(m[12 + row], 1.0f)));
-}
-
-// signed distance to clip plane p (inside iff >= 0): z >= -w, z <= w, x >= -G w, x <= G w, y >= -G w, y <= G w
-__device__ __forceinline__ float depth_plane(const float4& v, int p) {
-    const float gw = ml(kDepthGuard, v.w);
-    switch (p) {
-        case 0: return ad(v.z, v.w);
-        case 1: return sb(v.w, v.z);
-        case 2: return ad(v.x, gw);
-        case 3: return sb(gw, v.x);
-        case 4: return ad(v.y, gw);
-        default: return sb(gw, v.y);
-    }
-}
-
-// the point where edge (a inside, b outside) meets the plane, always computed from the inside vertex
-__device__ __forceinline__ float4 depth_cut(const float4& a, const float4& b, float da, float db) {
-    const float t = dv(da, sb(da, db));
-    return make_float4(ad(a.x, ml(t, sb(b.x, a.x))), ad(a.y, ml(t, sb(b.y, a.y))), ad(a.z, ml(t, sb(b.z, a.z))),
-                       ad(a.w, ml(t, sb(b.w, a.w))));
-}
-
 // triangle -> primitive (sorted, disjoint ranges); a triangle of no primitive or of a non-opaque one is not drawn
 __device__ __forceinline__ bool depth_opaque(const DepthArgs& a, uint32_t tri) {
     int lo = 0, hi = (int)a.nranges - 1;
@@ -62,80 +33,16 @@ __device__ __forceinline__ bool depth_opaque(const DepthArgs& a, uint32_t tri) {
     return false;
 }
 
-// clip-space polygon of source triangle `tri` after Sutherland-Hodgman against the six planes in order; returns its
-// vertex count (0: not drawn).  A polygon that would grow past kDepthMaxPoly vertices (only through rounding) keeps
-// its first kDepthMaxPoly.
+// clip-space polygon of source triangle `tri` (m2s_clip.cuh); returns its vertex count (0: not drawn)
 __device__ int depth_poly(const DepthArgs& a, uint32_t tri, float4 (&v)[kDepthMaxPoly]) {
     if (!depth_opaque(a, tri)) return 0;
-    bool finite = true;
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
         const float4 p = __ldg(a.tris + (size_t)tri * 9 + k * 3);
-        v[k] = make_float4(depth_row(a.pvm, 0, p.x, p.y, p.z), depth_row(a.pvm, 1, p.x, p.y, p.z),
-                           depth_row(a.pvm, 2, p.x, p.y, p.z), depth_row(a.pvm, 3, p.x, p.y, p.z));
-        finite &= isfinite(v[k].x) && isfinite(v[k].y) && isfinite(v[k].z) && isfinite(v[k].w);
+        v[k] = make_float4(clip_row(a.pvm, 0, p.x, p.y, p.z, 1.0f), clip_row(a.pvm, 1, p.x, p.y, p.z, 1.0f),
+                           clip_row(a.pvm, 2, p.x, p.y, p.z, 1.0f), clip_row(a.pvm, 3, p.x, p.y, p.z, 1.0f));
     }
-    if (!finite) return 0;
-    bool inside = true;
-#pragma unroll
-    for (int p = 0; p < 6; ++p)
-#pragma unroll
-        for (int k = 0; k < 3; ++k) inside &= depth_plane(v[k], p) >= 0.0f;
-    if (inside) return 3;
-    int n = 3;
-    for (int p = 0; p < 6 && n > 0; ++p) {
-        float4 o[kDepthMaxPoly];
-        int m = 0;
-        float dp = depth_plane(v[n - 1], p);
-        for (int i = 0; i < n; ++i) {
-            const float dc = depth_plane(v[i], p);
-            const int prev = i == 0 ? n - 1 : i - 1;
-            if (dc >= 0.0f) {
-                if (dp < 0.0f && m < kDepthMaxPoly) o[m++] = depth_cut(v[i], v[prev], dc, dp);
-                if (m < kDepthMaxPoly) o[m++] = v[i];
-            } else if (dp >= 0.0f && m < kDepthMaxPoly) {
-                o[m++] = depth_cut(v[prev], v[i], dp, dc);
-            }
-            dp = dc;
-        }
-        for (int i = 0; i < m; ++i) v[i] = o[i];
-        n = m;
-    }
-    return n;
-}
-
-struct DepthTri {
-    SplatTri t;
-    float z[3];   // window depth (z / w) 0.5 + 0.5 of the three vertices
-};
-
-// fan triangle (v0, vk+1, vk+2): perspective divide, the splat draw's viewport transform, snap and edge set-up
-__device__ __forceinline__ void depth_fan(const DepthArgs& a, const float4 (&v)[kDepthMaxPoly], int k, DepthTri& d) {
-    const float hw = ml((float)a.width, 0.5f), hh = ml((float)a.height, 0.5f);
-    int X[3], Y[3];
-    bool ok = true;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-        const float4 p = v[c == 0 ? 0 : k + c];
-        bool okc;
-        splat_snap(dv(p.x, p.w), dv(p.y, p.w), hw, hh, okc, X[c], Y[c]);
-        ok &= okc;
-        d.z[c] = ad(ml(dv(p.z, p.w), 0.5f), 0.5f);
-    }
-    splat_tri_setup(X, Y, ok, (int)a.width, (int)a.height, d.t);
-}
-
-__device__ __forceinline__ int depth_tiles_x(const DepthArgs& a) { return (int)((a.width + kSplatTile - 1) / kSplatTile); }
-
-// visits the tiles the fan triangle touches in tile-id order; returns their number
-template <typename F>
-__device__ __forceinline__ uint32_t depth_for_each_tile(const SplatTri& t, int tiles_x, F&& f) {
-    if (t.x1 < t.x0 || t.y1 < t.y0) return 0;
-    uint32_t c = 0;
-    for (int ty = t.y0 / kSplatTile; ty <= t.y1 / kSplatTile; ++ty)
-        for (int tx = t.x0 / kSplatTile; tx <= t.x1 / kSplatTile; ++tx)
-            if (splat_tri_touches(t, tx, ty)) f(c++, (uint32_t)(ty * tiles_x + tx));
-    return c;
+    return clip_poly(v);
 }
 
 }  // namespace
@@ -151,12 +58,12 @@ struct DepthBins {
     __device__ __forceinline__ uint32_t visit(uint32_t i, F&& f) const {
         float4 v[kDepthMaxPoly];
         const int np = depth_poly(a, i, v);
-        const int tx = depth_tiles_x(a);
+        const int tx = clip_tiles_x(a.width);
         uint32_t cnt = 0;
         for (int k = 0; k + 2 < np; ++k) {
             DepthTri d;
-            depth_fan(a, v, k, d);
-            cnt += depth_for_each_tile(d.t, tx, [&](uint32_t, uint32_t tile) { f(tile, i << 3 | (uint32_t)k); });
+            clip_fan<false>(v, k, a.width, a.height, d);
+            cnt += clip_for_each_tile(d.t, tx, [&](uint32_t, uint32_t tile) { f(tile, i << 3 | (uint32_t)k); });
         }
         return cnt;
     }
@@ -176,7 +83,7 @@ __device__ __noinline__ void depth_stage(const DepthArgs& a, uint32_t v, int ox,
     float4 poly[kDepthMaxPoly];
     depth_poly(a, v >> 3, poly);   // a triangle with pairs has fan triangle v & 7
     DepthTri d;
-    depth_fan(a, poly, (int)(v & 7u), d);
+    clip_fan<false>(poly, (int)(v & 7u), a.width, a.height, d);
     uint32_t incl = 0;
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
@@ -193,7 +100,7 @@ __global__ void __launch_bounds__(kSplatThreads) depth_tile_kernel(const __grid_
     __shared__ DepthStage s;
     const BinLayout l = bin_layout(a.ntri, splat_tiles(a.width, a.height));
     const uint32_t* start = reinterpret_cast<const uint32_t*>(a.scratch + l.ranges_off);
-    const uint32_t tile = blockIdx.x, tx = (uint32_t)depth_tiles_x(a);
+    const uint32_t tile = blockIdx.x, tx = (uint32_t)clip_tiles_x(a.width);
     const int ox = (int)(tile % tx) * kSplatTile, oy = (int)(tile / tx) * kSplatTile;
     const int tid = threadIdx.x, lx = tid % kSplatTile, ly = tid / kSplatTile;
     const int x = ox + lx, y = oy + ly;

@@ -301,8 +301,10 @@ __device__ __forceinline__ uint32_t light_u8(float v) { return __float2uint_rn(m
 __device__ __forceinline__ float light_unorm(uint32_t c) { return dv((float)c, 255.0f); }
 
 __global__ void __launch_bounds__(kLightThreads) deferred_light_kernel(const __grid_constant__ LightArgs a) {
-    const uint64_t px = (uint64_t)blockIdx.x * kLightThreads + threadIdx.x;
-    if (px >= (uint64_t)a.width * a.height) return;
+    const uint64_t i = (uint64_t)blockIdx.x * kLightThreads + threadIdx.x;
+    const uint32_t cols = a.x1 - a.x0;
+    if (i >= (uint64_t)cols * a.height) return;
+    const uint64_t px = cols == a.width ? i : (i / cols) * a.width + a.x0 + i % cols;   // pixel i of the column range
     const uint32_t ab = __ldg(reinterpret_cast<const uint32_t*>(a.albedo) + px);
     float out[3];
     if (a.mode == 5) {   // gaussianSplattingDeferredPS.glsl:105-109
@@ -409,7 +411,8 @@ cudaError_t shadow_draw_launch(const ShadowArgs& a, int sm_count, cudaStream_t s
 }
 
 cudaError_t deferred_light_launch(const LightArgs& a, cudaStream_t stream) {
-    const uint64_t n = (uint64_t)a.width * a.height;
+    const uint64_t n = (uint64_t)(a.x1 - a.x0) * a.height;
+    if (n == 0) return cudaSuccess;
     deferred_light_kernel<<<(unsigned)((n + kLightThreads - 1) / kLightThreads), kLightThreads, 0, stream>>>(a);
     return cudaGetLastError();
 }

@@ -66,6 +66,7 @@ struct LightArgs {
     uint32_t width, height, mode, shadow_size;
     float light[3], light_color[3], light_intensity, cam[3], far_plane;
     uint8_t* image;                 // width x height x 4, row 0 = the bottom row
+    uint32_t x0, x1;                // the columns [x0, x1) are lit (m2s_deferred_light: [0, width); split screen: one side)
 };
 
 cudaError_t deferred_light_launch(const LightArgs& a, cudaStream_t stream);

@@ -12,8 +12,6 @@
 //                         every blend), one coalesced store per live target
 // All arithmetic that decides a bit of the image is round-to-nearest fp32 with no contraction (__f*_rn), integer, or
 // the conversions to the target formats, so the image equals the oracle's (oracle/m2s_splat_oracle.c) bit for bit.
-#include <cuda_fp16.h>
-
 #include "m2s_bin.cuh"
 #include "m2s_splat.cuh"
 
@@ -41,14 +39,6 @@ struct SplatBins {
 
 // ---- fragment shader, blend, formats -------------------------------------------------------------------------------
 
-// fp32 -> fp16 bits, round to nearest even; overflow gives +-inf, NaN gives 0x7FFF, subnormals are kept
-__device__ __forceinline__ float splat_to_half(float v, uint16_t& bits) {
-    if (v != v) { bits = 0x7FFFu; return v; }
-    const __half h = __float2half_rn(v);
-    bits = __half_as_ushort(h);
-    return __half2float(h);
-}
-
 // RGBA16F: dst = src * f + dst in fp32, then one conversion to half.  dst holds the channel's half value as a float.
 __device__ __forceinline__ void splat_blend_f16(float (&dst)[4], const float (&src)[4], bool additive) {
     const float f = additive ? 1.0f : __fsub_rn(1.0f, dst[3]);
@@ -56,8 +46,6 @@ __device__ __forceinline__ void splat_blend_f16(float (&dst)[4], const float (&s
 #pragma unroll
     for (int c = 0; c < 4; ++c) dst[c] = splat_to_half(__fadd_rn(__fmul_rn(src[c], f), dst[c]), b);
 }
-
-__device__ __forceinline__ float splat_sat(float v) { return fminf(fmaxf(v, 0.0f), 1.0f); }
 
 // RGBA8: dst = d / 255; src, f and the result clamped to [0, 1]; stored as round-half-even(result * 255)
 __device__ __forceinline__ void splat_blend_u8(uint32_t (&dst)[4], const float (&src)[4], bool additive) {

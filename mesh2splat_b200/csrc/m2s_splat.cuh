@@ -3,6 +3,7 @@
 #pragma once
 #include <cstddef>
 #include <cstdint>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
 namespace m2s {
@@ -126,6 +127,18 @@ __device__ __forceinline__ uint32_t splat_for_each_tile(const SplatTri t[2], int
             if (splat_tri_touches(t[0], tx, ty) || splat_tri_touches(t[1], tx, ty)) f(c++, (uint32_t)(ty * tiles_x + tx));
     return c;
 }
+
+// ---- the G-buffer formats (DESIGN §2), shared with the mesh G-buffer pass (m2s_mesh.cu) ------------------------------
+// fp32 -> fp16 bits, round to nearest even; overflow gives +-inf, NaN gives 0x7FFF, subnormals are kept
+__device__ __forceinline__ float splat_to_half(float v, uint16_t& bits) {
+    if (v != v) { bits = 0x7FFFu; return v; }
+    const __half h = __float2half_rn(v);
+    bits = __half_as_ushort(h);
+    return __half2float(h);
+}
+
+// RGBA8 channels are clamped to [0, 1] and stored as round-half-even(v * 255); NaN clamps to 0
+__device__ __forceinline__ float splat_sat(float v) { return fminf(fmaxf(v, 0.0f), 1.0f); }
 
 // exp(x) from round-to-nearest fp32 operations only (the same steps as the oracle's orc_splat_exp): x = k ln2 + r with a
 // two-part ln2 (Cody-Waite), a degree-7 polynomial for e^r, then 2^k applied in two exact-or-once-rounded multiplies.

@@ -1,11 +1,13 @@
 // m2s_viewer.cu — C-ABI implementation (include/m2s.h): the viewer's passes.  Prepass, depth sort, splat draw, shadow
-// map, deferred lighting and mesh depth pre-pass: argument checks, the uniforms built on the host, and the launches.
+// map, deferred lighting (and its split screen), mesh depth pre-pass and mesh G-buffer pass: argument checks, the
+// uniforms built on the host, and the launches.
 #include <cmath>
 
 #include "m2s_bin.cuh"
 #include "m2s_ctx.cuh"
 #include "m2s_depth.cuh"
 #include "m2s_light.cuh"
+#include "m2s_mesh.cuh"
 #include "m2s_prepass.cuh"
 #include "m2s_sort.cuh"
 #include "m2s_splat.cuh"
@@ -413,21 +415,23 @@ M2S_EXPORT m2s_status m2s_shadow_map(m2s_ctx* ctx, const void* d_records, uint64
 }
 
 // ---- the viewer's deferred lighting (SURVEY 8 f-8): GaussianRelightingPass::execute + gaussianSplattingDeferredPS.glsl
-M2S_EXPORT m2s_status m2s_deferred_light_enqueue(m2s_ctx* ctx, const m2s_gbuffer* g, const float* d_cube, const m2s_light_params* p,
-                                                 uint8_t* d_image, void* stream_) {
-    const char* fn = "m2s_deferred_light";
-    if (!ctx || !g || !p || !d_image) return invalid(fn, "NULL argument");
-    if (!sizes_ok(fn, "width and height", kSplatMaxSide, {p->width, p->height})) return M2S_E_INVALID;
-    if (p->render_mode > 6) return invalid(fn, "render modes 0..6 only");
+// the checks of one G-buffer (and the image and cube) against the render mode
+static bool light_gbuffer_ok(const char* fn, const m2s_gbuffer* g, const float* d_cube, const m2s_light_params* p, const uint8_t* d_image) {
     const bool lit = p->render_mode == 6;
-    if (!g->albedo || ((p->render_mode == 5 || lit) && !g->metallic_roughness) || (lit && (!g->position || !g->normal || !d_cube)))
-        return invalid(fn, "NULL target or cube the render mode needs");
-    if ((lit && !sizes_ok(fn, "shadow_size", kShadowMaxSize, {p->shadow_size})) ||
-        !aligned_ok(fn, "RGBA16F targets must be 8-byte aligned, RGBA8 targets, the image and the cube 4-byte aligned",
-                    {{g->position, 8}, {g->normal, 8}, {g->albedo, 4}, {g->metallic_roughness, 4}, {d_image, 4}, {d_cube, 4}}))
-        return M2S_E_INVALID;
-    CUDA_TRY(cudaSetDevice(ctx->device));
-    LightArgs a;
+    if (!g->albedo || ((p->render_mode == 5 || lit) && !g->metallic_roughness) || (lit && (!g->position || !g->normal || !d_cube))) {
+        invalid(fn, "NULL target or cube the render mode needs");
+        return false;
+    }
+    return aligned_ok(fn, "RGBA16F targets must be 8-byte aligned, RGBA8 targets, the image and the cube 4-byte aligned",
+                      {{g->position, 8}, {g->normal, 8}, {g->albedo, 4}, {g->metallic_roughness, 4}, {d_image, 4}, {d_cube, 4}});
+}
+
+// the checks every lighting entry point makes, then the uniforms; the columns [0, width) and the G-buffer g
+static bool light_args(const char* fn, const m2s_gbuffer* g, const float* d_cube, const m2s_light_params* p, uint8_t* d_image, LightArgs& a) {
+    if (!sizes_ok(fn, "width and height", kSplatMaxSide, {p->width, p->height})) return false;
+    if (p->render_mode > 6) { invalid(fn, "render modes 0..6 only"); return false; }
+    if (!light_gbuffer_ok(fn, g, d_cube, p, d_image) || (p->render_mode == 6 && !sizes_ok(fn, "shadow_size", kShadowMaxSize, {p->shadow_size})))
+        return false;
     std::memset(&a, 0, sizeof(a));
     a.position = g->position; a.normal = g->normal; a.albedo = g->albedo; a.metallic_roughness = g->metallic_roughness;
     a.cube = d_cube;
@@ -435,6 +439,17 @@ M2S_EXPORT m2s_status m2s_deferred_light_enqueue(m2s_ctx* ctx, const m2s_gbuffer
     for (int k = 0; k < 3; ++k) { a.light[k] = p->light_position[k]; a.light_color[k] = p->light_color[k]; a.cam[k] = p->cam_pos[k]; }
     a.light_intensity = p->light_intensity; a.far_plane = p->far_plane;
     a.image = d_image;
+    a.x0 = 0; a.x1 = p->width;
+    return true;
+}
+
+M2S_EXPORT m2s_status m2s_deferred_light_enqueue(m2s_ctx* ctx, const m2s_gbuffer* g, const float* d_cube, const m2s_light_params* p,
+                                                 uint8_t* d_image, void* stream_) {
+    const char* fn = "m2s_deferred_light";
+    if (!ctx || !g || !p || !d_image) return invalid(fn, "NULL argument");
+    LightArgs a;
+    if (!light_args(fn, g, d_cube, p, d_image, a)) return M2S_E_INVALID;
+    CUDA_TRY(cudaSetDevice(ctx->device));
     CUDA_TRY(deferred_light_launch(a, pick_stream(ctx, stream_)));
     return M2S_OK;
 }
@@ -491,4 +506,105 @@ M2S_EXPORT m2s_status m2s_mesh_depth_enqueue(m2s_ctx* ctx, const m2s_dscene* sce
 
 M2S_EXPORT m2s_status m2s_mesh_depth(m2s_ctx* ctx, const m2s_dscene* scene, const m2s_mesh_depth_params* p, float* d_depth, uint64_t* pairs) {
     return mesh_depth_pass(ctx, scene, p, d_depth, nullptr, true, 0, pairs, nullptr);
+}
+
+// ---- the viewer's mesh G-buffer pass (SURVEY 8 row 14): MeshRenderPass::execute + meshRenderVS/PS.glsl ----------------
+// mat3(transpose(inverse(M))) with GLM 1.0.1's fp32 compute_inverse<4, 4>, m[c][r] = M[4c + r]; false for a singular M
+static bool glm_normal_matrix(const float* M, float N[9]) {
+    auto m = [M](int c, int r) { return M[4 * c + r]; };
+    const float c00 = m(2, 2) * m(3, 3) - m(3, 2) * m(2, 3), c02 = m(1, 2) * m(3, 3) - m(3, 2) * m(1, 3), c03 = m(1, 2) * m(2, 3) - m(2, 2) * m(1, 3);
+    const float c04 = m(2, 1) * m(3, 3) - m(3, 1) * m(2, 3), c06 = m(1, 1) * m(3, 3) - m(3, 1) * m(1, 3), c07 = m(1, 1) * m(2, 3) - m(2, 1) * m(1, 3);
+    const float c08 = m(2, 1) * m(3, 2) - m(3, 1) * m(2, 2), c10 = m(1, 1) * m(3, 2) - m(3, 1) * m(1, 2), c11 = m(1, 1) * m(2, 2) - m(2, 1) * m(1, 2);
+    const float c12 = m(2, 0) * m(3, 3) - m(3, 0) * m(2, 3), c14 = m(1, 0) * m(3, 3) - m(3, 0) * m(1, 3), c15 = m(1, 0) * m(2, 3) - m(2, 0) * m(1, 3);
+    const float c16 = m(2, 0) * m(3, 2) - m(3, 0) * m(2, 2), c18 = m(1, 0) * m(3, 2) - m(3, 0) * m(1, 2), c19 = m(1, 0) * m(2, 2) - m(2, 0) * m(1, 2);
+    const float c20 = m(2, 0) * m(3, 1) - m(3, 0) * m(2, 1), c22 = m(1, 0) * m(3, 1) - m(3, 0) * m(1, 1), c23 = m(1, 0) * m(2, 1) - m(2, 0) * m(1, 1);
+    const float f0[4] = {c00, c00, c02, c03}, f1[4] = {c04, c04, c06, c07}, f2[4] = {c08, c08, c10, c11};
+    const float f3[4] = {c12, c12, c14, c15}, f4[4] = {c16, c16, c18, c19}, f5[4] = {c20, c20, c22, c23};
+    float v0[4], v1[4], v2[4], v3[4], inv[4][4];
+    for (int i = 0; i < 4; ++i) {
+        const int c = i == 0 ? 1 : 0;
+        v0[i] = m(c, 0); v1[i] = m(c, 1); v2[i] = m(c, 2); v3[i] = m(c, 3);
+    }
+    const float sa[4] = {1, -1, 1, -1}, sbn[4] = {-1, 1, -1, 1};
+    for (int i = 0; i < 4; ++i) {
+        inv[0][i] = (v1[i] * f0[i] - v2[i] * f1[i] + v3[i] * f2[i]) * sa[i];
+        inv[1][i] = (v0[i] * f0[i] - v2[i] * f3[i] + v3[i] * f4[i]) * sbn[i];
+        inv[2][i] = (v0[i] * f1[i] - v1[i] * f3[i] + v3[i] * f5[i]) * sa[i];
+        inv[3][i] = (v0[i] * f2[i] - v1[i] * f4[i] + v2[i] * f5[i]) * sbn[i];
+    }
+    const float d0 = m(0, 0) * inv[0][0], d1 = m(0, 1) * inv[1][0], d2 = m(0, 2) * inv[2][0], d3 = m(0, 3) * inv[3][0];
+    const float det = (d0 + d1) + (d2 + d3);
+    if (det == 0.0f || !std::isfinite(det)) return false;
+    const float ood = 1.0f / det;
+    for (int c = 0; c < 3; ++c)
+        for (int r = 0; r < 3; ++r) N[c * 3 + r] = inv[r][c] * ood;   // transpose, upper 3 x 3
+    return true;
+}
+
+// both forms of the mesh G-buffer pass: the argument checks, the arguments, then bin_pass
+static m2s_status mesh_render_pass(m2s_ctx* ctx, const m2s_dscene* scene, const m2s_mesh_render_params* p, const m2s_gbuffer* g, void* stream,
+                                   bool sync, uint64_t max_pairs, uint64_t* pairs, uint32_t* d_drawn) {
+    const char* fn = "m2s_mesh_render";
+    if (!ctx || !scene || !p || !g) return invalid(fn, "NULL argument");
+    if (!sizes_ok(fn, "width and height", kSplatMaxSide, {p->width, p->height})) return M2S_E_INVALID;
+    if (p->render_mode > 6) return invalid(fn, "render modes 0..6 only");
+    if (!g->position && !g->normal && !g->albedo && !g->depth && !g->metallic_roughness) return invalid(fn, "no targets");
+    if (!aligned_ok(fn, "RGBA16F targets must be 8-byte aligned, RGBA8 targets 4-byte aligned",
+                    {{g->position, 8}, {g->normal, 8}, {g->depth, 8}, {g->albedo, 4}, {g->metallic_roughness, 4}}))
+        return M2S_E_INVALID;
+    if (scene->ntri >= kDepthMaxTris) return invalid(fn, "too many triangles (< 2^29 supported)");
+    if (!pair_budget_ok(fn, max_pairs)) return M2S_E_INVALID;
+    MeshArgs a;
+    std::memset(&a, 0, sizeof(a));
+    if (!glm_normal_matrix(p->model_to_world, a.N)) return invalid(fn, "model_to_world is singular");
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    std::memcpy(a.M, p->model_to_world, 64); std::memcpy(a.V, p->world_to_view, 64); std::memcpy(a.P, p->view_to_clip, 64);
+    a.near_far[0] = p->near_far[0]; a.near_far[1] = p->near_far[1];
+    a.tris = scene->d_tris; a.ntri = scene->ntri;
+    a.ranges = scene->d_ranges; a.nranges = scene->nranges; a.prims = scene->d_prims;
+    a.texs = scene->d_texs; a.arena = scene->d_arena;
+    a.width = p->width; a.height = p->height; a.mode = p->render_mode;
+    a.position = g->position; a.normal = g->normal; a.albedo = g->albedo; a.depth = g->depth; a.metallic_roughness = g->metallic_roughness;
+    return bin_pass(ctx, ctx->mesh_bins, bin_layout(a.ntri, splat_tiles(a.width, a.height)).total_bytes, a, mesh_count_launch,
+                    mesh_draw_launch, pick_stream(ctx, stream), sync, max_pairs, pairs, d_drawn,
+                    "m2s_mesh_render: the triangles need 2^30 or more (tile, triangle) pairs");
+}
+
+M2S_EXPORT m2s_status m2s_mesh_render_enqueue(m2s_ctx* ctx, const m2s_dscene* scene, const m2s_mesh_render_params* p, const m2s_gbuffer* g,
+                                              uint64_t max_pairs, uint64_t* d_pairs, uint32_t* d_drawn, void* stream_) {
+    return mesh_render_pass(ctx, scene, p, g, stream_, false, max_pairs, d_pairs, d_drawn);
+}
+
+M2S_EXPORT m2s_status m2s_mesh_render(m2s_ctx* ctx, const m2s_dscene* scene, const m2s_mesh_render_params* p, const m2s_gbuffer* g,
+                                      uint64_t* pairs) {
+    return mesh_render_pass(ctx, scene, p, g, nullptr, true, 0, pairs, nullptr);
+}
+
+// ---- split screen (GaussianRelightingPass.cpp:90-135): the mesh G-buffer left of splitPixelX, the splats right of it,
+// the same shader and uniforms, then the two divider columns cleared to white
+M2S_EXPORT m2s_status m2s_deferred_light_split_enqueue(m2s_ctx* ctx, const m2s_gbuffer* splat, const m2s_gbuffer* mesh, const float* d_cube,
+                                                       const m2s_light_params* p, float split_position, uint8_t* d_image, void* stream_) {
+    const char* fn = "m2s_deferred_light_split";
+    if (!ctx || !splat || !mesh || !p || !d_image) return invalid(fn, "NULL argument");
+    if (!(split_position >= 0.0f && split_position <= 1.0f)) return invalid(fn, "split_position must be in [0, 1]");
+    LightArgs right, left;
+    if (!light_args(fn, splat, d_cube, p, d_image, right) || !light_args(fn, mesh, d_cube, p, d_image, left)) return M2S_E_INVALID;
+    const uint32_t w = p->width, split = (uint32_t)(int)(split_position * (float)(int)w);   // int(position * w), fp32 product
+    left.x1 = split;
+    right.x0 = split;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    cudaStream_t stream = pick_stream(ctx, stream_);
+    CUDA_TRY(deferred_light_launch(right, stream));
+    CUDA_TRY(deferred_light_launch(left, stream));
+    const uint32_t x0 = split > 0 ? split - 1 : 0, x1 = std::min(w, x0 + 2);   // glScissor(max(0, split - 1), 0, 2, h)
+    CUDA_TRY(cudaMemset2DAsync(d_image + (size_t)x0 * 4, (size_t)w * 4, 0xFF, (size_t)(x1 - x0) * 4, p->height, stream));
+    return M2S_OK;
+}
+
+M2S_EXPORT m2s_status m2s_deferred_light_split(m2s_ctx* ctx, const m2s_gbuffer* splat, const m2s_gbuffer* mesh, const float* d_cube,
+                                               const m2s_light_params* p, float split_position, uint8_t* d_image) {
+    m2s_status st = m2s_deferred_light_split_enqueue(ctx, splat, mesh, d_cube, p, split_position, d_image, nullptr);
+    if (st != M2S_OK) return st;
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return M2S_OK;
 }
