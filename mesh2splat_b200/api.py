@@ -59,6 +59,15 @@ def _gbuffer(dev, width: int, height: int, targets, gbuffer):
     return g, gbuffer
 
 
+def _gbuffer_of(tensors: dict):
+    """The m2s_gbuffer of {target name: device tensor or None}."""
+    g = _abi.m2s_gbuffer()
+    for name, t in tensors.items():
+        if t is not None:
+            setattr(g, name, t.data_ptr())
+    return g
+
+
 def _gbuffer_images(gbuffer: dict, width: int, height: int, targets) -> dict:
     """The drawn targets as {name: numpy array (height, width, 4)}, float16 or uint8."""
     torch = _torch()
@@ -376,24 +385,9 @@ class Context:
         cube: device float32 tensor of 6 S^2 values or None (modes 0-5).  enqueue: m2s_deferred_light_enqueue on torch's
         current stream instead of the synchronous m2s_deferred_light.  image: optional caller-owned device tensor of
         width * height * 4 bytes."""
-        torch = _torch()
-        dev = next((t.device for t in gbuffer.values() if t is not None), cube.device if cube is not None else None)
-        g = _abi.m2s_gbuffer()
-        for name, t in gbuffer.items():
-            if t is not None:
-                setattr(g, name, t.data_ptr())
-        if image is None:
-            image = torch.empty(width * height * 4, dtype=torch.uint8, device=dev)
-        p = _abi.make_light_params(width, height, render_mode, light_position, light_color, light_intensity, cam_pos, far_plane, shadow_size)
-        cp = cube.data_ptr() if cube is not None else None
-        if enqueue:
-            check(lib().m2s_deferred_light_enqueue(self.handle, C.byref(g), cp, C.byref(p), image.data_ptr(),
-                                                   torch.cuda.current_stream(dev).cuda_stream))
-        else:
-            torch.cuda.synchronize(dev)
-            check(lib().m2s_deferred_light(self.handle, C.byref(g), cp, C.byref(p), image.data_ptr()))
-        torch.cuda.synchronize(dev)
-        return image.view(torch.uint8)[: width * height * 4].cpu().numpy().reshape(height, width, 4).copy()
+        return self._light((gbuffer,), cube, width, height, image, enqueue, lib().m2s_deferred_light_enqueue, lib().m2s_deferred_light,
+                           _abi.make_light_params(width, height, render_mode, light_position, light_color, light_intensity, cam_pos,
+                                                  far_plane, shadow_size))
 
     def deferred_light_split(self, splat_gbuffer: dict, mesh_gbuffer: dict, cube, width: int, height: int, split_position: float,
                              render_mode: int = 6, light_position=(0.0, 0.0, 0.0), light_color=(1.0, 1.0, 1.0),
@@ -402,24 +396,25 @@ class Context:
         """GaussianRelightingPass::execute in split screen: the mesh G-buffer lit left of int(split_position * width),
         the splat G-buffer right of it, the two divider columns white; the RGBA8 image (height, width, 4) as numpy.
         Everything else as deferred_light."""
+        return self._light((splat_gbuffer, mesh_gbuffer), cube, width, height, image, enqueue, lib().m2s_deferred_light_split_enqueue,
+                           lib().m2s_deferred_light_split,
+                           _abi.make_light_params(width, height, render_mode, light_position, light_color, light_intensity, cam_pos,
+                                                  far_plane, shadow_size), float(split_position))
+
+    def _light(self, gbuffers, cube, width, height, image, enqueue, light_enqueue, light, params, *extra):
+        """Both lighting calls: light(ctx, *gbuffers, cube, params, *extra, image), or light_enqueue with torch's current
+        stream appended; the image read back as numpy."""
         torch = _torch()
-        dev = next(t.device for t in list(splat_gbuffer.values()) + list(mesh_gbuffer.values()) if t is not None)
-        gs, gm = _abi.m2s_gbuffer(), _abi.m2s_gbuffer()
-        for g, gb in ((gs, splat_gbuffer), (gm, mesh_gbuffer)):
-            for name, t in gb.items():
-                if t is not None:
-                    setattr(g, name, t.data_ptr())
+        dev = next((t.device for gb in gbuffers for t in gb.values() if t is not None), cube.device if cube is not None else None)
         if image is None:
             image = torch.empty(width * height * 4, dtype=torch.uint8, device=dev)
-        p = _abi.make_light_params(width, height, render_mode, light_position, light_color, light_intensity, cam_pos, far_plane, shadow_size)
-        cp = cube.data_ptr() if cube is not None else None
+        args = (self.handle, *(C.byref(_gbuffer_of(gb)) for gb in gbuffers), cube.data_ptr() if cube is not None else None, C.byref(params),
+                *extra, image.data_ptr())
         if enqueue:
-            check(lib().m2s_deferred_light_split_enqueue(self.handle, C.byref(gs), C.byref(gm), cp, C.byref(p), float(split_position),
-                                                         image.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+            check(light_enqueue(*args, torch.cuda.current_stream(dev).cuda_stream))
         else:
             torch.cuda.synchronize(dev)
-            check(lib().m2s_deferred_light_split(self.handle, C.byref(gs), C.byref(gm), cp, C.byref(p), float(split_position),
-                                                 image.data_ptr()))
+            check(light(*args))
         torch.cuda.synchronize(dev)
         return image.view(torch.uint8)[: width * height * 4].cpu().numpy().reshape(height, width, 4).copy()
 

@@ -1,6 +1,7 @@
 // m2s_bin.cuh — the tile binning of the viewer's tiled rasterisers: the splat draw (m2s_splat.cu), the shadow pass's
-// cube raster (m2s_light.cu) and the mesh depth pre-pass (m2s_depth.cu).  Each pass bins its items (quads, light
-// records, source triangles) into 16 x 16 tiles and then runs its own tile kernel over each tile's run of pairs:
+// cube raster (m2s_light.cu), the mesh depth pre-pass (m2s_depth.cu) and the mesh G-buffer pass (m2s_mesh.cu).  Each
+// pass bins its items (quads, light records, source triangles) into 16 x 16 tiles and then runs its own tile kernel
+// over each tile's run of pairs (bin_draw_launch, in the frame of tile_frame and tile_batches):
 //   bin_count_kernel     per item: the number of its (tile, value) pairs, scanned within the block of kBinBlock items
 //   bin_scan_kernel      one CTA: exclusive prefix over the block sums; the total number of pairs
 //   bin_emit_kernel      per item of the longest prefix whose pairs fit the budget: its pairs at its scan offset, so the
@@ -22,6 +23,7 @@
 #include <cuda_runtime.h>
 
 #include "m2s_sort.cuh"
+#include "m2s_tile.cuh"
 
 namespace m2s {
 
@@ -153,6 +155,45 @@ __global__ void bin_ranges_kernel(B b, const uint32_t* keys) {
     }
 }
 
+// ---- the tile kernels' frame -----------------------------------------------------------------------------------------
+// one CTA of kTileThreads threads per tile: the tile's pixel origin, the thread's pixel in the tile and in the
+// viewport, and the tile's run [r0, r1) of the sorted pair values (empty without a budget: bin_pairs_launch zeroes the
+// ranges on every call)
+struct TileFrame {
+    int ox, oy, lx, ly, x, y;
+    uint32_t r0, r1;
+};
+
+// the CTA of ranges entry blockIdx.x (scratch laid out as l), which is tile `tile` of a viewport tiles_x tiles wide
+// (the same tile but for the cube raster, whose six faces share one ranges array)
+__device__ __forceinline__ TileFrame tile_frame(const unsigned char* scratch, const BinLayout& l, uint32_t tiles_x, uint32_t tile) {
+    const uint32_t* start = reinterpret_cast<const uint32_t*>(scratch + l.ranges_off);
+    TileFrame f;
+    f.ox = (int)(tile % tiles_x) * kTile;
+    f.oy = (int)(tile / tiles_x) * kTile;
+    f.lx = (int)threadIdx.x % kTile;
+    f.ly = (int)threadIdx.x / kTile;
+    f.x = f.ox + f.lx;
+    f.y = f.oy + f.ly;
+    f.r0 = start[blockIdx.x];
+    f.r1 = start[l.tiles + blockIdx.x];
+    return f;
+}
+
+// the tile's pairs in batches of kTileThreads: thread `slot` calls stage(slot, value) for pair `slot` of the batch, then
+// every thread calls test(j) for each staged slot j in pair order
+template <typename Stage, typename Test>
+__device__ __forceinline__ void tile_batches(const TileFrame& f, const uint32_t* __restrict__ vals, Stage&& stage, Test&& test) {
+    const int tid = threadIdx.x;
+    for (uint32_t base = f.r0; base < f.r1; base += kTileThreads) {
+        const uint32_t nb = min(f.r1 - base, (uint32_t)kTileThreads);
+        __syncthreads();
+        if ((uint32_t)tid < nb) stage(tid, vals[base + tid]);
+        __syncthreads();
+        for (uint32_t j = 0; j < nb; ++j) test(j);
+    }
+}
+
 // ---- launches ------------------------------------------------------------------------------------------------------
 // the pair values in tile order once bin_pairs_launch has run (the tile kernel's input); NULL without a budget
 template <typename B>
@@ -187,6 +228,15 @@ cudaError_t bin_pairs_launch(const B& b, int sm_count, cudaStream_t stream) {
         const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((max_pairs + 255) / 256, 8ull * sm_count));
         bin_ranges_kernel<B><<<grid, 256, 0, stream>>>(b, keys);
     }
+    return cudaGetLastError();
+}
+
+// bin_pairs_launch, then the pass's tile kernel, one CTA per tile, over the pair values in tile order
+template <typename B>
+cudaError_t bin_draw_launch(const B& b, void (*tile_kernel)(decltype(b.a), const uint32_t*), int sm_count, cudaStream_t stream) {
+    const cudaError_t e = bin_pairs_launch(b, sm_count, stream);
+    if (e != cudaSuccess) return e;
+    tile_kernel<<<(unsigned)b.tiles(), kTileThreads, 0, stream>>>(b.a, bin_vals(b));
     return cudaGetLastError();
 }
 

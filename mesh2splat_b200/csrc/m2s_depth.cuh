@@ -6,14 +6,11 @@
 #include <cuda_runtime.h>
 
 #include "m2s_device.cuh"
-#include "m2s_splat.cuh"
+#include "m2s_tile.cuh"
 
 namespace m2s {
 
 constexpr uint64_t kDepthMaxTris = 1ull << 29;     // pair value = source triangle << 3 | fan triangle
-constexpr int kDepthMaxPoly = 9;                    // a triangle clipped by six planes keeps at most 3 + 6 vertices
-constexpr float kDepthGuard = 2.0f;                 // x, y clipped to +-G w: |xw| <= 1.5 * 4096 < 8192 (DESIGN §2)
-constexpr uint32_t kDepthClearCode = 0xFFFFFFu;     // D24 clear value 1.0 = 2^24 - 1
 
 // Scratch: bin_layout (m2s_bin.cuh) with one pair count per SOURCE triangle, W x H pixels.
 struct DepthArgs {
@@ -25,8 +22,8 @@ struct DepthArgs {
     float pvm[16];                  // (P V) M, column-major, GLM's mat4 * mat4 in fp32
     uint32_t width, height;
     float* depth;                   // W x H floats: (float)code / 16777215, row 0 = window y 0
-    unsigned long long max_pairs;   // (tile, fan triangle) pair budget (< kSplatMaxPairs)
-    unsigned char* scratch;         // bin_layout(ntri, splat_tiles(width, height))
+    unsigned long long max_pairs;   // (tile, fan triangle) pair budget (< kTileMaxPairs)
+    unsigned char* scratch;         // bin_layout(ntri, tile_count(width, height))
     uint32_t* pairs;                // SortLayout(max_pairs) words (m2s_sort.cuh)
 };
 

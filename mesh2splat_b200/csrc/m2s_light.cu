@@ -20,14 +20,11 @@
 #include <cuda_fp16.h>
 
 #include "m2s_bin.cuh"
+#include "m2s_clip.cuh"
 #include "m2s_light.cuh"
 
 namespace m2s {
 
-__device__ __forceinline__ float ad(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ float sb(float a, float b) { return __fsub_rn(a, b); }
-__device__ __forceinline__ float ml(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ float dv(float a, float b) { return __fdiv_rn(a, b); }
 __device__ __forceinline__ float dot3(float x, float y, float z) { return ad(ad(ml(x, x), ml(y, y)), ml(z, z)); }   // GLM dot(v, v)
 
 // GLM mat3 * mat3, column-major: r[c][row] = (a[0][row] b[c][0] + a[1][row] b[c][1]) + a[2][row] b[c][2]
@@ -37,11 +34,6 @@ __device__ __forceinline__ void light_m3mul(const float* a, const float* b, floa
 #pragma unroll
         for (int row = 0; row < 3; ++row)
             r[c * 3 + row] = ad(ad(ml(a[row], b[c * 3]), ml(a[3 + row], b[c * 3 + 1])), ml(a[6 + row], b[c * 3 + 2]));
-}
-
-// GLM mat4 * vec4(x, y, z, 1): (m0 x + m1 y) + (m2 z + m3 1)
-__device__ __forceinline__ float light_m4row(const float* m, int row, float x, float y, float z, float w) {
-    return ad(ad(ml(m[row], x), ml(m[4 + row], y)), ad(ml(m[8 + row], z), ml(m[12 + row], w)));
 }
 
 // determineFaceIndex (gaussianPointShadowMappingCS.glsl:58-69) and the cube sampler's major axis (DESIGN §2): x wins
@@ -68,19 +60,19 @@ __global__ void __launch_bounds__(kLightPrepassThreads) light_prepass_kernel(con
         const float2* g = reinterpret_cast<const float2*>(a.records + gid * 56ull);
         const float2 f0 = __ldg(g), f1 = __ldg(g + 1), f2 = __ldg(g + 2), f3 = __ldg(g + 3), f4 = __ldg(g + 4);
         px = f0.x; py = f0.y; pz = f1.x; qx = f1.y; qy = f2.x; qz = f2.y; qw = f3.x;
-        sx = splat_exp(f3.y); sy = splat_exp(f4.x); sz = splat_exp(f4.y);
+        sx = rn_exp(f3.y); sy = rn_exp(f4.x); sz = rn_exp(f4.y);
     }
     float4 o0 = make_float4(0.f, 0.f, 0.f, 0.f), o1 = make_float4(0.f, 0.f, 0.f, __uint_as_float(kShadowCulled));
     // :80-82 world position, face from normalize(ws - light)
-    const float w0 = light_m4row(a.M, 0, px, py, pz, 1.0f), w1 = light_m4row(a.M, 1, px, py, pz, 1.0f), w2 = light_m4row(a.M, 2, px, py, pz, 1.0f);
+    const float w0 = clip_row(a.M, 0, px, py, pz, 1.0f), w1 = clip_row(a.M, 1, px, py, pz, 1.0f), w2 = clip_row(a.M, 2, px, py, pz, 1.0f);
     const float dx = sb(w0, a.light[0]), dy = sb(w1, a.light[1]), dz = sb(w2, a.light[2]);
     const float dd = dot3(dx, dy, dz), inv = dv(1.0f, __fsqrt_rn(dd));
     const int face = light_face(ml(dx, inv), ml(dy, inv), ml(dz, inv));
     const float* V = a.V[face];
-    const float v0 = light_m4row(V, 0, w0, w1, w2, 1.0f), v1 = light_m4row(V, 1, w0, w1, w2, 1.0f), v2 = light_m4row(V, 2, w0, w1, w2, 1.0f),
-                v3 = light_m4row(V, 3, w0, w1, w2, 1.0f);
-    const float c0 = light_m4row(a.P, 0, v0, v1, v2, v3), c1 = light_m4row(a.P, 1, v0, v1, v2, v3), c2 = light_m4row(a.P, 2, v0, v1, v2, v3),
-                c3 = light_m4row(a.P, 3, v0, v1, v2, v3);
+    const float v0 = clip_row(V, 0, w0, w1, w2, 1.0f), v1 = clip_row(V, 1, w0, w1, w2, 1.0f), v2 = clip_row(V, 2, w0, w1, w2, 1.0f),
+                v3 = clip_row(V, 3, w0, w1, w2, 1.0f);
+    const float c0 = clip_row(a.P, 0, v0, v1, v2, v3), c1 = clip_row(a.P, 1, v0, v1, v2, v3), c2 = clip_row(a.P, 2, v0, v1, v2, v3),
+                c3 = clip_row(a.P, 3, v0, v1, v2, v3);
     const float clip = ml(1.05f, c3);   // :89-94
     bool alive = !(c2 < -clip || c0 < -clip || c0 > clip || c1 < -clip || c1 > clip);
     if (alive) {
@@ -136,24 +128,16 @@ __global__ void __launch_bounds__(kLightPrepassThreads) light_prepass_kernel(con
 }
 
 // ---- cube raster ----------------------------------------------------------------------------------------------------
-// D24 (DESIGN §2): round-half-even(clamp(d, 0, 1) * (2^24 - 1)), the product exact in fp64; false for NaN (no write)
-__device__ __forceinline__ bool shadow_code(float d, uint32_t& code) {
-    if (d != d) return false;
-    code = __double2uint_rn((double)fminf(fmaxf(d, 0.0f), 1.0f) * 16777215.0);
-    return true;
-}
-
-// the record's two triangles in its face's S x S viewport (the splat draw's rule); false if it draws nothing
-__device__ __forceinline__ bool shadow_setup(const float4* r, uint32_t S, SplatTri t[2], uint32_t& face, uint32_t& code) {
+// the record's two triangles in its face's S x S viewport (the splat draw's rule) and its D24 code; false if it draws
+// nothing
+__device__ __forceinline__ bool shadow_setup(const float4* r, uint32_t S, TileTri t[2], uint32_t& face, uint32_t& code) {
     const float4 a = r[0], b = r[1];
     face = __float_as_uint(b.w);
-    if (face > 5u || !shadow_code(b.z, code)) return false;
+    if (face > 5u || !d24_encode((double)b.z, code)) return false;
     const float4 q[2] = {make_float4(a.x, a.y, 0.f, 0.f), make_float4(a.z, a.w, b.x, b.y)};   // mean, quadScaleNdc
-    splat_quad_setup(q, (int)S, (int)S, t);
+    tile_quad_setup(q, (int)S, (int)S, t);
     return true;
 }
-
-__device__ __forceinline__ int shadow_tiles_x(uint32_t S) { return (int)((S + kSplatTile - 1) / kSplatTile); }
 
 // the binning (m2s_bin.cuh): light records, n = min(count, *d_count), tile = face * (S/16)^2 + tile of the face, pair
 // value = record index
@@ -168,69 +152,41 @@ struct ShadowBins {
     }
     template <typename F>
     __device__ __forceinline__ uint32_t visit(uint32_t i, F&& f) const {
-        SplatTri t[2];
+        TileTri t[2];
         uint32_t face, code;
         if (!shadow_setup(a.light_quads + (uint64_t)i * 2, a.size, t, face, code)) return 0;
-        const int tx = shadow_tiles_x(a.size);
+        const int tx = tiles_x(a.size);
         const uint32_t base = face * (uint32_t)(tx * tx);
-        return splat_for_each_tile(t, tx, [&](uint32_t, uint32_t tile) { f(base + tile, i); });
+        return tile_walk_quad(t, tx, [&](uint32_t, uint32_t tile) { f(base + tile, i); });
     }
 };
 
 struct ShadowStage {
-    int32_t A[6][kSplatThreads], B[6][kSplatThreads];
-    long long C[6][kSplatThreads];
-    uint32_t code[kSplatThreads];
+    QuadEdges e;
+    uint32_t code[kTileThreads];
 };
 
-__global__ void __launch_bounds__(kSplatThreads) shadow_tile_kernel(ShadowArgs a, const uint32_t* __restrict__ vals) {
+__global__ void __launch_bounds__(kTileThreads) shadow_tile_kernel(ShadowArgs a, const uint32_t* __restrict__ vals) {
     __shared__ ShadowStage s;
-    const BinLayout l = bin_layout(a.count, shadow_tiles(a.size));
-    const uint32_t* start = reinterpret_cast<const uint32_t*>(a.scratch + l.ranges_off);
-    const uint32_t S = a.size, tx = (uint32_t)shadow_tiles_x(S), tpf = tx * tx;
-    const uint32_t tile = blockIdx.x, face = tile / tpf, lt = tile % tpf;
-    const int ox = (int)(lt % tx) * kSplatTile, oy = (int)(lt / tx) * kSplatTile;
-    const int tid = threadIdx.x, lx = tid % kSplatTile, ly = tid / kSplatTile;
-    const int x = ox + lx, y = oy + ly;
-    const uint32_t r0 = vals ? start[tile] : 0u, r1 = vals ? start[l.tiles + tile] : 0u;
-    uint32_t best = kShadowClearCode;
-    for (uint32_t base = r0; base < r1; base += kSplatThreads) {
-        const uint32_t nb = min(r1 - base, (uint32_t)kSplatThreads);
-        __syncthreads();
-        if ((uint32_t)tid < nb) {
-            SplatTri t[2];
-            uint32_t f, code;
-            shadow_setup(a.light_quads + (uint64_t)vals[base + tid] * 2, S, t, f, code);   // a record with pairs draws
-#pragma unroll
-            for (int e = 0; e < 6; ++e) {
-                const SplatTri& tt = t[e / 3];
-                const int k = e % 3;
-                s.A[e][tid] = tt.A[k];
-                s.B[e][tid] = tt.B[k];
-                s.C[e][tid] = tt.C[k] + (long long)tt.A[k] * ox + (long long)tt.B[k] * oy - (tt.incl[k] ? 0 : 1);
-            }
-            s.code[tid] = code;
-        }
-        __syncthreads();
-        for (uint32_t j = 0; j < nb; ++j) {
-            const uint32_t code = s.code[j];
-            if (code >= best) continue;   // LESS against the best so far
-            bool cover = false;
-#pragma unroll
-            for (int tri = 0; tri < 2; ++tri) {
-                bool in = true;
-#pragma unroll
-                for (int k = 0; k < 3; ++k) {
-                    const int e = tri * 3 + k;
-                    in &= s.C[e][j] + (long long)s.A[e][j] * lx + (long long)s.B[e][j] * ly >= 0;
-                }
-                cover |= in;
-            }
-            if (cover) best = code;
-        }
-    }
-    if (x >= (int)S || y >= (int)S) return;
-    a.cube[((size_t)face * S + y) * S + x] = __fdiv_rn(__uint2float_rn(best), 16777215.0f);
+    const uint32_t S = a.size, tx = tiles_x(S), tpf = tx * tx;
+    const uint32_t face = blockIdx.x / tpf;
+    const TileFrame f = tile_frame(a.scratch, bin_layout(a.count, shadow_tiles(S)), tx, blockIdx.x % tpf);
+    uint32_t best = kD24Clear;
+    auto stage = [&](int tid, uint32_t val) {
+        TileTri t[2];
+        uint32_t fc, code;
+        shadow_setup(a.light_quads + (uint64_t)val * 2, S, t, fc, code);   // a record with pairs draws
+        quad_stage(t, f.ox, f.oy, s.e, tid);
+        s.code[tid] = code;
+    };
+    tile_batches(f, vals, stage, [&](uint32_t j) {
+        const uint32_t code = s.code[j];
+        // LESS against the best so far; either triangle covering is enough (the OR of the two tests keeps this loop as
+        // short as it was: comparing quad_cover's count with 0 costs two more instructions per staged record)
+        if (code < best && (quad_tri_in(s.e, j, 0, f.lx, f.ly) | quad_tri_in(s.e, j, 1, f.lx, f.ly))) best = code;
+    });
+    if (f.x >= (int)S || f.y >= (int)S) return;
+    a.cube[((size_t)face * S + f.y) * S + f.x] = d24_decode(best);
 }
 
 // ---- deferred lighting ----------------------------------------------------------------------------------------------
@@ -297,7 +253,6 @@ __device__ __forceinline__ float light_cube_fetch(const float* cube, uint32_t S,
     return __ldg(cube + ((size_t)face * S + j) * S + i);
 }
 
-__device__ __forceinline__ uint32_t light_u8(float v) { return __float2uint_rn(ml(fminf(fmaxf(v, 0.0f), 1.0f), 255.0f)); }
 __device__ __forceinline__ float light_unorm(uint32_t c) { return dv((float)c, 255.0f); }
 
 __global__ void __launch_bounds__(kLightThreads) deferred_light_kernel(const __grid_constant__ LightArgs a) {
@@ -390,7 +345,7 @@ __global__ void __launch_bounds__(kLightThreads) deferred_light_kernel(const __g
             out[c] = light_pow(col, 1.0f / 2.2f);
         }
     }
-    reinterpret_cast<uint32_t*>(a.image)[px] = light_u8(out[0]) | light_u8(out[1]) << 8 | light_u8(out[2]) << 16 | 255u << 24;
+    reinterpret_cast<uint32_t*>(a.image)[px] = unorm8(out[0]) | unorm8(out[1]) << 8 | unorm8(out[2]) << 16 | 255u << 24;
 }
 
 // ---- launches -------------------------------------------------------------------------------------------------------
@@ -403,11 +358,7 @@ cudaError_t light_prepass_launch(const ShadowArgs& a, cudaStream_t stream) {
 cudaError_t shadow_count_launch(const ShadowArgs& a, cudaStream_t stream) { return bin_count_launch(ShadowBins{a}, stream); }
 
 cudaError_t shadow_draw_launch(const ShadowArgs& a, int sm_count, cudaStream_t stream) {
-    const ShadowBins b{a};
-    const cudaError_t e = bin_pairs_launch(b, sm_count, stream);
-    if (e != cudaSuccess) return e;
-    shadow_tile_kernel<<<(unsigned)b.tiles(), kSplatThreads, 0, stream>>>(a, bin_vals(b));
-    return cudaGetLastError();
+    return bin_draw_launch(ShadowBins{a}, shadow_tile_kernel, sm_count, stream);
 }
 
 cudaError_t deferred_light_launch(const LightArgs& a, cudaStream_t stream) {

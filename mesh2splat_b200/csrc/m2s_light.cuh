@@ -5,13 +5,12 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
-#include "m2s_splat.cuh"
+#include "m2s_tile.cuh"
 
 namespace m2s {
 
 constexpr uint32_t kShadowMaxSize = 1024;                 // 6 faces x 64 x 64 tiles of 16 x 16: a tile id fits in 16 bits
 constexpr uint64_t kShadowMaxCount = 1ull << 30;
-constexpr uint32_t kShadowClearCode = 0xFFFFFFu;          // D24 clear value 1.0 = 2^24 - 1
 constexpr uint32_t kShadowCulled = 0xFFFFFFFFu;           // face word of a culled light record
 constexpr int kLightPrepassThreads = 256;
 constexpr int kLightThreads = 256;                        // deferred lighting: one thread per pixel
@@ -22,7 +21,7 @@ constexpr int kLightThreads = 256;                        // deferred lighting: 
 constexpr size_t kLightRecordBytes = 32;
 
 // the cube raster's tiles: 6 faces of S x S pixels, each ceil(S/16)^2 tiles of 16 x 16
-__host__ __device__ inline uint64_t shadow_tiles(uint32_t size) { return splat_tiles(size, size) * 6; }
+__host__ __device__ inline uint64_t shadow_tiles(uint32_t size) { return tile_count(size, size) * 6; }
 
 struct ShadowArgs {
     // light prepass (gaussianPointShadowMappingCS.glsl)
@@ -44,7 +43,7 @@ struct ShadowArgs {
     // cube raster (gaussianPointLightCubeMapShadowVS/PS.glsl into 6 x size^2 D24 texels)
     uint32_t size;
     float* cube;                    // 6 x size x size floats: (float)code / 16777215
-    unsigned long long max_pairs;   // (tile, record) pair budget (< kSplatMaxPairs)
+    unsigned long long max_pairs;   // (tile, record) pair budget (< kTileMaxPairs)
     unsigned char* scratch;         // bin_layout(count, shadow_tiles(size)) (m2s_bin.cuh)
     uint32_t* pairs;                // SortLayout(max_pairs) words (m2s_sort.cuh)
 };

@@ -24,25 +24,8 @@
 namespace m2s {
 
 namespace {
-__device__ __forceinline__ float ad(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ float sb(float a, float b) { return __fsub_rn(a, b); }
-__device__ __forceinline__ float ml(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ float dv(float a, float b) { return __fdiv_rn(a, b); }
 __device__ __forceinline__ double dad(double a, double b) { return __dadd_rn(a, b); }
 __device__ __forceinline__ double dml(double a, double b) { return __dmul_rn(a, b); }
-
-// the primitive range of triangle `tri` (sorted, disjoint ranges); false: no primitive, not drawn
-__device__ __forceinline__ bool mesh_range(const MeshArgs& a, uint32_t tri, DRange& out) {
-    int lo = 0, hi = (int)a.nranges - 1;
-    while (lo <= hi) {
-        const int mid = (lo + hi) >> 1;
-        const DRange r = a.ranges[mid];
-        if (tri < r.first) hi = mid - 1;
-        else if (tri >= r.end) lo = mid + 1;
-        else { out = r; return true; }
-    }
-    return false;
-}
 
 // meshRenderVS.glsl:26-37: worldPos = M (p, 1), viewPos = V worldPos, gl_Position = P viewPos (GLM's mat4 * vec4 each)
 __device__ __forceinline__ void mesh_positions(const MeshArgs& a, float x, float y, float z, float (&w)[4], float (&v)[4], float4& c) {
@@ -54,26 +37,16 @@ __device__ __forceinline__ void mesh_positions(const MeshArgs& a, float x, float
                     clip_row(a.P, 2, v[0], v[1], v[2], v[3]), clip_row(a.P, 3, v[0], v[1], v[2], v[3]));
 }
 
-__device__ __forceinline__ void mesh_set(float4& v, const float4& c, int) { v = c; }
-__device__ __forceinline__ void mesh_set(ClipVert& v, const float4& c, int k) {
-    v.p = c;
-#pragma unroll
-    for (int j = 0; j < 3; ++j) v.b[j] = j == k ? 1.0f : 0.0f;
-}
-
-// clip-space polygon of source triangle `tri` (m2s_clip.cuh); returns its vertex count
-template <typename V>
-__device__ __forceinline__ int mesh_poly(const MeshArgs& a, uint32_t tri, V (&v)[kDepthMaxPoly]) {
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-        const float4 p = __ldg(a.tris + (size_t)tri * 9 + k * 3);
-        float w[4], vw[4];
+// the vertex transform of the clip stage: gl_Position
+struct MeshXf {
+    const MeshArgs& a;
+    __device__ __forceinline__ float4 operator()(float x, float y, float z) const {
+        float w[4], v[4];
         float4 c;
-        mesh_positions(a, p.x, p.y, p.z, w, vw, c);
-        mesh_set(v[k], c, k);
+        mesh_positions(a, x, y, z, w, v, c);
+        return c;
     }
-    return clip_poly(v);
-}
+};
 
 // GLM: dot(v, v) = (x x + y y) + z z; normalize(v) = v * (1 / sqrt(dot(v, v)))
 __device__ __forceinline__ void mesh_normalize(float (&v)[3]) {
@@ -177,14 +150,6 @@ __device__ __forceinline__ void mesh_sample(const MeshArgs& a, const TexRef& ref
     out[2] = filt2<2>(bl.w, tx, k4b); out[3] = filt2<3>(bl.w, tx, k4b);
 }
 
-__device__ __forceinline__ uint32_t mesh_half2(float x, float y) {
-    uint16_t hx, hy;
-    splat_to_half(x, hx);
-    splat_to_half(y, hy);
-    return hx | (uint32_t)hy << 16;
-}
-__device__ __forceinline__ uint32_t mesh_u8(float v) { return __float2uint_rn(ml(splat_sat(v), 255.0f)); }
-
 }  // namespace
 
 // the binning (m2s_bin.cuh): source triangles, n = ntri, one pair per tile each front-facing fan triangle touches, pair
@@ -192,74 +157,47 @@ __device__ __forceinline__ uint32_t mesh_u8(float v) { return __float2uint_rn(ml
 struct MeshBins {
     MeshArgs a;
     __host__ __device__ unsigned long long items() const { return a.ntri; }
-    __host__ __device__ uint64_t tiles() const { return splat_tiles(a.width, a.height); }
+    __host__ __device__ uint64_t tiles() const { return tile_count(a.width, a.height); }
     __device__ __forceinline__ uint32_t n() const { return (uint32_t)a.ntri; }
     template <typename F>
     __device__ __forceinline__ uint32_t visit(uint32_t i, F&& f) const {
-        DRange r;
-        if (!mesh_range(a, i, r)) return 0;
-        float4 v[kDepthMaxPoly];
-        const int np = mesh_poly(a, i, v);
-        const int tx = clip_tiles_x(a.width);
-        uint32_t cnt = 0;
-        for (int k = 0; k + 2 < np; ++k) {
-            DepthTri d;
-            clip_fan<true>(v, k, a.width, a.height, d);
-            cnt += clip_for_each_tile(d.t, tx, [&](uint32_t, uint32_t tile) { f(tile, i << 3 | (uint32_t)k); });
-        }
-        return cnt;
+        auto drawn = [&](uint32_t t) {
+            DRange r;
+            return prim_range(a.ranges, a.nranges, t, r);
+        };
+        return clip_visit<true>(a.tris, i, a.width, a.height, drawn, MeshXf{a}, f);
     }
 };
 
 struct MeshStage {
-    int32_t A[3][kSplatThreads], B[3][kSplatThreads];
-    long long C[3][kSplatThreads];   // exact edge values at the tile's pixel (0, 0)
-    float z[3][kSplatThreads];
-    uint32_t incl[kSplatThreads];    // bit k: edge k owns the samples on it (top-left rule)
-    uint32_t prim[kSplatThreads];    // the draw order is (primitive, pair value)
-    uint32_t val[kSplatThreads];
+    FanEdges e;
+    uint32_t prim[kTileThreads];   // the draw order is (primitive, pair value)
+    uint32_t val[kTileThreads];
 };
 
 // stages fan triangle v & 7 of source triangle v >> 3 in slot `slot`, edge values relative to pixel (ox, oy).  Not
 // inlined, as depth_stage.
 __device__ __noinline__ void mesh_stage(const MeshArgs& a, uint32_t v, int ox, int oy, MeshStage& s, int slot) {
     DRange r;
-    mesh_range(a, v >> 3, r);   // a triangle with pairs has a primitive
-    float4 poly[kDepthMaxPoly];
-    mesh_poly(a, v >> 3, poly);
-    DepthTri d;
-    clip_fan<true>(poly, (int)(v & 7u), a.width, a.height, d);
-    uint32_t incl = 0;
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-        s.A[k][slot] = d.t.A[k];
-        s.B[k][slot] = d.t.B[k];
-        s.C[k][slot] = d.t.C[k] + (long long)d.t.A[k] * ox + (long long)d.t.B[k] * oy;
-        s.z[k][slot] = d.z[k];
-        incl |= d.t.incl[k] ? 1u << k : 0u;
-    }
-    s.incl[slot] = incl;
+    prim_range(a.ranges, a.nranges, v >> 3, r);   // a triangle with pairs has a primitive
+    float4 poly[kClipMaxPoly];
+    clip_tri_poly(a.tris, v >> 3, MeshXf{a}, poly);
+    clip_stage<true>(poly, (int)(v & 7u), a.width, a.height, ox, oy, s.e, slot);
     s.prim[slot] = r.prim;
     s.val[slot] = v;
 }
 
-// the five targets of one pixel: RGBA16F as two words of fp16 bits, RGBA8 as one word
-struct MeshOut {
-    uint2 pos, nrm, dep;
-    uint32_t alb, mr;
-};
-
 // meshRenderVS.glsl + meshRenderPS.glsl for pixel (x, y) whose winner is pair value `val`: the fan triangle's set-up, the
 // vertex stage of its source triangle, the varyings at the pixel and at the three quad pixels the derivatives need, the
 // maps, the shading and the target formats.  Not inlined: the tile kernel's pass 1 keeps its registers.
-__device__ __noinline__ void mesh_shade(const MeshArgs& a, uint32_t val, int x, int y, MeshOut& o) {
+__device__ __noinline__ void mesh_shade(const MeshArgs& a, uint32_t val, int x, int y, GTexel& o) {
     const uint32_t tri = val >> 3;
     const int k = (int)(val & 7u);
     DRange r;
-    mesh_range(a, tri, r);
-    ClipVert poly[kDepthMaxPoly];
-    mesh_poly(a, tri, poly);
-    DepthTri d;
+    prim_range(a.ranges, a.nranges, tri, r);
+    ClipVert poly[kClipMaxPoly];
+    clip_tri_poly(a.tris, tri, MeshXf{a}, poly);
+    FanTri d;
     clip_fan<true>(poly, k, a.width, a.height, d);
     double w[3], bc[3][3];   // the fan vertices' clip w and source barycentrics
 #pragma unroll
@@ -357,10 +295,10 @@ __device__ __noinline__ void mesh_shade(const MeshArgs& a, uint32_t val, int x, 
         metal = tex[2];
         rough = tex[1];
     }
-    // computeExponentialDepth (common.glsl:80-84) with GLM's clamp = min(max(x, lo), hi) and splat_exp
+    // computeExponentialDepth (common.glsl:80-84) with GLM's clamp = min(max(x, lo), hi) and rn_exp
     auto glm_clamp01 = [](float x) { const float t = x < 0.0f ? 0.0f : x; return 1.0f < t ? 1.0f : t; };
     const float nd = glm_clamp01(dv(sb(v[12], a.near_far[0]), sb(a.near_far[1], a.near_far[0])));
-    const float dep = glm_clamp01(splat_exp(ml(-20.0f, nd)));
+    const float dep = glm_clamp01(rn_exp(ml(-20.0f, nd)));
     float col[3] = {alb[0], alb[1], alb[2]};   // modes 0, 5, 6
     if (a.mode == 1) { col[0] = col[1] = col[2] = dep; }
     else if (a.mode == 2) { col[0] = en[0]; col[1] = en[1]; col[2] = en[2]; }
@@ -370,73 +308,38 @@ __device__ __noinline__ void mesh_shade(const MeshArgs& a, uint32_t val, int x, 
         col[1] = mesh_hash(ad(ml(id, 269.5f), 1.3f));
         col[2] = mesh_hash(ad(ml(id, 183.3f), 2.7f));
     } else if (a.mode == 4) { col[0] = 0.01f; col[1] = 0.005f; col[2] = 0.0f; }
-    o.pos = make_uint2(mesh_half2(v[0], v[1]), mesh_half2(v[2], 1.0f));
-    o.nrm = make_uint2(mesh_half2(en[0], en[1]), mesh_half2(en[2], 1.0f));
-    o.dep = make_uint2(mesh_half2(dep, dep), mesh_half2(dep, 1.0f));
-    o.alb = mesh_u8(col[0]) | mesh_u8(col[1]) << 8 | mesh_u8(col[2]) << 16 | 255u << 24;
-    o.mr = mesh_u8(metal) | mesh_u8(rough) << 8 | 255u << 24;
+    o.pos = half4(v[0], v[1], v[2], 1.0f);
+    o.nrm = half4(en[0], en[1], en[2], 1.0f);
+    o.dep = half4(dep, dep, dep, 1.0f);
+    o.alb = unorm8(col[0]) | unorm8(col[1]) << 8 | unorm8(col[2]) << 16 | 255u << 24;
+    o.mr = unorm8(metal) | unorm8(rough) << 8 | 255u << 24;
 }
 
-__global__ void __launch_bounds__(kSplatThreads) mesh_tile_kernel(const __grid_constant__ MeshArgs a, const uint32_t* __restrict__ vals) {
+__global__ void __launch_bounds__(kTileThreads) mesh_tile_kernel(const __grid_constant__ MeshArgs a, const uint32_t* __restrict__ vals) {
     __shared__ MeshStage s;
-    const BinLayout l = bin_layout(a.ntri, splat_tiles(a.width, a.height));
-    const uint32_t* start = reinterpret_cast<const uint32_t*>(a.scratch + l.ranges_off);
-    const uint32_t tile = blockIdx.x, tx = (uint32_t)clip_tiles_x(a.width);
-    const int ox = (int)(tile % tx) * kSplatTile, oy = (int)(tile / tx) * kSplatTile;
-    const int tid = threadIdx.x, lx = tid % kSplatTile, ly = tid / kSplatTile;
-    const int x = ox + lx, y = oy + ly;
-    const uint32_t r0 = vals ? start[tile] : 0u, r1 = vals ? start[l.tiles + tile] : 0u;
+    const TileFrame f = tile_frame(a.scratch, bin_layout(a.ntri, tile_count(a.width, a.height)), tiles_x(a.width), blockIdx.x);
     // pass 1: LESS on D24 codes in draw order (primitive table order, then triangle order): the minimum code, and among
     // the fragments that reach it the first one drawn; a code equal to the clear value never passes
-    uint32_t best = kDepthClearCode;
+    uint32_t best = kD24Clear;
     unsigned long long key = ~0ull;
-    for (uint32_t base = r0; base < r1; base += kSplatThreads) {
-        const uint32_t nb = min(r1 - base, (uint32_t)kSplatThreads);
-        __syncthreads();
-        if ((uint32_t)tid < nb) mesh_stage(a, vals[base + tid], ox, oy, s, tid);
-        __syncthreads();
-        for (uint32_t j = 0; j < nb; ++j) {
-            const uint32_t incl = s.incl[j];
-            long long e[3];
-            bool in = true;
-#pragma unroll
-            for (int k = 0; k < 3; ++k) {
-                e[k] = s.C[k][j] + (long long)s.A[k][j] * lx + (long long)s.B[k][j] * ly;
-                in &= e[k] >= ((incl >> k & 1u) ? 0ll : 1ll);
-            }
-            if (!in) continue;
-            // the depth pass's window depth: ((E0 z0 + E1 z1) + E2 z2) / (E0 + E1 + E2) in fp64, D24
-            const double num = dad(dad(dml((double)e[0], (double)s.z[0][j]), dml((double)e[1], (double)s.z[1][j])),
-                                   dml((double)e[2], (double)s.z[2][j]));
-            const double z = __ddiv_rn(num, (double)(e[0] + e[1] + e[2]));
-            if (z != z) continue;   // NaN writes nothing
-            const double zc = z < 0.0 ? 0.0 : (z > 1.0 ? 1.0 : z);
-            const uint32_t code = __double2uint_rn(dml(zc, 16777215.0));
-            const unsigned long long kj = (unsigned long long)s.prim[j] << 32 | s.val[j];
-            if (code < best || (code == best && kj < key)) { best = code; key = kj; }
-        }
-    }
-    if (x >= (int)a.width || y >= (int)a.height) return;
+    tile_batches(f, vals, [&](int tid, uint32_t val) { mesh_stage(a, val, f.ox, f.oy, s, tid); }, [&](uint32_t j) {
+        uint32_t code;
+        if (!clip_depth(s.e, j, f.lx, f.ly, code)) return;
+        const unsigned long long kj = (unsigned long long)s.prim[j] << 32 | s.val[j];
+        if (code < best || (code == best && kj < key)) { best = code; key = kj; }
+    });
+    if (f.x >= (int)a.width || f.y >= (int)a.height) return;
     // pass 2: the winner's fragment shader; the clear colour 0 elsewhere
-    MeshOut o = {make_uint2(0, 0), make_uint2(0, 0), make_uint2(0, 0), 0u, 0u};
-    if (best < kDepthClearCode) mesh_shade(a, (uint32_t)key, x, y, o);
-    const size_t px = (size_t)y * a.width + x;
-    if (a.position) reinterpret_cast<uint2*>(a.position)[px] = o.pos;
-    if (a.normal) reinterpret_cast<uint2*>(a.normal)[px] = o.nrm;
-    if (a.albedo) reinterpret_cast<uint32_t*>(a.albedo)[px] = o.alb;
-    if (a.depth) reinterpret_cast<uint2*>(a.depth)[px] = o.dep;
-    if (a.metallic_roughness) reinterpret_cast<uint32_t*>(a.metallic_roughness)[px] = o.mr;
+    GTexel o = {make_uint2(0, 0), make_uint2(0, 0), make_uint2(0, 0), 0u, 0u};
+    if (best < kD24Clear) mesh_shade(a, (uint32_t)key, f.x, f.y, o);
+    gbuffer_store(a, (size_t)f.y * a.width + f.x, o);
 }
 
 // ---- launches -------------------------------------------------------------------------------------------------------
 cudaError_t mesh_count_launch(const MeshArgs& a, cudaStream_t stream) { return bin_count_launch(MeshBins{a}, stream); }
 
 cudaError_t mesh_draw_launch(const MeshArgs& a, int sm_count, cudaStream_t stream) {
-    const MeshBins b{a};
-    const cudaError_t e = bin_pairs_launch(b, sm_count, stream);
-    if (e != cudaSuccess) return e;
-    mesh_tile_kernel<<<(unsigned)b.tiles(), kSplatThreads, 0, stream>>>(a, bin_vals(b));
-    return cudaGetLastError();
+    return bin_draw_launch(MeshBins{a}, mesh_tile_kernel, sm_count, stream);
 }
 
 }  // namespace m2s

@@ -7,7 +7,7 @@
 
 #include "m2s_depth.cuh"
 #include "m2s_device.cuh"
-#include "m2s_splat.cuh"
+#include "m2s_tile.cuh"
 
 namespace m2s {
 
@@ -29,8 +29,8 @@ struct MeshArgs {
     uint8_t* albedo;                // W x H x 4 uint8, or NULL
     uint16_t* depth;
     uint8_t* metallic_roughness;
-    unsigned long long max_pairs;   // (tile, fan triangle) pair budget (< kSplatMaxPairs)
-    unsigned char* scratch;         // bin_layout(ntri, splat_tiles(width, height))
+    unsigned long long max_pairs;   // (tile, fan triangle) pair budget (< kTileMaxPairs)
+    unsigned char* scratch;         // bin_layout(ntri, tile_count(width, height))
     uint32_t* pairs;                // SortLayout(max_pairs) words (m2s_sort.cuh)
 };
 

@@ -23,8 +23,25 @@ static bool sizes_ok(const char* fn, const char* names, uint32_t max, std::initi
 }
 // a pair budget the pair sort can take
 static bool pair_budget_ok(const char* fn, uint64_t max_pairs) {
-    if (max_pairs >= kSplatMaxPairs) { invalid(fn, "max_pairs too large (< 2^30 supported)"); return false; }
+    if (max_pairs >= kTileMaxPairs) { invalid(fn, "max_pairs too large (< 2^30 supported)"); return false; }
     return true;
+}
+// a G-buffer (m2s_splat_draw, m2s_mesh_render) with at least one target, each aligned for its format
+static bool gbuffer_ok(const char* fn, const m2s_gbuffer* g) {
+    if (!g->position && !g->normal && !g->albedo && !g->depth && !g->metallic_roughness) { invalid(fn, "no targets"); return false; }
+    return aligned_ok(fn, "RGBA16F targets must be 8-byte aligned, RGBA8 targets 4-byte aligned",
+                      {{g->position, 8}, {g->normal, 8}, {g->depth, 8}, {g->albedo, 4}, {g->metallic_roughness, 4}});
+}
+// a scene the mesh passes can bin, and their pair budget
+static bool mesh_scene_ok(const char* fn, const m2s_dscene* scene, uint64_t max_pairs) {
+    if (scene->ntri >= kDepthMaxTris) { invalid(fn, "too many triangles (< 2^29 supported)"); return false; }
+    return pair_budget_ok(fn, max_pairs);
+}
+// the synchronous form of an enqueue form that ran on the context's stream: st, after the stream has finished
+static m2s_status synced(m2s_ctx* ctx, m2s_status st) {
+    if (st != M2S_OK) return st;
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return M2S_OK;
 }
 
 // ---- the viewer prepass (SURVEY 8 f-4): GaussiansPrepass::execute + gaussianSplattingPrepassCS.glsl ----------------
@@ -51,15 +68,16 @@ static bool invert4(const double m[16], double inv[16]) {   // column-major, cof
     return true;
 }
 
-// the `layout` of m2s_prepass* / m2s_shadow_map*: the record layout and the reference's u_format / u_plyHasPbr it stands for
+// the `layout` of m2s_prepass* / m2s_shadow_map*: the record layout and the reference's u_format / u_plyHasPbr it stands
+// for; false, with the error "<fn>: ...", for any other layout
 struct ViewInput { uint32_t layout, fmt, ply_has_pbr; };
-static bool view_input(uint32_t layout, ViewInput& v) {
+static bool view_input(const char* fn, uint32_t layout, ViewInput& v) {
     switch (layout) {
         case M2S_LAYOUT_REF96: v = {0u, 0u, 0u}; return true;     // a conversion's records
         case M2S_LAYOUT_PACKED56: v = {1u, 1u, 0u}; return true;  // a standard 3DGS gaussian, u_format 1 without PBR values
         case M2S_VIEW_PLY: v = {0u, 1u, 0u}; return true;         // REF96 records as m2s_ply_read loads them
         case M2S_VIEW_PLY_PBR: v = {0u, 1u, 1u}; return true;
-        default: return false;
+        default: invalid(fn, "layouts REF96, PACKED56, VIEW_PLY and VIEW_PLY_PBR only"); return false;
     }
 }
 
@@ -69,7 +87,7 @@ static m2s_status prepass_check(const m2s_ctx* ctx, const void* d_records, uint6
     const char* fn = "m2s_prepass";
     if (!ctx || !p || !has_valid || (count && (!d_records || !d_quads || !d_depths))) return invalid(fn, "NULL argument");
     ViewInput v;
-    if (!view_input(p->layout, v)) return invalid(fn, "layouts REF96, PACKED56, VIEW_PLY and VIEW_PLY_PBR only");
+    if (!view_input(fn, p->layout, v)) return M2S_E_INVALID;
     if (p->render_mode == 3 || (p->render_mode > 2 && p->render_mode != 6)) return invalid(fn, "render modes 0 (6), 1 and 2 only");
     if (count >= (1ull << 32)) return invalid(fn, "too many gaussians (< 2^32 supported)");
     return aligned_ok(fn, "the record and quad buffers must be 16-byte aligned", {{d_quads, 16}, {d_records, 16}}) ? M2S_OK : M2S_E_INVALID;
@@ -97,7 +115,7 @@ static m2s_status prepass_fill(const void* d_records, uint64_t count, const uint
     a.mscale2[0] = (float)l0; a.mscale2[1] = (float)l0; a.mscale2[2] = (float)l1;   // (|M[0]|, |M[0]|, |M[1]|) squared — sic (:96)
     a.res[0] = p->resolution[0]; a.res[1] = p->resolution[1]; a.near_far[0] = p->near_far[0]; a.near_far[1] = p->near_far[1];
     ViewInput v;
-    view_input(p->layout, v);   // checked by prepass_check
+    view_input("m2s_prepass", p->layout, v);   // checked by prepass_check
     a.std_dev = p->std_dev; a.render_mode = p->render_mode; a.layout = v.layout; a.fmt = v.fmt; a.ply_has_pbr = v.ply_has_pbr;
     a.count = count; a.d_count = (const unsigned long long*)d_count;
     a.records = (const unsigned char*)d_records; a.quads = (float4*)d_quads; a.depths = d_depths; a.valid = d_valid;
@@ -125,7 +143,7 @@ static m2s_status prepass_depth_check(const m2s_ctx* ctx, const void* d_records,
     m2s_status st = prepass_check(ctx, d_records, count, p, d_quads, d_depths, has_valid);
     if (st != M2S_OK) return st;
     if (!d_mesh_depth || (reinterpret_cast<uintptr_t>(d_mesh_depth) & 3u)) return invalid(fn, "the depth map must be a non-NULL, 4-byte aligned device buffer");
-    return sizes_ok(fn, "depth_width and depth_height", kSplatMaxSide, {depth_width, depth_height}) ? M2S_OK : M2S_E_INVALID;
+    return sizes_ok(fn, "depth_width and depth_height", kTileMaxSide, {depth_width, depth_height}) ? M2S_OK : M2S_E_INVALID;
 }
 
 M2S_EXPORT m2s_status m2s_prepass_mesh_depth_enqueue(m2s_ctx* ctx, const void* d_records, uint64_t count, const uint64_t* d_count,
@@ -211,10 +229,7 @@ M2S_EXPORT m2s_status m2s_depth_sort_enqueue(m2s_ctx* ctx, const void* d_quads, 
 
 M2S_EXPORT m2s_status m2s_depth_sort(m2s_ctx* ctx, const void* d_quads, const float* d_depths, uint64_t count, void* d_sorted_quads,
                                      uint32_t* d_order, uint32_t* d_draw) {
-    m2s_status st = m2s_depth_sort_enqueue(ctx, d_quads, d_depths, count, nullptr, d_sorted_quads, d_order, d_draw, nullptr);
-    if (st != M2S_OK) return st;
-    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    return M2S_OK;
+    return synced(ctx, m2s_depth_sort_enqueue(ctx, d_quads, d_depths, count, nullptr, d_sorted_quads, d_order, d_draw, nullptr));
 }
 
 // Test aid (not part of m2s.h): the number of keys one tile of a sort pass holds.
@@ -242,7 +257,7 @@ static m2s_status bin_pass(m2s_ctx* ctx, BinScratch& s, size_t scratch_bytes, Ar
         CUDA_TRY(cudaMemcpyAsync(ctx->h_total, a.scratch, sizeof(uint64_t), cudaMemcpyDeviceToHost, stream));
         CUDA_TRY(cudaStreamSynchronize(stream));
         max_pairs = *ctx->h_total;
-        if (max_pairs >= kSplatMaxPairs) { set_error(too_many); return M2S_E_INVALID; }
+        if (max_pairs >= kTileMaxPairs) { set_error(too_many); return M2S_E_INVALID; }
     }
     if (max_pairs) {
         st = grow(ctx, s.pairs, sort_layout(max_pairs).total_bytes, stream);
@@ -270,12 +285,9 @@ static m2s_status splat_pass(m2s_ctx* ctx, const void* d_quads, uint64_t count, 
     if (count && !d_quads) return invalid(fn, "NULL quads");
     if (!aligned_ok(fn, "the quad buffer must be 16-byte aligned", {{d_quads, 16}})) return M2S_E_INVALID;
     if (count >= kSplatMaxCount) return invalid(fn, "too many quads (< 2^30 supported)");
-    if (!pair_budget_ok(fn, max_pairs) || !sizes_ok(fn, "width and height", kSplatMaxSide, {p->width, p->height})) return M2S_E_INVALID;
+    if (!pair_budget_ok(fn, max_pairs) || !sizes_ok(fn, "width and height", kTileMaxSide, {p->width, p->height})) return M2S_E_INVALID;
     if (p->render_mode > 6) return invalid(fn, "render modes 0..6 only");
-    if (!g->position && !g->normal && !g->albedo && !g->depth && !g->metallic_roughness) return invalid(fn, "no targets");
-    if (!aligned_ok(fn, "RGBA16F targets must be 8-byte aligned, RGBA8 targets 4-byte aligned",
-                    {{g->position, 8}, {g->normal, 8}, {g->depth, 8}, {g->albedo, 4}, {g->metallic_roughness, 4}}))
-        return M2S_E_INVALID;
+    if (!gbuffer_ok(fn, g)) return M2S_E_INVALID;
     CUDA_TRY(cudaSetDevice(ctx->device));
     SplatArgs a;
     std::memset(&a, 0, sizeof(a));
@@ -284,7 +296,7 @@ static m2s_status splat_pass(m2s_ctx* ctx, const void* d_quads, uint64_t count, 
     a.d_draw = d_draw;
     a.width = p->width; a.height = p->height; a.mode = p->render_mode;
     a.position = g->position; a.normal = g->normal; a.albedo = g->albedo; a.depth = g->depth; a.metallic_roughness = g->metallic_roughness;
-    return bin_pass(ctx, ctx->splat_bins, bin_layout(count, splat_tiles(p->width, p->height)).total_bytes, a, splat_count_launch,
+    return bin_pass(ctx, ctx->splat_bins, bin_layout(count, tile_count(p->width, p->height)).total_bytes, a, splat_count_launch,
                     splat_draw_launch, pick_stream(ctx, stream), sync, max_pairs, pairs, d_drawn,
                     "m2s_splat_draw: the quads need 2^30 or more (tile, quad) pairs");
 }
@@ -362,7 +374,7 @@ static void shadow_uniforms(const m2s_shadow_params* p, ShadowArgs& a) {
     a.near_far[0] = n; a.near_far[1] = fa;
     a.std_dev = p->std_dev;
     ViewInput v;
-    view_input(p->layout, v);   // checked by shadow_pass
+    view_input("m2s_shadow_map", p->layout, v);   // checked by shadow_pass
     a.layout = v.layout;
     a.fmt = v.fmt;
     a.size = p->size;
@@ -377,7 +389,7 @@ static m2s_status shadow_pass(m2s_ctx* ctx, const void* d_records, uint64_t coun
     if (!ctx || !p || !d_cube) return invalid(fn, "NULL argument");
     if (count && !d_records) return invalid(fn, "NULL records");
     ViewInput v;
-    if (!view_input(p->layout, v)) return invalid(fn, "layouts REF96, PACKED56, VIEW_PLY and VIEW_PLY_PBR only");
+    if (!view_input(fn, p->layout, v)) return M2S_E_INVALID;
     if (!aligned_ok(fn, "the record and light-record buffers must be 16-byte aligned, the cube 4-byte aligned",
                     {{d_records, 16}, {d_light_quads, 16}, {d_cube, 4}}))
         return M2S_E_INVALID;
@@ -428,7 +440,7 @@ static bool light_gbuffer_ok(const char* fn, const m2s_gbuffer* g, const float* 
 
 // the checks every lighting entry point makes, then the uniforms; the columns [0, width) and the G-buffer g
 static bool light_args(const char* fn, const m2s_gbuffer* g, const float* d_cube, const m2s_light_params* p, uint8_t* d_image, LightArgs& a) {
-    if (!sizes_ok(fn, "width and height", kSplatMaxSide, {p->width, p->height})) return false;
+    if (!sizes_ok(fn, "width and height", kTileMaxSide, {p->width, p->height})) return false;
     if (p->render_mode > 6) { invalid(fn, "render modes 0..6 only"); return false; }
     if (!light_gbuffer_ok(fn, g, d_cube, p, d_image) || (p->render_mode == 6 && !sizes_ok(fn, "shadow_size", kShadowMaxSize, {p->shadow_size})))
         return false;
@@ -455,10 +467,7 @@ M2S_EXPORT m2s_status m2s_deferred_light_enqueue(m2s_ctx* ctx, const m2s_gbuffer
 }
 
 M2S_EXPORT m2s_status m2s_deferred_light(m2s_ctx* ctx, const m2s_gbuffer* g, const float* d_cube, const m2s_light_params* p, uint8_t* d_image) {
-    m2s_status st = m2s_deferred_light_enqueue(ctx, g, d_cube, p, d_image, nullptr);
-    if (st != M2S_OK) return st;
-    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    return M2S_OK;
+    return synced(ctx, m2s_deferred_light_enqueue(ctx, g, d_cube, p, d_image, nullptr));
 }
 
 // ---- the viewer's mesh depth pre-pass (SURVEY 8 f-9): DepthPrepass::execute + depthPrepassVS/PS.glsl ----------------
@@ -476,10 +485,8 @@ static m2s_status mesh_depth_pass(m2s_ctx* ctx, const m2s_dscene* scene, const m
     const char* fn = "m2s_mesh_depth";
     if (!ctx || !scene || !p || !d_depth) return invalid(fn, "NULL argument");
     if (!aligned_ok(fn, "the depth map must be 4-byte aligned", {{d_depth, 4}}) ||
-        !sizes_ok(fn, "width and height", kSplatMaxSide, {p->width, p->height}))
+        !sizes_ok(fn, "width and height", kTileMaxSide, {p->width, p->height}) || !mesh_scene_ok(fn, scene, max_pairs))
         return M2S_E_INVALID;
-    if (scene->ntri >= kDepthMaxTris) return invalid(fn, "too many triangles (< 2^29 supported)");
-    if (!pair_budget_ok(fn, max_pairs)) return M2S_E_INVALID;
     CUDA_TRY(cudaSetDevice(ctx->device));
     DepthArgs a;
     std::memset(&a, 0, sizeof(a));
@@ -494,7 +501,7 @@ static m2s_status mesh_depth_pass(m2s_ctx* ctx, const m2s_dscene* scene, const m
     a.width = p->width;
     a.height = p->height;
     a.depth = d_depth;
-    return bin_pass(ctx, ctx->depth_bins, bin_layout(a.ntri, splat_tiles(a.width, a.height)).total_bytes, a, depth_count_launch,
+    return bin_pass(ctx, ctx->depth_bins, bin_layout(a.ntri, tile_count(a.width, a.height)).total_bytes, a, depth_count_launch,
                     depth_draw_launch, pick_stream(ctx, stream), sync, max_pairs, pairs, d_drawn,
                     "m2s_mesh_depth: the triangles need 2^30 or more (tile, triangle) pairs");
 }
@@ -546,14 +553,9 @@ static m2s_status mesh_render_pass(m2s_ctx* ctx, const m2s_dscene* scene, const 
                                    bool sync, uint64_t max_pairs, uint64_t* pairs, uint32_t* d_drawn) {
     const char* fn = "m2s_mesh_render";
     if (!ctx || !scene || !p || !g) return invalid(fn, "NULL argument");
-    if (!sizes_ok(fn, "width and height", kSplatMaxSide, {p->width, p->height})) return M2S_E_INVALID;
+    if (!sizes_ok(fn, "width and height", kTileMaxSide, {p->width, p->height})) return M2S_E_INVALID;
     if (p->render_mode > 6) return invalid(fn, "render modes 0..6 only");
-    if (!g->position && !g->normal && !g->albedo && !g->depth && !g->metallic_roughness) return invalid(fn, "no targets");
-    if (!aligned_ok(fn, "RGBA16F targets must be 8-byte aligned, RGBA8 targets 4-byte aligned",
-                    {{g->position, 8}, {g->normal, 8}, {g->depth, 8}, {g->albedo, 4}, {g->metallic_roughness, 4}}))
-        return M2S_E_INVALID;
-    if (scene->ntri >= kDepthMaxTris) return invalid(fn, "too many triangles (< 2^29 supported)");
-    if (!pair_budget_ok(fn, max_pairs)) return M2S_E_INVALID;
+    if (!gbuffer_ok(fn, g) || !mesh_scene_ok(fn, scene, max_pairs)) return M2S_E_INVALID;
     MeshArgs a;
     std::memset(&a, 0, sizeof(a));
     if (!glm_normal_matrix(p->model_to_world, a.N)) return invalid(fn, "model_to_world is singular");
@@ -565,7 +567,7 @@ static m2s_status mesh_render_pass(m2s_ctx* ctx, const m2s_dscene* scene, const 
     a.texs = scene->d_texs; a.arena = scene->d_arena;
     a.width = p->width; a.height = p->height; a.mode = p->render_mode;
     a.position = g->position; a.normal = g->normal; a.albedo = g->albedo; a.depth = g->depth; a.metallic_roughness = g->metallic_roughness;
-    return bin_pass(ctx, ctx->mesh_bins, bin_layout(a.ntri, splat_tiles(a.width, a.height)).total_bytes, a, mesh_count_launch,
+    return bin_pass(ctx, ctx->mesh_bins, bin_layout(a.ntri, tile_count(a.width, a.height)).total_bytes, a, mesh_count_launch,
                     mesh_draw_launch, pick_stream(ctx, stream), sync, max_pairs, pairs, d_drawn,
                     "m2s_mesh_render: the triangles need 2^30 or more (tile, triangle) pairs");
 }
@@ -603,8 +605,5 @@ M2S_EXPORT m2s_status m2s_deferred_light_split_enqueue(m2s_ctx* ctx, const m2s_g
 
 M2S_EXPORT m2s_status m2s_deferred_light_split(m2s_ctx* ctx, const m2s_gbuffer* splat, const m2s_gbuffer* mesh, const float* d_cube,
                                                const m2s_light_params* p, float split_position, uint8_t* d_image) {
-    m2s_status st = m2s_deferred_light_split_enqueue(ctx, splat, mesh, d_cube, p, split_position, d_image, nullptr);
-    if (st != M2S_OK) return st;
-    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    return M2S_OK;
+    return synced(ctx, m2s_deferred_light_split_enqueue(ctx, splat, mesh, d_cube, p, split_position, d_image, nullptr));
 }
