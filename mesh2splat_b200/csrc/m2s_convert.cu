@@ -40,6 +40,7 @@ struct ConvertPlan {
     uint64_t direct_ok;               // the raster kernel shades light units itself (PACKED56, multi-round, one GPU)
     uint64_t claim_late;              // ... and claims a warp's next unit once its current one is done (< 3 units per warp)
     uint64_t direct_max;              // M2S_DIRECT_MAX: the heaviest unit (small-triangle fragments) the direct path takes
+    uint64_t pair_first;              // 16-triangle units; a warp's first pass sets up units 2g and 2g + 1, one per half warp
 };
 
 static void convert_plan(const m2s_ctx* ctx, const m2s_dscene* s, const m2s_params* p, uint64_t out_capacity, uint32_t world,
@@ -55,6 +56,21 @@ static void convert_plan(const m2s_ctx* ctx, const m2s_dscene* s, const m2s_para
     const uint64_t rounds = std::max<uint64_t>(1, (count + warps * kUnitTris - 1) / (warps * kUnitTris));
     pl->unit_tris = std::min<uint64_t>(std::max<uint64_t>((count + warps * rounds - 1) / (warps * rounds), 1), kUnitTris);
     pl->n_units = (count + pl->unit_tris - 1) / pl->unit_tris;
+    pl->multi_round = pl->n_units > warps;
+    pl->direct_ok = klayout == M2S_LAYOUT_PACKED56 && pl->multi_round && world <= 1;
+    // the late claim evens out the weights of the direct units when each warp gets only two of them; with more units
+    // per warp they average out anyway and the claim's exposed atomic round trip is not worth it (DESIGN §4)
+    pl->claim_late = pl->direct_ok && pl->n_units < 3 * warps;
+    pl->direct_max = M2S_DIRECT_MAX;
+    // a balanced unit of 17-24 triangles leaves 8-15 lanes of every set-up and walk idle.  With units of 16 a warp's first
+    // pass sets up two of them on its 32 lanes; the units beyond the static pairs are claimed late, one at a time.  Only
+    // up to 3 units of 16 per warp: a warp then runs the pair and at most one more unit on average, never more passes
+    // than with the balanced units (DESIGN §4)
+    pl->pair_first = pl->claim_late && count <= 3 * warps * (kUnitTris / 2);
+    if (pl->pair_first) {
+        pl->unit_tris = kUnitTris / 2;
+        pl->n_units = (count + pl->unit_tris - 1) / pl->unit_tris;
+    }
     // work-item granularity: ~8 items per SM at the expected output (O(2 R^2) fragments) so that small conversions
     // still spread over the GPU, at most 2048 fragments; an oversized row block (<= 32 rows x R pixels) takes at most
     // kMaxSplit queue slots
@@ -70,12 +86,6 @@ static void convert_plan(const m2s_ctx* ctx, const m2s_dscene* s, const m2s_para
     // cannot overflow.
     pl->queue_cap = std::min<uint64_t>(2 * pl->n_units + pl->cap / 32 + pl->cap / pl->flush_frags + pl->cap / pl->item_max +
                                        warps * (2ull * kMaxSplit + kStashItems) + 64, (1u << 24) - 1);
-    pl->multi_round = pl->n_units > warps;
-    pl->direct_ok = klayout == M2S_LAYOUT_PACKED56 && pl->multi_round && world <= 1;
-    // the late claim evens out the weights of the direct units when each warp gets only two of them; with more units
-    // per warp they average out anyway and the claim's exposed atomic round trip is not worth it (DESIGN §4)
-    pl->claim_late = pl->direct_ok && pl->n_units < 3 * warps;
-    pl->direct_max = M2S_DIRECT_MAX;
 }
 
 // Test and tuning aid (not part of m2s.h): the plan m2s_convert would launch with for these arguments.  `plan` receives
@@ -163,6 +173,7 @@ m2s_status m2s::convert_enqueue_impl(m2s_ctx* ctx, const m2s_dscene* s, const m2
     a.n_units = (uint32_t)pl.n_units;
     a.direct_ok = (uint32_t)pl.direct_ok;
     a.claim_late = (uint32_t)pl.claim_late;
+    a.pair_first = (uint32_t)pl.pair_first;
     a.trace = g_trace;
     if (peers && peers->world > 1) {
         a.world = peers->world; a.rank = peers->rank;

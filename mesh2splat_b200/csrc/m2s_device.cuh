@@ -116,6 +116,7 @@ struct ConvertArgs {
     uint32_t n_units;
     uint32_t direct_ok;                // the raster kernel may shade light units itself (ConvertPlan::direct_ok)
     uint32_t claim_late;               // ... and claims its next unit once the current one is done (ConvertPlan::claim_late)
+    uint32_t pair_first;               // a warp's first pass sets up units 2g and 2g + 1 on its two half warps (ConvertPlan::pair_first)
     unsigned long long* trace;         // M2S_TRACE builds only: 16 per-phase sums per raster warp (TraceSlot)
     // multi-GPU fused gather (world <= 1: off).  peer_out[p] / peer_xch[p] are rank p's final buffer and
     // exchange block mapped into this process (NVLink peer memory); every rank's fragment kernel stores its

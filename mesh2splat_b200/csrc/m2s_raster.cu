@@ -8,7 +8,9 @@
 // raster_kernel (persistent, one CTA per SM, every warp an autonomous pipeline; one __syncthreads after the descriptor
 // tables are copied to shared memory, none in the steady state)
 //   work unit = <= 32 consecutive triangles; a warp's first unit is static (global warp id), further ones are
-//     claimed from a global counter; the next unit's triangles are in flight (TMA) while this one is processed
+//     claimed from a global counter; the next unit's triangles are in flight (TMA) while this one is processed.
+//     Launches of 16-triangle units (ConvertPlan::pair_first): the first pass sets up units 2g and 2g + 1 on the two
+//     half warps, and the second unit's direct shading is shared with the CTA's other warps (CtaQueue)
 //   TMA (cp.async.bulk + mbarrier complete_tx) stages the unit's 144 B/triangle into shared memory
 //   per-triangle stage, one LANE per triangle (converterGS.glsl:326-443): longest edge, face normal, dominant
 //     axis, orthographic uv, quaternion, UV->3D Jacobian scale; rasteriser set-up: 24.8 fixed-point window
@@ -84,6 +86,7 @@ struct __align__(128) WarpBlock {
     uint32_t itTotal[kStashItems];                // fragments per item
     uint64_t bar;
     double logtab[RK == 1 ? 32 : 1];              // PACKED56: the direct path's copy of ref_logf's table (kLogfTab)
+    uint32_t left;                                // shared pieces of this warp's second unit not yet shaded (CtaQueue)
 };
 
 // The scene's descriptor tables as the set-up sees them: in shared memory when they fit (each CTA copies
@@ -425,16 +428,16 @@ __device__ __forceinline__ void list_pixels(T* list, uint32_t k, unsigned long l
 
 // the unit's small triangles as one item (blocks implicit: one per triangle, TriRec::first/hits).  A unit with at
 // most 32 such fragments (sub-pixel meshes: most units of a 1 M-triangle scan) lists them in the item instead: the
-// fragment kernel then needs neither the staged unit nor its span table.  hits/w/first: this lane's triangle.
+// fragment kernel then needs neither the staged unit nor its span table.  hits/w/first/slot: this lane's triangle.
 template <int RK>
 __device__ __forceinline__ void stash_unit_item(const ConvertArgs& a, WarpBlock<RK>& wb, uint32_t unit, Stash& st, uint32_t total_small,
-                                                uint32_t ntri, unsigned long long hits, uint32_t w, uint32_t first, int lane) {
+                                                uint32_t ntri, unsigned long long hits, uint32_t w, uint32_t first, uint32_t slot, int lane) {
     if (total_small == 0) return;
     // the open item (if any) stays open: closed items occupy the slots below n_it, the open one is written at n_it
     // only when it closes — so insert the unit item by closing the open one first
     stash_close_item<RK>(a, wb, unit, st, lane);
     const bool micro = total_small <= 32;
-    if (micro) list_pixels(reinterpret_cast<uint32_t*>(wb.pend + st.n_it * kItemBlocks), first, hits, w, (uint32_t)lane);
+    if (micro) list_pixels(reinterpret_cast<uint32_t*>(wb.pend + st.n_it * kItemBlocks), first, hits, w, slot);
     if (lane == 0) { wb.itN[st.n_it] = ntri | kItUnit | (micro ? kItMicro : 0u); wb.itTotal[st.n_it] = total_small; }
     st.frags += total_small; st.slots += 1; st.n_it += 1;
     if (st.n_it == kStashItems) stash_flush<RK>(a, wb, unit, st, lane);
@@ -458,14 +461,24 @@ __device__ __forceinline__ void count_blocks(const ConvertArgs& a, WarpBlock<RK>
 // others are done: it posts its tall triangles here, in pieces of kDeferBlocks row blocks, and every warp of the CTA that
 // has run out of units takes tickets.  Shared-memory atomics only: a grid-wide queue was tried (r02) and lost to the
 // serialisation of same-address global atomics (one per unit / per claim: 8-30 us at 2-30 k units).
+// The same queue shares the shading of a paired first pass's second unit (h < 0, SharePiece): pieces of kShareGroups
+// groups of 32 listed fragments, shaded by whichever warp of the CTA takes them first: the owner or a warp out of units.
+struct SharePiece {
+    unsigned long long first;     // output index of the owner's listed fragment 0
+    uint32_t owner;               // warp of the CTA whose slice holds the records and the list
+    uint32_t tri0;                // the scene triangle of the owner's record 0
+    uint32_t f0, f1;              // listed fragments [f0, f1)
+};
 struct CtaEntry {
-    RowState rs;                  // 64 B
-    int h;
+    union { RowState rs; SharePiece sp; };   // 64 B
+    int h;                        // < 0: a shading piece (sp)
     uint32_t unit, slot, rb0, rb1;
     volatile uint32_t ready;      // written last
-    uint32_t pad[2];
+    uint32_t taken;               // shading pieces: set by the warp that shades it
+    uint32_t pad;
 };
-constexpr uint32_t kCtaQueueCap = 40;
+constexpr uint32_t kCtaQueueCap = 48;
+constexpr uint32_t kShareGroups = 2;
 struct CtaQueue {
     uint32_t tail;                // entries posted (may exceed the capacity: the poster keeps the overflow)
     uint32_t head;                // tickets taken
@@ -482,32 +495,35 @@ struct CtaQueue {
 // warps of an SM are too few to hide the latency of the shading chain and the unit goes to the fragment kernel (that was
 // faster than the direct path, also with CTA-level group stealing and software pipelining, when measured during
 // development).
-// The worker: the `total` listed fragments of this warp's unit, 32 at a time (PACKED56).  Out of line: its registers are
-// not the raster loop's.  It takes the few per-launch values it needs as arguments (through a ConvertArgs reference every
-// group re-loaded them).  tri0: the unit's first triangle of the scene; base / room: OutRange; logtab: ref_logf's table.
+// The worker: the listed fragments [f0, f1) of the unit(s) in `src`'s slice, 32 at a time (PACKED56).  Out of line: its
+// registers are not the raster loop's.  It takes the few per-launch values it needs as arguments (through a ConvertArgs
+// reference every group re-loaded them).  dfirst: the output index of listed fragment 0; tri0: the scene triangle of
+// record 0; base / room: OutRange; logtab: ref_logf's table.  `src` is the shading warp's own slice, or another warp's
+// for a shared piece (CtaQueue); the stage is always the shading warp's own dead triangle staging area.
 // A group's records leave the stage as one bulk async copy issued by lane 0 (bulk_span, with emit_records' capacity cut);
 // the groups alternate between the two halves of the stage, so a group is shaded while the previous one's copy reads.
+// `par` is the half of the next group; the half after the last group is returned, so that the alternation holds across calls.
 // ------------------------------------------------------------------------------------------
-__device__ __noinline__ void direct_run(WarpBlock<1>& wb, uint32_t total, unsigned long long dfirst, uint32_t tri0, uint8_t* out,
-                                        unsigned long long* keys, const uint32_t* __restrict__ texb, const double* logtab, float log_sz,
-                                        unsigned long long base, unsigned long long room, int lane) {
+__device__ __noinline__ uint32_t direct_run(const WarpBlock<1>& src, uint32_t f0, uint32_t f1, unsigned long long dfirst, uint32_t tri0,
+                                            unsigned char* stage0, uint32_t par, uint8_t* out, unsigned long long* keys,
+                                            const uint32_t* __restrict__ texb, const double* logtab, float log_sz,
+                                            unsigned long long base, unsigned long long room, int lane) {
     constexpr int kStride = Cfg<1>::kStride;
     constexpr uint32_t kHalf = kUnitTris * kTriBytes / 2;
     static_assert(8 + 32 * kStride <= kHalf && kHalf % 16 == 0, "two output stages (32 records + the shift) in the triangle staging area");
-    unsigned char* const stage0 = reinterpret_cast<unsigned char*>(wb.tri);   // dead since the set-up of the unit
-    const unsigned short* list = reinterpret_cast<const unsigned short*>(wb.pend);
-    for (uint32_t g0 = 0; g0 < total; g0 += 32) {
-        const uint32_t nfr = min(32u, total - g0);
+    const unsigned short* list = reinterpret_cast<const unsigned short*>(src.pend);
+    for (uint32_t g0 = f0; g0 < f1; g0 += 32, par ^= 1u) {
+        const uint32_t nfr = min(32u, f1 - g0);
         const uint32_t e = list[g0 + min((uint32_t)lane, nfr - 1u)];  // idle lanes shadow the last fragment
         const uint32_t slot = e & 31u;
         const int dxi = (int)((e >> 5) & 63u), dyi = (int)(e >> 11);
         const unsigned long long idx = dfirst + g0;
-        unsigned char* const stage = stage0 + ((g0 >> 5) & 1u) * kHalf;
+        unsigned char* const stage = stage0 + par * kHalf;
         Frag1 s;
-        shade1_fetch(wb.rec[slot], dxi, dyi, texb, s);
+        shade1_fetch(src.rec[slot], dxi, dyi, texb, s);
         if (lane == 0) tma_store_wait_read_but_last();   // the copy from this half, two groups ago
         __syncwarp();
-        shade1_finish(log_sz, logtab, wb.rec[slot], s, stage + stage_shift<kStride>(base + idx) + lane * kStride);
+        shade1_finish(log_sz, logtab, src.rec[slot], s, stage + stage_shift<kStride>(base + idx) + lane * kStride);
         fence_proxy_async();   // the stage's writes, before the bulk copy reads them
         __syncwarp();
         const uint32_t nval = idx < room ? (uint32_t)min((unsigned long long)nfr, room - idx) : 0u;
@@ -515,8 +531,9 @@ __device__ __noinline__ void direct_run(WarpBlock<1>& wb, uint32_t total, unsign
             bulk_span<kStride>(out, (base + idx) * (unsigned long long)kStride, stage, nval * kStride);
             tma_store_commit();
         }
-        if (keys != nullptr && (uint32_t)lane < nval) keys[base + idx + lane] = fragment_key(tri0 + slot, wb.rec[slot].meta, (uint32_t)dxi, (uint32_t)dyi);
+        if (keys != nullptr && (uint32_t)lane < nval) keys[base + idx + lane] = fragment_key(tri0 + slot, src.rec[slot].meta, (uint32_t)dxi, (uint32_t)dyi);
     }
+    return par;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -543,17 +560,21 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
     }
     __syncwarp();
     // the first unit of every warp is static (unit = global warp id): no atomic, and nobody can grab two units
-    // while a neighbour gets none; its triangles start moving before the descriptor tables are copied
+    // while a neighbour gets none; its triangles start moving before the descriptor tables are copied.  Paired launches
+    // (ConvertPlan::pair_first): the first pass takes units 2g and 2g + 1, one per half warp, on one load
     const uint32_t nwarps_total = gridDim.x * (blockDim.x >> 5);
-    uint32_t unit = blockIdx.x + gridDim.x * warp;  // warp w of every CTA before warp w+1 of any: SMs fill evenly
-    auto issue_load = [&](uint32_t u) {  // lane 0 only
+    const uint32_t gwarp = blockIdx.x + gridDim.x * warp;  // warp w of every CTA before warp w+1 of any: SMs fill evenly
+    bool pair = kDirectOK && a.pair_first != 0;
+    uint32_t unit = pair ? 2 * gwarp : gwarp;
+    const uint32_t claim_base = pair ? 2 * nwarps_total : nwarps_total;   // the first unit the counter hands out
+    auto issue_load = [&](uint32_t u, uint32_t n) {  // lane 0 only: up to n triangles from unit u on
         const uint32_t t0 = u * a.unit_tris;
-        const uint32_t bytes = min(a.unit_tris, a.tri_count - t0) * kTriBytes;
+        const uint32_t bytes = min(n, a.tri_count - t0) * kTriBytes;
         fence_proxy_async();
         mbar_arrive_expect_tx(&wb.bar, bytes);
         tma_load_1d(wb.tri, tri_bytes + ((size_t)a.tri_first + t0) * kTriBytes, bytes, &wb.bar);
     };
-    if (lane == 0 && unit < a.n_units) issue_load(unit);
+    if (lane == 0 && unit < a.n_units) issue_load(unit, pair ? 2 * a.unit_tris : a.unit_tris);
     // ref_logf's table for the direct path's opacities -> the warp's slice, as an asynchronous copy that lands while the
     // first unit is set up (waited for before the first shading; a CTA-wide copy would wait at the barrier below: ~1 us
     // more per warp, measured on the H100)
@@ -579,17 +600,28 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
     }
     CtaQueue& cq = *reinterpret_cast<CtaQueue*>(smem + (size_t)C::kWarps * sizeof(WarpBlock<RK>) + kTableSmemBytes);
     if (threadIdx.x == 0) { cq.tail = 0; cq.head = 0; cq.active = blockDim.x >> 5; }
-    if (threadIdx.x < kCtaQueueCap) cq.q[threadIdx.x].ready = 0u;
+    if (threadIdx.x < kCtaQueueCap) { cq.q[threadIdx.x].ready = 0u; cq.q[threadIdx.x].taken = 0u; }
     __syncthreads();  // tables + help queue: the only CTA-wide barrier before the end of the kernel
     const OutRange out = out_range(a);   // the direct path's records
     uint32_t phase = 0;
+    uint32_t spar = 0;   // the half of this warp's output stage that its next group of direct records goes to
     Stash st;
     st.n_it = 0; st.cur_nb = 0; st.cur_total = 0; st.frags = 0; st.slots = 0; st.seen = 0;
+    // the listed fragments [f0, f1) of the unit(s) in slice `src`, shaded by this warp through its own stage (direct_run)
+    auto shade = [&](const WarpBlock<RK>& src, uint32_t f0, uint32_t f1, unsigned long long first, uint32_t tri0) {
+        if constexpr (kDirectOK) {
+            spar = direct_run(src, f0, f1, first, tri0, reinterpret_cast<unsigned char*>(wb.tri), spar, a.out, a.keys, a.tex_base,
+                              wb.logtab, a.log_sz, out.base, out.room, lane);
+            TR_ADD(a, kTrGroups, (f1 - f0 + 31) / 32);
+        }
+    };
     TR_PHASE(a, kTrEntry);
 
     while (unit < a.n_units) {
         const uint32_t t0 = unit * a.unit_tris;
-        const uint32_t ntri = min(a.unit_tris, a.tri_count - t0);
+        const uint32_t ntri = min(pair ? 2 * a.unit_tris : a.unit_tris, a.tri_count - t0);   // triangles of this pass
+        const uint32_t nu = pair && ntri > a.unit_tris ? 2u : 1u;                              // units of this pass
+        const int sw = pair ? 16 : 32;   // lanes per unit: lane l sets up triangle l of the pass, of unit `unit + l / sw`
         uint32_t next = 0xffffffffu;
         // launches with a direct path and fewer than three units per warp: the next unit is claimed only once this unit's
         // work is known (after its shading for a direct unit).  A direct unit shades anything from 0 to 16 groups of 32
@@ -599,14 +631,14 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         // weights average out and the claim stays up front.  The host decides (ConvertPlan::claim_late).
         const bool claim_late = kDirectOK && a.claim_late != 0;
         if (lane == 0) {
-            if (a.n_units > nwarps_total && !claim_late) next = nwarps_total + atomicAdd(SCHED(a, 0), 1u);  // needed only after the set-up
+            if (a.n_units > nwarps_total && !claim_late) next = claim_base + atomicAdd(SCHED(a, 0), 1u);  // needed only after the set-up
             tma_store_wait_read();  // the previous unit's record store has finished reading wb.rec
         }
         mbar_wait(&wb.bar, phase);
         phase ^= 1;
         __syncwarp();
         TR_PHASE(a, kTrLoadWait);
-        TR_ADD(a, kTrUnits, 1);
+        TR_ADD(a, kTrUnits, nu);
 
         // ---- per-triangle stage: one lane per triangle ----
         uint32_t cnt = 0;
@@ -641,19 +673,21 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         const uint32_t mine = small ? cnt : 0u;
         const unsigned long long hits = box_mask(e0, e1, e2, a0, a1, a2, b0, b1, b2, w, mine, __reduce_max_sync(0xffffffffu, mine));
         const uint32_t nh = (uint32_t)__popcll(hits);
-        uint32_t incl_scan = nh;  // inclusive warp scan
+        // the scans run over the lanes of one unit: TriRec::first is relative to the triangle's own unit
+        uint32_t incl_scan = nh;  // inclusive scan
 #pragma unroll
         for (int d = 1; d < 32; d <<= 1) {
-            const uint32_t v = __shfl_up_sync(0xffffffffu, incl_scan, d);
-            if (lane >= d) incl_scan += v;
+            const uint32_t v = __shfl_up_sync(0xffffffffu, incl_scan, d, sw);
+            if ((lane & (sw - 1)) >= d) incl_scan += v;
         }
-        const uint32_t total_small = __shfl_sync(0xffffffffu, incl_scan, 31);
+        const uint32_t tot0 = __shfl_sync(0xffffffffu, incl_scan, sw - 1);   // small-triangle fragments of the first unit
+        const uint32_t tot1 = __shfl_sync(0xffffffffu, incl_scan, 31);       // ... and of the second (paired pass)
         const uint32_t myrows = small ? (uint32_t)ts.h : 0u;  // rows this triangle contributes to the unit item's span table
         uint32_t rows_scan = myrows;
 #pragma unroll
         for (int d = 1; d < 32; d <<= 1) {
-            const uint32_t v = __shfl_up_sync(0xffffffffu, rows_scan, d);
-            if (lane >= d) rows_scan += v;
+            const uint32_t v = __shfl_up_sync(0xffffffffu, rows_scan, d, sw);
+            if ((lane & (sw - 1)) >= d) rows_scan += v;
         }
         if ((uint32_t)lane < ntri) {
             myrec.hits = hits;
@@ -662,87 +696,142 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         }
         __syncwarp();
         TR_PHASE(a, kTrWalkScan);
-        // DIRECT path (REF96 / PACKED56, single GPU): when the unit's small triangles emit at most M2S_DIRECT_MAX fragments
+        // DIRECT path (REF96 / PACKED56, single GPU): when a unit's small triangles emit at most M2S_DIRECT_MAX fragments
         // this warp shades them itself, straight from the records in its shared-memory slice — no work item, no record
         // round trip through L2, no second kernel on the critical path.  The triangle staging area (dead since the set-up)
         // is the warp's output stage then, so the next unit's triangles start flying in after the shading instead of now.
-        const bool direct = kDirectOK && a.direct_ok != 0 && total_small != 0 && total_small <= (uint32_t)M2S_DIRECT_MAX;
+        const bool direct_ok = kDirectOK && a.direct_ok != 0;
+        const bool direct0 = direct_ok && tot0 != 0 && tot0 <= (uint32_t)M2S_DIRECT_MAX;
+        const bool direct1 = nu == 2 && direct_ok && tot1 != 0 && tot1 <= (uint32_t)M2S_DIRECT_MAX;
+        const bool direct = direct0 || direct1;
+        const uint32_t hf = (uint32_t)lane / (uint32_t)sw;                 // this lane's unit of the pass
+        const unsigned hmask = sw == 32 ? 0xffffffffu : 0xffffu << (hf * 16);   // the lanes of that unit
+        const bool my_direct = hf ? direct1 : direct0;
+        const uint32_t dfr0 = direct0 ? tot0 : 0u, dsum = dfr0 + (direct1 ? tot1 : 0u);   // the pass's list: unit 0's, then unit 1's
         auto claim = [&]() {   // the next unit, claimed once this one's work is known
-            if (lane == 0) next = nwarps_total + atomicAdd(SCHED(a, 0), 1u);
+            if (lane == 0) next = claim_base + atomicAdd(SCHED(a, 0), 1u);
             next = __shfl_sync(0xffffffffu, next, 0);
         };
         if (claim_late && !direct) claim();
-        if (!direct && lane == 0 && next < a.n_units) issue_load(next);
+        if (!direct && lane == 0 && next < a.n_units) issue_load(next, a.unit_tris);
 
         // ---- all other triangles: the warp counts one triangle at a time, one lane per pixel row; the tall triangles of
-        // a heavy unit are posted to the CTA's help queue instead (see CtaQueue) ----
-        const uint32_t gm_all = __ballot_sync(0xffffffffu, cnt != 0 && !small);
-        const uint32_t myblocks = (cnt != 0 && !small) ? (uint32_t)(ts.h + 31) / 32u : 0u;
-        const uint32_t unit_blocks = __reduce_add_sync(0xffffffffu, myblocks);
-        unsigned gm = gm_all;
-        if (unit_blocks > kDeferUnitBlocks) {
-            unsigned dm = __ballot_sync(0xffffffffu, myblocks >= 2);
-            while (dm) {
-                const int s = __ffs(dm) - 1;
-                dm &= dm - 1;
-                int h;
-                const RowState rs = row_state(wb.rec[s], h);
-                const uint32_t nb = (uint32_t)(h + 31) / 32u, nent = (nb + kDeferBlocks - 1) / kDeferBlocks;
-                uint32_t base = 0;
-                if (lane == 0) base = atomicAdd_block(&cq.tail, nent);
-                base = __shfl_sync(0xffffffffu, base, 0);
-                const uint32_t fit = base < kCtaQueueCap ? min(nent, kCtaQueueCap - base) : 0u;  // the first `fit` pieces go to the queue
-                if ((uint32_t)lane < fit) {
-                    CtaEntry& e = cq.q[base + lane];
-                    e.rs = rs; e.h = h; e.unit = unit; e.slot = (uint32_t)s;
-                    e.rb0 = lane * kDeferBlocks; e.rb1 = min(nb, (lane + 1) * kDeferBlocks);
-                    __threadfence_block();
-                    e.ready = 1u;
+        // a heavy unit are posted to the CTA's help queue instead (see CtaQueue).  Every work item names one unit, so the
+        // first unit of a paired pass reserves its items before the second unit's are stashed ----
+        const bool larger = cnt != 0 && !small;
+        const uint32_t gm_all = __ballot_sync(0xffffffffu, larger);
+        const uint32_t myblocks = larger ? (uint32_t)(ts.h + 31) / 32u : 0u;
+        for (uint32_t k = 0; k < nu; ++k) {
+            const uint32_t u = unit + k, lo = k * (uint32_t)sw;
+            const unsigned umask = nu == 1 ? 0xffffffffu : 0xffffu << lo;
+            const bool in_u = (umask >> lane) & 1u;
+            const uint32_t unit_blocks = __reduce_add_sync(0xffffffffu, in_u ? myblocks : 0u);
+            unsigned gm = gm_all & umask;
+            if (unit_blocks > kDeferUnitBlocks) {
+                unsigned dm = __ballot_sync(0xffffffffu, myblocks >= 2) & umask;
+                while (dm) {
+                    const int s = __ffs(dm) - 1;
+                    dm &= dm - 1;
+                    int h;
+                    const RowState rs = row_state(wb.rec[s], h);
+                    const uint32_t nb = (uint32_t)(h + 31) / 32u, nent = (nb + kDeferBlocks - 1) / kDeferBlocks;
+                    uint32_t base = 0;
+                    if (lane == 0) base = atomicAdd_block(&cq.tail, nent);
+                    base = __shfl_sync(0xffffffffu, base, 0);
+                    const uint32_t fit = base < kCtaQueueCap ? min(nent, kCtaQueueCap - base) : 0u;  // the first `fit` pieces go to the queue
+                    if ((uint32_t)lane < fit) {
+                        CtaEntry& e = cq.q[base + lane];
+                        e.rs = rs; e.h = h; e.unit = u; e.slot = (uint32_t)s - lo;
+                        e.rb0 = lane * kDeferBlocks; e.rb1 = min(nb, (lane + 1) * kDeferBlocks);
+                        __threadfence_block();
+                        e.ready = 1u;
+                    }
+                    if (fit < nent) count_blocks<RK>(a, wb, u, st, rs, h, (uint32_t)s - lo, (int)(fit * kDeferBlocks), 1 << 20, lane);  // the rest stays here
+                    gm &= ~(1u << s);
                 }
-                if (fit < nent) count_blocks<RK>(a, wb, unit, st, rs, h, (uint32_t)s, (int)(fit * kDeferBlocks), 1 << 20, lane);  // the rest stays here
-                gm &= ~(1u << s);
             }
-        }
-        while (gm) {
-            const int s = __ffs(gm) - 1;
-            gm &= gm - 1;
-            int h;
-            const RowState rs = row_state(wb.rec[s], h);  // broadcast reads of the record
-            count_blocks<RK>(a, wb, unit, st, rs, h, (uint32_t)s, 0, 1 << 20, lane);
-        }
-        // ONE atomicAdd per unit (unless the stash filled up on the way) reserves the output range and the queue
-        // slots of everything the unit emits
-        stash_close_item<RK>(a, wb, unit, st, lane);
-        if (!direct) {
-            stash_unit_item<RK>(a, wb, unit, st, total_small, ntri, hits, (uint32_t)w, incl_scan - nh, lane);
-            stash_flush<RK>(a, wb, unit, st, lane);
+            while (gm) {
+                const int s = __ffs(gm) - 1;
+                gm &= gm - 1;
+                int h;
+                const RowState rs = row_state(wb.rec[s], h);  // broadcast reads of the record
+                count_blocks<RK>(a, wb, u, st, rs, h, (uint32_t)s - lo, 0, 1 << 20, lane);
+            }
+            stash_close_item<RK>(a, wb, u, st, lane);
+            if (!(k ? direct1 : direct0))
+                stash_unit_item<RK>(a, wb, u, st, k ? tot1 : tot0, k ? ntri - lo : min(ntri, (uint32_t)sw), in_u ? hits : 0ull,
+                                    (uint32_t)w, incl_scan - nh, (uint32_t)lane - lo, lane);
+            if (k + 1 < nu) stash_flush<RK>(a, wb, u, st, lane);
         }
         TR_PHASE(a, kTrLarger);
+        // ONE atomicAdd per pass (unless the stash filled up on the way, or both units of a pair queue items) reserves the
+        // output range and the queue slots of everything the pass emits; the direct fragments come last
+        const unsigned long long dfirst = stash_flush<RK>(a, wb, unit + nu - 1, st, lane, dsum);   // the stash area is free after this
+        TR_PHASE(a, kTrReserve);
         if constexpr (kDirectOK) {
             if (direct) {
-                const unsigned long long dfirst = stash_flush<RK>(a, wb, unit, st, lane, total_small);   // the stash area is free after this
-                TR_PHASE(a, kTrReserve);
-                TR_ADD(a, kTrDirectUnits, 1);
-                // every lane lists the covered pixels of its triangle at their place in the unit
-                list_pixels(reinterpret_cast<unsigned short*>(wb.pend), incl_scan - nh, hits, (uint32_t)w, (uint32_t)lane);
+                TR_ADD(a, kTrDirectUnits, (direct0 ? 1 : 0) + (direct1 ? 1 : 0));
+                // every lane of a direct unit lists the covered pixels of its triangle at their place in the pass's list
+                list_pixels(reinterpret_cast<unsigned short*>(wb.pend), (hf ? dfr0 : 0u) + incl_scan - nh, my_direct ? hits : 0ull,
+                            (uint32_t)w, (uint32_t)lane);
                 cp_async_wait_all();   // wb.logtab has landed (a no-op after the first direct unit)
                 __syncwarp();
                 TR_PHASE(a, kTrList);
-                direct_run(wb, total_small, dfirst, a.tri_first + t0, a.out, a.keys, a.tex_base, wb.logtab, a.log_sz, out.base, out.room, lane);
+                const uint32_t tri0 = a.tri_first + t0;
+                // a paired pass posts its second unit's groups to the CTA's help queue, then shades its first unit: a warp that
+                // is out of units takes the pieces this warp has not reached (the late claim cannot balance a pass's weight)
+                uint32_t npiece = 0, qbase = 0, fit = 0;
+                if (direct1) {
+                    npiece = (tot1 + 32 * kShareGroups - 1) / (32 * kShareGroups);
+                    if (lane == 0) qbase = atomicAdd_block(&cq.tail, npiece);
+                    qbase = __shfl_sync(0xffffffffu, qbase, 0);
+                    fit = qbase < kCtaQueueCap ? min(npiece, kCtaQueueCap - qbase) : 0u;   // the rest is this warp's own
+                    if (lane == 0) wb.left = fit;
+                    __threadfence_block();   // the count, the records and the list, before the pieces are posted
+                    __syncwarp();
+                    if ((uint32_t)lane < fit) {
+                        CtaEntry& e = cq.q[qbase + lane];
+                        e.h = -1;
+                        e.sp.first = dfirst; e.sp.owner = (uint32_t)warp; e.sp.tri0 = tri0;
+                        e.sp.f0 = dfr0 + lane * 32 * kShareGroups; e.sp.f1 = min(dsum, e.sp.f0 + 32 * kShareGroups);
+                        __threadfence_block();
+                        e.ready = 1u;
+                    }
+                }
+                if (direct0) shade(wb, 0, dfr0, dfirst, tri0);
+                uint32_t done = 0;   // posted pieces this warp shaded itself
+                for (uint32_t p = 0; p < npiece; ++p) {
+                    uint32_t won = 1;
+                    if (p < fit) {
+                        if (lane == 0) won = atomicExch(&cq.q[qbase + p].taken, 1u) == 0u;
+                        won = __shfl_sync(0xffffffffu, won, 0);
+                        done += won;
+                    }
+                    const uint32_t f0 = dfr0 + p * 32 * kShareGroups;
+                    if (won) shade(wb, f0, min(dsum, f0 + 32 * kShareGroups), dfirst, tri0);
+                }
                 TR_PHASE(a, kTrShade);
-                TR_ADD(a, kTrGroups, (total_small + 31) / 32);
                 // the stage was written through the generic proxy: every writer fences before the TMA engine writes there again
                 fence_proxy_async();
                 __syncwarp();
                 if (claim_late) claim();
                 if (lane == 0) tma_store_wait_read();   // the last groups' copies have read the stage
-                if (lane == 0 && next < a.n_units) issue_load(next);
+                if (lane == 0 && next < a.n_units) issue_load(next, a.unit_tris);
+                if (fit) {   // other warps may still read this slice's records and list: wait before they are rewritten
+                    if (lane == 0) {
+                        if (done) atomicSub_block(&wb.left, done);
+                        while (*reinterpret_cast<volatile uint32_t*>(&wb.left) != 0u) __nanosleep(32);
+                        __threadfence_block();
+                    }
+                    __syncwarp();
+                }
             }
         }
 
-        // ---- the unit's records go to global memory for the fragment kernel: one TMA bulk store straight out of
-        // this warp's shared-memory slice (every writer fences its generic-proxy writes, then the barrier) ----
-        const bool any = __any_sync(0xffffffffu, cnt != 0) && (!direct || gm_all != 0);  // a fully direct unit leaves nothing for the fragment kernel
+        // ---- the pass's records go to global memory for the fragment kernel: one TMA bulk store straight out of
+        // this warp's shared-memory slice (every writer fences its generic-proxy writes, then the barrier).  A fully
+        // direct unit leaves nothing for the fragment kernel ----
+        const bool any = __any_sync(0xffffffffu, cnt != 0 && (!my_direct || (gm_all & hmask) != 0));
         if (any) {
             fence_proxy_async();
             __syncwarp();
@@ -752,6 +841,7 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
             }
         }
         unit = next;
+        pair = false;
         TR_PHASE(a, kTrUnitEnd);
     }
     // ---- help: tickets on the CTA's queue until no warp of the CTA can post any more ----
@@ -775,6 +865,21 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         }
         if (!__shfl_sync(0xffffffffu, (int)have, 0)) break;
         const CtaEntry& e = cq.q[t];
+        if (e.h < 0) {   // a shading piece: unless its owner got there first
+            if constexpr (kDirectOK) {
+                uint32_t won = 0;
+                if (lane == 0) won = atomicExch(&cq.q[t].taken, 1u) == 0u;
+                if (__shfl_sync(0xffffffffu, won, 0)) {
+                    WarpBlock<RK>& src = *reinterpret_cast<WarpBlock<RK>*>(smem + (size_t)e.sp.owner * sizeof(WarpBlock<RK>));
+                    cp_async_wait_all();   // this warp's wb.logtab, if it never shaded a unit of its own
+                    __syncwarp();
+                    shade(src, e.sp.f0, e.sp.f1, e.sp.first, e.sp.tri0);
+                    __syncwarp();
+                    if (lane == 0) { __threadfence_block(); atomicSub_block(&src.left, 1u); }   // its slice may be rewritten
+                }
+            }
+            continue;
+        }
         const RowState rs = e.rs;
         const int h = e.h;
         const uint32_t eu = e.unit, es = e.slot;

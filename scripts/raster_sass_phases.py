@@ -24,7 +24,7 @@ def source_lines(src):
     find = lambda pat, start=0: next(i + 1 for i in range(start, len(lines)) if re.search(pat, lines[i]))
     setup = find(r"cnt = setup_triangle<RK>\(")
     walk0, walk1 = find(r"const uint32_t mine = "), find(r"const uint32_t nh = ")
-    d0 = find(r"__noinline__ void direct_run\(")
+    d0 = find(r"__noinline__ \w+ direct_run\(")
     d1 = find(r"^}", d0)
     return lines, setup, (walk0, walk1), (d0, d1)
 
