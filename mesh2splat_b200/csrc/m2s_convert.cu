@@ -11,6 +11,10 @@ using namespace m2s;
 
 static unsigned long long* g_trace = nullptr;  // debugging aid for M2S_TRACE builds (scripts/trace_raster.py)
 M2S_EXPORT void m2s_debug_set_trace(void* p) { g_trace = (unsigned long long*)p; }
+// Test aid: conversions leave every small triangle to the fragment kernel (no direct path), the route the direct path's
+// records are compared against
+static bool g_direct_off = false;
+M2S_EXPORT void m2s_debug_set_direct_off(int off) { g_direct_off = off != 0; }
 
 // ---- the hot path -----------------------------------------------------------------------------
 uint64_t m2s::effective_cap(const m2s_dscene* s, const m2s_params* p, uint64_t out_capacity) {
@@ -57,7 +61,7 @@ static void convert_plan(const m2s_ctx* ctx, const m2s_dscene* s, const m2s_para
     pl->unit_tris = std::min<uint64_t>(std::max<uint64_t>((count + warps * rounds - 1) / (warps * rounds), 1), kUnitTris);
     pl->n_units = (count + pl->unit_tris - 1) / pl->unit_tris;
     pl->multi_round = pl->n_units > warps;
-    pl->direct_ok = klayout == M2S_LAYOUT_PACKED56 && pl->multi_round && world <= 1;
+    pl->direct_ok = klayout == M2S_LAYOUT_PACKED56 && pl->multi_round && world <= 1 && !g_direct_off;
     // the late claim evens out the weights of the direct units when each warp gets only two of them; with more units
     // per warp they average out anyway and the claim's exposed atomic round trip is not worth it (DESIGN §4)
     pl->claim_late = pl->direct_ok && pl->n_units < 3 * warps;

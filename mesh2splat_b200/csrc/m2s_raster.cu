@@ -10,7 +10,7 @@
 //   work unit = <= 32 consecutive triangles; a warp's first unit is static (global warp id), further ones are
 //     claimed from a global counter; the next unit's triangles are in flight (TMA) while this one is processed.
 //     Launches of 16-triangle units (ConvertPlan::pair_first): the first pass sets up units 2g and 2g + 1 on the two
-//     half warps, and the second unit's direct shading is shared with the CTA's other warps (CtaQueue)
+//     half warps.  A pass's direct shading is shared with the CTA's other warps (CtaQueue)
 //   TMA (cp.async.bulk + mbarrier complete_tx) stages the unit's 144 B/triangle into shared memory
 //   per-triangle stage, one LANE per triangle (converterGS.glsl:326-443): longest edge, face normal, dominant
 //     axis, orthographic uv, quaternion, UV->3D Jacobian scale; rasteriser set-up: 24.8 fixed-point window
@@ -86,7 +86,7 @@ struct __align__(128) WarpBlock {
     uint32_t itTotal[kStashItems];                // fragments per item
     uint64_t bar;
     double logtab[RK == 1 ? 32 : 1];              // PACKED56: the direct path's copy of ref_logf's table (kLogfTab)
-    uint32_t left;                                // shared pieces of this warp's second unit not yet shaded (CtaQueue)
+    uint32_t left;                                // posted pieces of this warp's direct pass not yet shaded (CtaQueue)
 };
 
 // The scene's descriptor tables as the set-up sees them: in shared memory when they fit (each CTA copies
@@ -461,8 +461,8 @@ __device__ __forceinline__ void count_blocks(const ConvertArgs& a, WarpBlock<RK>
 // others are done: it posts its tall triangles here, in pieces of kDeferBlocks row blocks, and every warp of the CTA that
 // has run out of units takes tickets.  Shared-memory atomics only: a grid-wide queue was tried (r02) and lost to the
 // serialisation of same-address global atomics (one per unit / per claim: 8-30 us at 2-30 k units).
-// The same queue shares the shading of a paired first pass's second unit (h < 0, SharePiece): pieces of kShareGroups
-// groups of 32 listed fragments, shaded by whichever warp of the CTA takes them first: the owner or a warp out of units.
+// The same queue shares the shading of a direct pass (h < 0, SharePiece): the pieces of kSharePiece listed fragments after
+// the owner's first kShareFirst, each shaded by whichever warp of the CTA takes it first: the owner or a warp out of units.
 struct SharePiece {
     unsigned long long first;     // output index of the owner's listed fragment 0
     uint32_t owner;               // warp of the CTA whose slice holds the records and the list
@@ -477,8 +477,15 @@ struct CtaEntry {
     uint32_t taken;               // shading pieces: set by the warp that shades it
     uint32_t pad;
 };
-constexpr uint32_t kCtaQueueCap = 48;
-constexpr uint32_t kShareGroups = 2;
+// Capacity and piece sizes of a direct pass's sharing: the queue takes the CTA's shared memory up to the 227 KB limit (58
+// entries of 88 B).  On the bench scene (H100, 16 warps per CTA, ~300 listed fragments per pass) an owner that keeps 192
+// fragments posts 33-45 pieces of 64 per CTA; one that keeps only 64 would post 63-74, the queue would be full before
+// the last warps post, and those would keep all their pieces (DESIGN.md section 4)
+constexpr uint32_t kCtaQueueCap = 58;
+constexpr uint32_t kShareFirst = 6 * 32;   // fragments of a direct pass its owner shades before the posted pieces
+constexpr uint32_t kSharePiece = 2 * 32;   // fragments per posted piece
+static_assert(kShareFirst % 32 == 0 && kSharePiece % 32 == 0 && 2 * M2S_DIRECT_MAX <= kShareFirst + 32 * kSharePiece,
+              "pieces start on a group; one lane posts each piece of a pass");
 struct CtaQueue {
     uint32_t tail;                // entries posted (may exceed the capacity: the poster keeps the overflow)
     uint32_t head;                // tickets taken
@@ -778,11 +785,14 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
                 __syncwarp();
                 TR_PHASE(a, kTrList);
                 const uint32_t tri0 = a.tri_first + t0;
-                // a paired pass posts its second unit's groups to the CTA's help queue, then shades its first unit: a warp that
-                // is out of units takes the pieces this warp has not reached (the late claim cannot balance a pass's weight)
-                uint32_t npiece = 0, qbase = 0, fit = 0;
-                if (direct1) {
-                    npiece = (tot1 + 32 * kShareGroups - 1) / (32 * kShareGroups);
+                // the pass's list [0, dsum) is cut into groups of 32 from 0, across the boundary of its two units: only the
+                // last group can be partial.  This warp shades the first kShareFirst fragments at once; the rest goes to the
+                // CTA's help queue in pieces of kSharePiece, which this warp then shades in order unless another warp has
+                // taken them: a warp that is out of units takes the pieces this warp has not reached (the late claim cannot
+                // balance a pass's weight)
+                const uint32_t npiece = dsum > kShareFirst ? (dsum - kShareFirst + kSharePiece - 1) / kSharePiece : 0u;
+                uint32_t qbase = 0, fit = 0;
+                if (npiece) {
                     if (lane == 0) qbase = atomicAdd_block(&cq.tail, npiece);
                     qbase = __shfl_sync(0xffffffffu, qbase, 0);
                     fit = qbase < kCtaQueueCap ? min(npiece, kCtaQueueCap - qbase) : 0u;   // the rest is this warp's own
@@ -793,12 +803,12 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
                         CtaEntry& e = cq.q[qbase + lane];
                         e.h = -1;
                         e.sp.first = dfirst; e.sp.owner = (uint32_t)warp; e.sp.tri0 = tri0;
-                        e.sp.f0 = dfr0 + lane * 32 * kShareGroups; e.sp.f1 = min(dsum, e.sp.f0 + 32 * kShareGroups);
+                        e.sp.f0 = kShareFirst + lane * kSharePiece; e.sp.f1 = min(dsum, e.sp.f0 + kSharePiece);
                         __threadfence_block();
                         e.ready = 1u;
                     }
                 }
-                if (direct0) shade(wb, 0, dfr0, dfirst, tri0);
+                shade(wb, 0, min(dsum, kShareFirst), dfirst, tri0);
                 uint32_t done = 0;   // posted pieces this warp shaded itself
                 for (uint32_t p = 0; p < npiece; ++p) {
                     uint32_t won = 1;
@@ -807,8 +817,8 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
                         won = __shfl_sync(0xffffffffu, won, 0);
                         done += won;
                     }
-                    const uint32_t f0 = dfr0 + p * 32 * kShareGroups;
-                    if (won) shade(wb, f0, min(dsum, f0 + 32 * kShareGroups), dfirst, tri0);
+                    const uint32_t f0 = kShareFirst + p * kSharePiece;
+                    if (won) shade(wb, f0, min(dsum, f0 + kSharePiece), dfirst, tri0);
                 }
                 TR_PHASE(a, kTrShade);
                 // the stage was written through the generic proxy: every writer fences before the TMA engine writes there again

@@ -33,7 +33,7 @@ t = t[live]
 mhz = t[:, CYC].sum() / t[:, NS].sum() * 1e3
 print(f"{which} R={R} layout={layout}: device_ms={out.device_ms:.4f} total={out.total} warps={len(t)} SM clock {mhz:.0f} MHz (clock64 / globaltimer)")
 print(f"units/warp p50 {np.median(t[:, UNITS]):.0f} max {t[:, UNITS].max():.0f}; direct units/warp p50 {np.median(t[:, DUNITS]):.0f}; "
-      f"32-fragment groups/warp p50 {np.median(t[:, GROUPS]):.1f} max {t[:, GROUPS].max():.0f}")
+      f"32-fragment groups/warp p50 {np.median(t[:, GROUPS]):.1f} max {t[:, GROUPS].max():.0f} total {t[:, GROUPS].sum():.0f}")
 us = lambda c: c / mhz
 print(f"{'phase (per-warp sum)':24s} {'p50 us':>8s} {'p90 us':>8s} {'mean us':>8s}")
 for k, n in enumerate(PHASES + ["entry (tables)"]):
