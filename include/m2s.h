@@ -41,6 +41,8 @@
  *   SceneManager::loadPly + parsers::loadPlyFile                 m2s_ply_parse_header, m2s_ply_decode_enqueue,
  *     (src/utils/SceneManager.cpp:37-47,                         m2s_ply_read; M2S_VIEW_PLY / M2S_VIEW_PLY_PBR
  *      src/parsers/parsers.cpp:516-629)                          as the viewer passes' input
+ *   beyond the reference: a loaded .ply's view-dependent colour  m2s_ply_read_sh, m2s_ply_decode_sh_enqueue,
+ *     (the SH rest coefficients, graphdeco's computeColorFromSH) m2s_prepass_sh, m2s_prepass_sh_enqueue
  *
  * Plain pointers and sizes only; no C++/torch types.  All functions return an
  * m2s_status; m2s_last_error() gives the thread-local message of the last
@@ -278,7 +280,9 @@ m2s_status m2s_ply_write(const char* path, const void* h_ref96, uint64_t count, 
  * bit-identical to it on all 2^32 inputs (tests/test_gpu_codec.py); against a glibc that uses its non-FMA variant
  * scale.xyz and color.a may differ by 1 ulp, every other field is bit-exact.  The writers' encodings are exact the same
  * way: SH0 = (c - 0.5f) / SH_COEFF0 (the IEEE quotient), the opacity logit and the log-scale with glibc's logf, in the
- * conversion's .ply and PACKED56 layouts, m2s_ply_encode and m2s_convert_file.  Denormals are kept.  SH rest coefficients are skipped, as in the reference.
+ * conversion's .ply and PACKED56 layouts, m2s_ply_encode and m2s_convert_file.  Denormals are kept.  The records hold no
+ * SH rest coefficients; m2s_ply_read_sh / m2s_ply_decode_sh_enqueue also copy them into a separate buffer (beyond the
+ * reference, which skips them; see m2s_ply_info.sh_degree).
  * Property rules (happly): the properties are found by name in the first element "vertex" (order and extra properties do
  * not matter); x y z f_dc_0..2 opacity scale_0..2 rot_0..3 are required; every property read must be float / float32
  * (happly does not narrow a double); has_pbr = nx ny nz metallicFactor roughnessFactor all present, and 1 for a file of 0
@@ -299,6 +303,10 @@ enum {   /* index into m2s_ply_info.offset */
     M2S_PLY_ROT_0, M2S_PLY_ROT_1, M2S_PLY_ROT_2, M2S_PLY_ROT_3
 };
 #define M2S_PLY_MAX_STRIDE 4096u   /* bytes per vertex row the decoder takes */
+#define M2S_SH_REST_MAX 45         /* f_rest_* floats of a degree-3 file */
+/* floats per gaussian in an SH buffer of degree d (0..3): 3 K rounded up to a multiple of 4, so each gaussian's block is
+ * 16-byte aligned (12, 24, 48) */
+#define M2S_SH_FLOATS(d) ((d) == 1 ? 12u : (d) == 2 ? 24u : (d) == 3 ? 48u : 0u)
 typedef struct m2s_ply_info {
     uint64_t vertex_count;
     uint64_t body_offset;            /* file offset of vertex row 0 */
@@ -306,6 +314,12 @@ typedef struct m2s_ply_info {
     uint32_t has_pbr;                /* loadPlyFile's hasPbr */
     int32_t offset[M2S_PLY_PROPS];   /* byte offset in the row of x y z nx ny nz f_dc_0..2 metallicFactor roughnessFactor
                                         opacity scale_0..2 rot_0..3; -1 = absent */
+    /* SH rest coefficients (beyond the reference).  sh_degree = d (1..3) when the vertex element's f_rest_* properties
+     * are exactly f_rest_0 .. f_rest_{3K-1}, K = (d+1)^2 - 1 = 3, 8 or 15, in any order and all float; 0 in every other
+     * case (none, a partial or odd-sized set, a non-float one), which never makes a file fail to load.  The file order is
+     * graphdeco's, channel-major: coefficient k (1..K) of channel c is f_rest_{c K + k - 1}. */
+    uint32_t sh_degree;
+    int32_t f_rest[M2S_SH_REST_MAX]; /* byte offset in the row of f_rest_i, i < 3K; -1 = absent (all -1 when sh_degree 0) */
 } m2s_ply_info;
 /* Host only.  bytes/size: the first `size` bytes of the file (the whole file, or any prefix that holds the header);
  * file_size: the size of the whole file.  Never reads outside [bytes, bytes + size). */
@@ -319,6 +333,15 @@ m2s_status m2s_ply_decode_enqueue(m2s_ctx* ctx, const m2s_ply_info* info, const 
  * while the next block is read from the file.  d_ref96 == NULL: only fills *info (the probe that sizes the buffer).
  * capacity < vertex_count: M2S_E_CAPACITY, *info filled, nothing written. */
 m2s_status m2s_ply_read(m2s_ctx* ctx, const char* path, void* d_ref96, uint64_t capacity, m2s_ply_info* info);
+/* The decode and the load that also copy the SH rest coefficients (m2s_ply_decode_enqueue and m2s_ply_read are these calls
+ * with d_sh NULL; the records are the same with and without d_sh).  d_sh: count (capacity) x M2S_SH_FLOATS(info->sh_degree)
+ * floats, 16-byte aligned; gaussian i's block holds the r, g, b of coefficient k (1..K) at floats 3 (k - 1) .. 3 (k - 1) + 2
+ * (coefficient-major), copied bit for bit from the file, and zero padding.  Nothing is written to d_sh when sh_degree is 0;
+ * d_sh NULL skips the coefficients. */
+m2s_status m2s_ply_decode_sh_enqueue(m2s_ctx* ctx, const m2s_ply_info* info, const void* d_rows, uint64_t count,
+                                     void* d_ref96, float* d_sh, void* stream);
+m2s_status m2s_ply_read_sh(m2s_ctx* ctx, const char* path, void* d_ref96, float* d_sh, uint64_t capacity,
+                           m2s_ply_info* info);
 /* Payload bytes m2s_ply_read copied host -> device on this context so far (accounting for benchmarks). */
 uint64_t m2s_ply_h2d_bytes(const m2s_ctx* ctx);
 /* `layout` values of m2s_prepass* and m2s_shadow_map* for REF96 records as loadPlyFile fills them (not conversion
@@ -382,6 +405,23 @@ m2s_status m2s_prepass_enqueue(m2s_ctx* ctx, const void* d_records, uint64_t cou
 /* Synchronous variant on the context stream; *valid receives the counter. */
 m2s_status m2s_prepass(m2s_ctx* ctx, const void* d_records, uint64_t count, const m2s_prepass_params* params,
                        void* d_quads, float* d_depths, uint32_t* valid);
+/* The prepass with view-dependent colour from the SH rest coefficients of a loaded .ply (beyond the reference: graphdeco's
+ * computeColorFromSH).  Layouts M2S_VIEW_PLY and M2S_VIEW_PLY_PBR only.  d_sh: count x M2S_SH_FLOATS(buffer_degree)
+ * floats as m2s_ply_read_sh writes them (16-byte aligned); sh_degree (0..buffer_degree) is the degree evaluated.  For a
+ * gaussian that survives the frustum cull, in render modes 0 and 6 (the albedo the lighting sees):
+ *   c = the translation column of inverse(V M), in fp64 from the fp32 matrices, rounded once to fp32 (the camera in
+ *       model space); d = p - c for the record's position p; inv = 1 / sqrt((dx dx + dy dy) + dz dz); (x, y, z) = d inv;
+ *   rest = sum over k = 1..K of B_k coeff_k in k order from 0 (0 when the length is 0), B_k graphdeco's basis with its
+ *       constants and signs; colour = max(record colour + rest, 0) per channel (glm::max: NaN kept), alpha unchanged.
+ * Every operation is one fp32 rounding, without contraction.  Modes 1 and 2 and sh_degree 0 give m2s_prepass's output.
+ * M2S_E_INVALID before any launch for another layout, buffer_degree > 3, sh_degree > buffer_degree, d_sh NULL with
+ * sh_degree > 0, or a singular V M.  Everything else as m2s_prepass_enqueue / m2s_prepass. */
+m2s_status m2s_prepass_sh_enqueue(m2s_ctx* ctx, const void* d_records, uint64_t count, const uint64_t* d_count,
+                                  const m2s_prepass_params* params, const float* d_sh, uint32_t buffer_degree,
+                                  uint32_t sh_degree, void* d_quads, float* d_depths, uint32_t* d_valid, void* stream);
+m2s_status m2s_prepass_sh(m2s_ctx* ctx, const void* d_records, uint64_t count, const m2s_prepass_params* params,
+                          const float* d_sh, uint32_t buffer_degree, uint32_t sh_degree, void* d_quads, float* d_depths,
+                          uint32_t* valid);
 
 /* ---- the mesh depth pre-pass (SURVEY 8 f-9) and the prepass's mesh depth test -----------------------------------------
  * DepthPrepass::execute (src/renderer/renderPasses/DepthPrepass.cpp:8-49) + depthPrepassVS/PS.glsl: every triangle of

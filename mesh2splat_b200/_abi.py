@@ -26,6 +26,9 @@ VIEW_PLY, VIEW_PLY_PBR = 16, 17
 PLY_PROPS = ("x", "y", "z", "nx", "ny", "nz", "f_dc_0", "f_dc_1", "f_dc_2", "metallicFactor", "roughnessFactor", "opacity",
              "scale_0", "scale_1", "scale_2", "rot_0", "rot_1", "rot_2", "rot_3")
 PLY_MAX_STRIDE = 4096
+# SH rest coefficients of a loaded .ply (m2s_ply_info.sh_degree): floats per gaussian of an SH buffer by degree
+SH_REST_MAX = 45
+SH_FLOATS = {0: 0, 1: 12, 2: 24, 3: 48}
 # m2s_debug_codec_eval function ids (m2s_codec.cu; not in m2s.h)
 CODEC_SH0, CODEC_LOGIT, CODEC_LOG_SCALE, CODEC_EXPF, CODEC_SIGMOID = range(5)
 
@@ -33,7 +36,7 @@ CODEC_SH0, CODEC_LOGIT, CODEC_LOG_SCALE, CODEC_EXPF, CODEC_SIGMOID = range(5)
 class m2s_ply_info(C.Structure):
     """include/m2s.h: what m2s_ply_parse_header reads from a .ply header."""
     _fields_ = [("vertex_count", C.c_uint64), ("body_offset", C.c_uint64), ("row_stride", C.c_uint32), ("has_pbr", C.c_uint32),
-                ("offset", C.c_int32 * len(PLY_PROPS))]
+                ("offset", C.c_int32 * len(PLY_PROPS)), ("sh_degree", C.c_uint32), ("f_rest", C.c_int32 * SH_REST_MAX)]
 
     def offsets(self) -> dict:
         """{property name: byte offset in the row} of the properties present."""

@@ -25,6 +25,7 @@ SYMBOLS = [
     "m2s_prepass_mesh_depth", "m2s_prepass_mesh_depth_enqueue", "m2s_mesh_render", "m2s_mesh_render_enqueue",
     "m2s_deferred_light_split", "m2s_deferred_light_split_enqueue",
     "m2s_ply_parse_header", "m2s_ply_decode_enqueue", "m2s_ply_read", "m2s_ply_h2d_bytes",
+    "m2s_ply_decode_sh_enqueue", "m2s_ply_read_sh", "m2s_prepass_sh", "m2s_prepass_sh_enqueue",
 ]
 
 
@@ -153,6 +154,14 @@ def lib() -> C.CDLL:
     L.m2s_ply_read.argtypes = [vp, C.c_char_p, vp, u64, C.POINTER(_abi.m2s_ply_info)]
     L.m2s_ply_h2d_bytes.restype = u64
     L.m2s_ply_h2d_bytes.argtypes = [vp]
+    L.m2s_ply_decode_sh_enqueue.restype = i32
+    L.m2s_ply_decode_sh_enqueue.argtypes = [vp, C.POINTER(_abi.m2s_ply_info), vp, u64, vp, vp, vp]
+    L.m2s_ply_read_sh.restype = i32
+    L.m2s_ply_read_sh.argtypes = [vp, C.c_char_p, vp, vp, u64, C.POINTER(_abi.m2s_ply_info)]
+    L.m2s_prepass_sh_enqueue.restype = i32
+    L.m2s_prepass_sh_enqueue.argtypes = [vp, vp, u64, vp, C.POINTER(_abi.m2s_prepass_params), vp, u32, u32, vp, vp, vp, vp]
+    L.m2s_prepass_sh.restype = i32
+    L.m2s_prepass_sh.argtypes = [vp, vp, u64, C.POINTER(_abi.m2s_prepass_params), vp, u32, u32, vp, vp, C.POINTER(u32)]
     _lib = L
     return L
 

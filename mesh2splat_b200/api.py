@@ -241,12 +241,15 @@ class Context:
                                         total.data_ptr() if total is not None else None, stream or None))
 
     def prepass(self, records, count: int, layout: int, world_to_view, view_to_clip, model_to_world, resolution, near_far,
-                std_dev: float, render_mode: int = 0, quads=None, depths=None, mesh_depth=None):
+                std_dev: float, render_mode: int = 0, quads=None, depths=None, mesh_depth=None, sh=None, sh_degree=None):
         """GaussiansPrepass::execute on device-resident records (a torch uint8 tensor, e.g. ConvertOutput.data): returns
         (quads [m, 24] float32, depths [m] float32) as numpy arrays, in atomic arrival order (m2s_prepass).
         quads / depths: optional caller-owned device tensors of at least count * 96 bytes / count floats.
         mesh_depth: None, or a float32 device tensor (H, W) from mesh_depth(..., depth=...): the prepass with the mesh
-        depth test (m2s_prepass_mesh_depth)."""
+        depth test (m2s_prepass_mesh_depth).
+        sh / sh_degree: view-dependent colour from a loaded .ply's SH rest coefficients (m2s_prepass_sh; layouts VIEW_PLY
+        and VIEW_PLY_PBR).  sh: the (count, 12 | 24 | 48) float32 device tensor of ply_read_sh, whose width sets the
+        buffer's degree; sh_degree: the degree evaluated (default the buffer's).  Both None: m2s_prepass."""
         import torch
         dev = records.device
         if quads is None:
@@ -255,7 +258,20 @@ class Context:
             depths = torch.empty(max(1, count), dtype=torch.float32, device=dev)
         p = _abi.make_prepass_params(world_to_view, view_to_clip, model_to_world, resolution, near_far, std_dev, render_mode, layout)
         valid = C.c_uint32(0)
-        if mesh_depth is None:
+        if sh is not None or sh_degree is not None:
+            if mesh_depth is not None:
+                raise ValueError("sh and mesh_depth do not combine (a loaded .ply never reads the mesh depth map)")
+            buffer_degree = 0
+            if sh is not None:
+                degrees = {f: d for d, f in _abi.SH_FLOATS.items() if f}
+                if sh.dim() != 2 or sh.shape[1] not in degrees or sh.dtype != torch.float32 or sh.device != dev or not sh.is_contiguous():
+                    raise ValueError("sh must be a contiguous (count, 12 | 24 | 48) float32 tensor on the records' device")
+                buffer_degree = degrees[sh.shape[1]]
+            torch.cuda.synchronize(dev)   # the coefficients torch holds are ready before the context stream reads them
+            check(lib().m2s_prepass_sh(self.handle, records.data_ptr(), count, C.byref(p), sh.data_ptr() if sh is not None else None,
+                                       buffer_degree, buffer_degree if sh_degree is None else int(sh_degree), quads.data_ptr(),
+                                       depths.data_ptr(), C.byref(valid)))
+        elif mesh_depth is None:
             check(lib().m2s_prepass(self.handle, records.data_ptr(), count, C.byref(p), quads.data_ptr(), depths.data_ptr(), C.byref(valid)))
         else:
             if (mesh_depth.dim() != 2 or mesh_depth.dtype != torch.float32 or mesh_depth.device != dev
@@ -490,6 +506,30 @@ class Context:
         check(lib().m2s_ply_read(self.handle, path.encode(), out.data_ptr(), out.numel() // 96, C.byref(info)))
         return out[: n * 96], n, bool(info.has_pbr)
 
+    def ply_read_sh(self, path: str, out=None, sh=None):
+        """ply_read that also loads the SH rest coefficients (m2s_ply_read_sh): returns (records, sh, count, has_pbr,
+        sh_degree); sh is a (count, M2S_SH_FLOATS(sh_degree)) float32 device tensor, coefficient-major with zero padding,
+        or None for a file of degree 0.  out / sh: optional caller-owned device tensors (sh float32, at least count *
+        M2S_SH_FLOATS(sh_degree) values); M2SError with M2S_E_CAPACITY when either holds fewer than count gaussians."""
+        torch = _torch()
+        info = _abi.m2s_ply_info()
+        check(lib().m2s_ply_read_sh(self.handle, path.encode(), None, None, 0, C.byref(info)))
+        n, deg = int(info.vertex_count), int(info.sh_degree)
+        nf = _abi.SH_FLOATS[deg]
+        dev = torch.device("cuda", self.device)
+        if out is None:
+            out = torch.empty(max(1, n) * 96, dtype=torch.uint8, device=dev)
+        if nf and sh is None:
+            sh = torch.empty(max(1, n) * nf, dtype=torch.float32, device=dev)
+        cap = out.numel() // 96
+        if nf:
+            if sh.dtype != torch.float32 or not sh.is_contiguous():
+                raise ValueError("sh must be a contiguous float32 device tensor")
+            cap = min(cap, sh.numel() // nf)
+        torch.cuda.synchronize(out.device)   # the buffers torch hands out are idle before the context stream writes them
+        check(lib().m2s_ply_read_sh(self.handle, path.encode(), out.data_ptr(), sh.data_ptr() if nf else None, cap, C.byref(info)))
+        return out[: n * 96], (sh.reshape(-1)[: n * nf].view(n, nf) if nf else None), n, bool(info.has_pbr), deg
+
     def ply_h2d_bytes(self) -> int:
         return int(lib().m2s_ply_h2d_bytes(self.handle))
 
@@ -554,6 +594,8 @@ class RenderContext:
         self.lastResult: ConvertOutput | None = None
         self.format = 0                      # u_format: 0 the conversion's records, 1 a loaded .ply (RenderContext.hpp)
         self.plyHasPbr = False               # format 1: the .ply carries normals and metallic / roughness
+        self.shCoefficients = None           # format 1 loaded withSh: (n, 12 | 24 | 48) float32 device tensor (beyond the reference)
+        self.shDegree = 0                    # ... its degree (0: no view-dependent colour)
 
     def viewLayout(self) -> int:
         """The `layout` the viewer passes (prepass, shadow_map) take for gaussianBuffer."""
@@ -583,18 +625,24 @@ class SceneManager:
             print(f"Failed to parse GLTF file: {filePath}: {e}")
             return False
 
-    def loadPly(self, filePath: str) -> bool:
+    def loadPly(self, filePath: str, withSh: bool = False) -> bool:
         """SceneManager::loadPly (SceneManager.cpp:37-47) + parsers::loadPlyFile: the file's gaussians become
-        gaussianBuffer (REF96 on the device), format 1, plyHasPbr from the file.  Deviation: a file the loader does not
-        take returns False and leaves the previous gaussians in place (the reference prints the error and returns true)."""
+        gaussianBuffer (REF96 on the device), format 1, plyHasPbr from the file.  withSh (beyond the reference): also
+        load the SH rest coefficients into shCoefficients / shDegree (prepass(sh=...)); without it they are None / 0, as
+        the reference skips them.  Deviation: a file the loader does not take returns False and leaves the previous
+        gaussians in place (the reference prints the error and returns true)."""
         rc = self.renderContext
         try:
             ply_parse_file(filePath)   # header and size checked on the host before anything reaches the device
-            records, n, has_pbr = rc.ctx.ply_read(filePath)
+            if withSh:
+                records, sh, n, has_pbr, degree = rc.ctx.ply_read_sh(filePath)
+            else:
+                (records, n, has_pbr), sh, degree = rc.ctx.ply_read(filePath), None, 0
         except (OSError, M2SError) as e:
             print(f"Error loading PLY file: {filePath}: {e}")
             return False
         rc.gaussianBuffer, rc.numberOfGaussians, rc.format, rc.plyHasPbr = records, n, 1, has_pbr
+        rc.shCoefficients, rc.shDegree = sh, degree
         return True
 
     def exportPly(self, outputFile: str, exportFormat: int = 0) -> None:

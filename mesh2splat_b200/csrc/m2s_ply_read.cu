@@ -5,7 +5,8 @@
 // Shape: the header is parsed on the host (happly's line rules); the body goes from the file through the two pinned
 // staging buffers of the context to a two-slot device staging area, and a streaming kernel decodes the raw rows into
 // 96-byte records (row_stride bytes in, 96 out, bandwidth-bound).  The file read of block b+1 overlaps the copy and the
-// decode of block b.
+// decode of block b.  Beyond the reference, the same kernel also copies the SH rest coefficients into a separate buffer
+// (m2s_ply_read_sh / m2s_ply_decode_sh_enqueue).
 #include <sys/stat.h>
 
 #include <cstdio>
@@ -78,6 +79,36 @@ struct PlyProp { std::string name; uint32_t bytes; bool is_float; };
 struct PlyElement { std::string name; uint64_t count; std::vector<PlyProp> props; bool has_list = false; };
 
 m2s_status format_error(const std::string& msg) { set_error("m2s_ply: " + msg); return M2S_E_FORMAT; }
+
+// The SH rest coefficients of the vertex element (beyond the reference, m2s.h): sh_degree d and the f_rest offsets when the
+// f_rest_* properties are exactly f_rest_0 .. f_rest_{3K-1}, all float; otherwise info is left at degree 0.
+void sh_rest_props(const PlyElement& v, m2s_ply_info* info) {
+    std::vector<std::pair<const PlyProp*, uint64_t>> rest;   // the f_rest_* properties and their byte offsets
+    uint64_t off = 0;
+    for (const PlyProp& p : v.props) {
+        if (starts(p.name, "f_rest_")) rest.push_back({&p, off});
+        off += p.bytes;
+    }
+    uint32_t d = 0;
+    for (uint32_t k = 1; k <= 3; ++k)
+        if (rest.size() == 3u * ((k + 1) * (k + 1) - 1)) d = k;
+    if (d == 0) return;
+    int32_t f[M2S_SH_REST_MAX];
+    for (int32_t& o : f) o = -1;
+    for (const auto& r : rest) {   // 3K properties, each a distinct f_rest_i with i < 3K: exactly the set
+        const std::string idx = r.first->name.substr(7);
+        if (!r.first->is_float || idx.empty() || idx.size() > 2 || (idx.size() == 2 && idx[0] == '0')) return;
+        uint32_t i = 0;
+        for (char ch : idx) {
+            if (ch < '0' || ch > '9') return;
+            i = i * 10 + (uint32_t)(ch - '0');
+        }
+        if (i >= rest.size() || f[i] >= 0) return;
+        f[i] = (int32_t)r.second;
+    }
+    info->sh_degree = d;
+    std::memcpy(info->f_rest, f, sizeof(f));
+}
 
 }  // namespace
 
@@ -167,6 +198,7 @@ m2s_status ply_parse_header(const unsigned char* bytes, size_t size, uint64_t fi
         info->offset[k] = (int32_t)std::min<uint64_t>(off, INT32_MAX);
     }
     if (stride > M2S_PLY_MAX_STRIDE) return format_error("vertex rows of " + std::to_string(stride) + " bytes (at most 4096 supported)");
+    sh_rest_props(*v, info);
     bool pbr = true;
     for (int k : kPbrProps) pbr = pbr && info->offset[k] >= 0;
     info->vertex_count = v->count;
@@ -191,6 +223,9 @@ struct PlyDecodeArgs {
     uint32_t stride, rows_per_warp, has_pbr;
     int32_t off[M2S_PLY_PROPS];
     float4* out;
+    float4* sh;                        // NULL: no SH rest coefficients
+    uint32_t sh_vec;                   // float4 per gaussian in sh: M2S_SH_FLOATS(sh_degree) / 4
+    int32_t sh_off[M2S_SH_FLOATS(3)];  // byte offset in the row of each float of a gaussian's SH block, -1 = zero padding
 };
 
 // the float at byte p of the shared stage (any alignment: odd strides and offsets)
@@ -201,7 +236,9 @@ __device__ __forceinline__ float ld_f32(const unsigned char* p) {
 __global__ void __launch_bounds__(kDecodeThreads) ply_decode_kernel(const __grid_constant__ PlyDecodeArgs a) {
     __shared__ uint4 stage[kDecodeThreads / 32][kWarpStage / 16 + 2];   // + 32 B: the span's 16-byte-aligned cover
     __shared__ unsigned long long tab[32];
+    __shared__ int32_t sh_off[M2S_SH_FLOATS(3)];   // a.sh_off: the lanes of a warp read different entries
     if (threadIdx.x < 32) tab[threadIdx.x] = kExp2Tab[threadIdx.x];
+    if (a.sh && threadIdx.x < M2S_SH_FLOATS(3)) sh_off[threadIdx.x] = a.sh_off[threadIdx.x];
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const unsigned long long r0 = ((unsigned long long)blockIdx.x * (kDecodeThreads / 32) + warp) * a.rows_per_warp;
@@ -242,6 +279,21 @@ __global__ void __launch_bounds__(kDecodeThreads) ply_decode_kernel(const __grid
         }
         q5 = a.has_pbr ? make_float4(f(M2S_PLY_METALLIC), f(M2S_PLY_ROUGHNESS), 0.0f, 0.0f) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
+    // ---- the SH rest coefficients (m2s_ply_decode_sh_enqueue): gathered from the rows still in the stage and stored
+    // straight to the caller's buffer, the warp's blocks as one contiguous span of 16-byte stores (the 8 KB stage holds
+    // the rows; 32 blocks of up to 192 B do not fit beside them) ----
+    if (a.sh) {
+        const unsigned char* rows = reinterpret_cast<const unsigned char*>(stage[warp]) + (s - lo);
+        float4* dst = a.sh + r0 * a.sh_vec;
+        for (uint32_t i = lane; i < nrows * a.sh_vec; i += 32) {
+            const uint32_t r = i / a.sh_vec, j = (i - r * a.sh_vec) * 4;
+            const unsigned char* row = rows + (size_t)r * a.stride;
+            float v[4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) v[k] = sh_off[j + k] < 0 ? 0.0f : ld_f32(row + sh_off[j + k]);
+            __stcs(dst + i, make_float4(v[0], v[1], v[2], v[3]));
+        }
+    }
     __syncwarp();   // every lane has read its row: the stage takes the warp's records
     if ((uint32_t)lane < nrows) {
         float4* r = reinterpret_cast<float4*>(stage[warp]) + lane * 6;
@@ -253,7 +305,8 @@ __global__ void __launch_bounds__(kDecodeThreads) ply_decode_kernel(const __grid
     for (uint32_t i = lane; i < nrows * 6; i += 32) __stcs(dst + i, src[i]);
 }
 
-cudaError_t ply_decode_launch(const m2s_ply_info* info, const void* d_rows, uint64_t count, void* d_ref96, cudaStream_t stream) {
+// d_sh: NULL, or the SH blocks of the `count` rows (info->sh_degree 1..3)
+cudaError_t ply_decode_launch(const m2s_ply_info* info, const void* d_rows, uint64_t count, void* d_ref96, float* d_sh, cudaStream_t stream) {
     if (count == 0) return cudaSuccess;
     PlyDecodeArgs a;
     std::memset(&a, 0, sizeof(a));
@@ -264,6 +317,12 @@ cudaError_t ply_decode_launch(const m2s_ply_info* info, const void* d_rows, uint
     a.has_pbr = info->has_pbr;
     for (int k = 0; k < M2S_PLY_PROPS; ++k) a.off[k] = info->offset[k] < 0 ? 0 : info->offset[k];   // absent: never read (has_pbr 0)
     a.out = static_cast<float4*>(d_ref96);
+    if (d_sh && info->sh_degree) {   // coefficient k (1..K) of channel c: float 3 (k - 1) + c of the block, f_rest_{c K + k - 1}
+        const uint32_t K = (info->sh_degree + 1) * (info->sh_degree + 1) - 1, nf = M2S_SH_FLOATS(info->sh_degree);
+        a.sh = reinterpret_cast<float4*>(d_sh);
+        a.sh_vec = nf / 4;
+        for (uint32_t j = 0; j < nf; ++j) a.sh_off[j] = j < 3 * K ? info->f_rest[(j % 3) * K + j / 3] : -1;
+    }
     const unsigned long long warps = (count + a.rows_per_warp - 1) / a.rows_per_warp;
     const unsigned long long blocks = (warps + kDecodeThreads / 32 - 1) / (kDecodeThreads / 32);
     ply_decode_kernel<<<(unsigned)blocks, kDecodeThreads, 0, stream>>>(a);
@@ -277,6 +336,7 @@ using namespace m2s;
 static void ply_info_clear(m2s_ply_info* info) {
     std::memset(info, 0, sizeof(*info));
     for (int k = 0; k < M2S_PLY_PROPS; ++k) info->offset[k] = -1;
+    for (int k = 0; k < M2S_SH_REST_MAX; ++k) info->f_rest[k] = -1;
 }
 
 M2S_EXPORT m2s_status m2s_ply_parse_header(const void* bytes, size_t size, uint64_t file_size, m2s_ply_info* info) {
@@ -288,8 +348,8 @@ M2S_EXPORT m2s_status m2s_ply_parse_header(const void* bytes, size_t size, uint6
     return st;
 }
 
-M2S_EXPORT m2s_status m2s_ply_decode_enqueue(m2s_ctx* ctx, const m2s_ply_info* info, const void* d_rows, uint64_t count, void* d_ref96,
-                                             void* stream) {
+M2S_EXPORT m2s_status m2s_ply_decode_sh_enqueue(m2s_ctx* ctx, const m2s_ply_info* info, const void* d_rows, uint64_t count, void* d_ref96,
+                                                float* d_sh, void* stream) {
     const char* fn = "m2s_ply_decode";
     if (!ctx || !info || (count && (!d_rows || !d_ref96))) return invalid(fn, "NULL argument");
     if (info->row_stride < 1 || info->row_stride > M2S_PLY_MAX_STRIDE) return invalid(fn, "row_stride must be 1..4096");
@@ -300,14 +360,28 @@ M2S_EXPORT m2s_status m2s_ply_decode_enqueue(m2s_ctx* ctx, const m2s_ply_info* i
         if ((needed && o < 0) || (o >= 0 && (uint32_t)o + 4u > info->row_stride))
             return invalid(fn, std::string("offset of '") + kPlyNames[k] + "' outside the row");
     }
+    if (d_sh) {
+        if (info->sh_degree > 3) return invalid(fn, "sh_degree must be 0..3");
+        const uint32_t K = (info->sh_degree + 1) * (info->sh_degree + 1) - 1;
+        for (uint32_t i = 0; i < 3 * K; ++i)
+            if (info->f_rest[i] < 0 || (uint32_t)info->f_rest[i] + 4u > info->row_stride)
+                return invalid(fn, "offset of 'f_rest_" + std::to_string(i) + "' outside the row");
+    }
     if (count >= (1ull << 32)) return invalid(fn, "too many rows (< 2^32 supported)");
-    if (!aligned_ok(fn, "the record buffer must be 16-byte aligned", {{d_ref96, 16}})) return M2S_E_INVALID;
+    if (!aligned_ok(fn, "the record buffer must be 16-byte aligned", {{d_ref96, 16}}) ||
+        !aligned_ok(fn, "the SH buffer must be 16-byte aligned", {{d_sh, 16}}))
+        return M2S_E_INVALID;
     CUDA_TRY(cudaSetDevice(ctx->device));
-    CUDA_TRY(ply_decode_launch(info, d_rows, count, d_ref96, pick_stream(ctx, stream)));
+    CUDA_TRY(ply_decode_launch(info, d_rows, count, d_ref96, d_sh, pick_stream(ctx, stream)));
     return M2S_OK;
 }
 
-M2S_EXPORT m2s_status m2s_ply_read(m2s_ctx* ctx, const char* path, void* d_ref96, uint64_t capacity, m2s_ply_info* info) {
+M2S_EXPORT m2s_status m2s_ply_decode_enqueue(m2s_ctx* ctx, const m2s_ply_info* info, const void* d_rows, uint64_t count, void* d_ref96,
+                                             void* stream) {
+    return m2s_ply_decode_sh_enqueue(ctx, info, d_rows, count, d_ref96, nullptr, stream);
+}
+
+M2S_EXPORT m2s_status m2s_ply_read_sh(m2s_ctx* ctx, const char* path, void* d_ref96, float* d_sh, uint64_t capacity, m2s_ply_info* info) {
     const char* fn = "m2s_ply_read";
     if (!ctx || !path || !info) return invalid(fn, "NULL argument");
     ply_info_clear(info);
@@ -328,8 +402,11 @@ M2S_EXPORT m2s_status m2s_ply_read(m2s_ctx* ctx, const char* path, void* d_ref96
         set_error("m2s_ply_read: " + std::to_string(n) + " vertices, capacity " + std::to_string(capacity));
         return M2S_E_CAPACITY;
     }
-    if (!aligned_ok(fn, "the record buffer must be 16-byte aligned", {{d_ref96, 16}})) return M2S_E_INVALID;
+    if (!aligned_ok(fn, "the record buffer must be 16-byte aligned", {{d_ref96, 16}}) ||
+        !aligned_ok(fn, "the SH buffer must be 16-byte aligned", {{d_sh, 16}}))
+        return M2S_E_INVALID;
     if (n == 0) return M2S_OK;
+    const uint32_t sh_floats = d_sh ? M2S_SH_FLOATS(info->sh_degree) : 0u;
     CUDA_TRY(cudaSetDevice(ctx->device));
     for (int i = 0; i < 2; ++i)
         if (!ctx->h_stage[i]) CUDA_TRY(cudaMallocHost(&ctx->h_stage[i], m2s_ctx::kStageBytes));
@@ -358,7 +435,9 @@ M2S_EXPORT m2s_status m2s_ply_read(m2s_ctx* ctx, const char* path, void* d_ref96
         }
         unsigned char* d = d_slots + slot * slot_bytes;
         e = cudaMemcpyAsync(d, ctx->h_stage[slot], bytes, cudaMemcpyHostToDevice, ctx->stream);
-        if (e == cudaSuccess) e = ply_decode_launch(info, d, rows, static_cast<unsigned char*>(d_ref96) + first * 96, ctx->stream);
+        if (e == cudaSuccess)
+            e = ply_decode_launch(info, d, rows, static_cast<unsigned char*>(d_ref96) + first * 96, sh_floats ? d_sh + first * sh_floats : nullptr,
+                                  ctx->stream);
         if (e == cudaSuccess) e = cudaEventRecord(ctx->ev_chunk[slot], ctx->stream);
         if (e == cudaSuccess) ctx->ply_h2d += bytes;
     }
@@ -366,6 +445,10 @@ M2S_EXPORT m2s_status m2s_ply_read(m2s_ctx* ctx, const char* path, void* d_ref96
     if (e == cudaSuccess) e = es;
     if (e != cudaSuccess) { set_error(std::string("m2s_ply_read: ") + cudaGetErrorString(e)); return M2S_E_CUDA; }
     return st;
+}
+
+M2S_EXPORT m2s_status m2s_ply_read(m2s_ctx* ctx, const char* path, void* d_ref96, uint64_t capacity, m2s_ply_info* info) {
+    return m2s_ply_read_sh(ctx, path, d_ref96, nullptr, capacity, info);
 }
 
 M2S_EXPORT uint64_t m2s_ply_h2d_bytes(const m2s_ctx* ctx) { return ctx ? ctx->ply_h2d : 0; }

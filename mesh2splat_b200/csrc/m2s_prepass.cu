@@ -8,6 +8,8 @@
 // shared memory and written as one contiguous span with 16-byte stores.  Consumes the conversion's REF96 records
 // (u_format 0), its PACKED56 records (a standard 3DGS gaussian: u_format 1 without PBR values), or the REF96 records
 // m2s_ply_read loads from a .ply (u_format 1, u_plyHasPbr 0 or 1): the record layout and u_format are separate arguments.
+// Beyond the reference, prepass_sh_kernel gives those loaded records their view-dependent colour from the SH rest
+// coefficients m2s_ply_read_sh keeps (render modes 0 and 6).
 #include "m2s_prepass.cuh"
 
 namespace m2s {
@@ -48,9 +50,68 @@ __device__ __forceinline__ bool prepass_behind_mesh(const PrepassArgs& a, const 
     return my > __fadd_rn(depth, 0.00002f);
 }
 
-// kDepth: the prepass with the mesh depth test (map: dw x dh floats as m2s_mesh_depth writes them)
-template <bool kStage, bool kDepth>
-__device__ __forceinline__ void prepass_body(const PrepassArgs& a, const float* map, uint32_t dw, uint32_t dh) {
+// ---- view-dependent colour (m2s_prepass_sh, beyond the reference): graphdeco's computeColorFromSH with its constants and
+// the signs folded into the basis; every operation one round-to-nearest fp32 step without contraction, as
+// oracle/m2s_sh_oracle.c restates it ----
+// rest = sum over k = 1..K of B_k coeff_k, in k order per channel; c: the gaussian's block (coefficient-major r g b)
+template <int D>
+__device__ __forceinline__ void sh_rest(const float4* c, float x, float y, float z, float rest[3]) {
+    constexpr int K = (D + 1) * (D + 1) - 1;
+    const float C1 = 0.4886025119029199f;
+    float B[15];
+    B[0] = __fmul_rn(-C1, y); B[1] = __fmul_rn(C1, z); B[2] = __fmul_rn(-C1, x);
+    if (D >= 2) {
+        const float xx = __fmul_rn(x, x), yy = __fmul_rn(y, y), zz = __fmul_rn(z, z);
+        const float xy = __fmul_rn(x, y), yz = __fmul_rn(y, z), xz = __fmul_rn(x, z);
+        B[3] = __fmul_rn(1.0925484305920792f, xy);
+        B[4] = __fmul_rn(-1.0925484305920792f, yz);
+        B[5] = __fmul_rn(0.31539156525252005f, __fsub_rn(__fsub_rn(__fmul_rn(2.0f, zz), xx), yy));
+        B[6] = __fmul_rn(-1.0925484305920792f, xz);
+        B[7] = __fmul_rn(0.5462742152960396f, __fsub_rn(xx, yy));
+        if (D >= 3) {
+            B[8] = __fmul_rn(__fmul_rn(-0.5900435899266435f, y), __fsub_rn(__fmul_rn(3.0f, xx), yy));
+            B[9] = __fmul_rn(__fmul_rn(2.890611442640554f, xy), z);
+            B[10] = __fmul_rn(__fmul_rn(-0.4570457994644658f, y), __fsub_rn(__fsub_rn(__fmul_rn(4.0f, zz), xx), yy));
+            B[11] = __fmul_rn(__fmul_rn(0.3731763325901154f, z), __fsub_rn(__fsub_rn(__fmul_rn(2.0f, zz), __fmul_rn(3.0f, xx)), __fmul_rn(3.0f, yy)));
+            B[12] = __fmul_rn(__fmul_rn(-0.4570457994644658f, x), __fsub_rn(__fsub_rn(__fmul_rn(4.0f, zz), xx), yy));
+            B[13] = __fmul_rn(__fmul_rn(1.445305721320277f, z), __fsub_rn(xx, yy));
+            B[14] = __fmul_rn(__fmul_rn(-0.5900435899266435f, x), __fsub_rn(xx, __fmul_rn(3.0f, yy)));
+        }
+    }
+    rest[0] = rest[1] = rest[2] = 0.0f;
+#pragma unroll
+    for (int v = 0; v < (3 * K + 3) / 4; ++v) {   // every load of the block first: one round trip to memory
+        const float4 q = __ldg(c + v);
+        const float e[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+            if (4 * v + j < 3 * K) rest[(4 * v + j) % 3] = __fadd_rn(rest[(4 * v + j) % 3], __fmul_rn(B[(4 * v + j) / 3], e[j]));
+    }
+}
+
+// the colour of gaussian gid at model-space position p seen from s.cam: max(colour + rest, 0) per channel (glm::max: NaN kept)
+__device__ __forceinline__ void sh_colour(const PrepassShArgs& s, unsigned long long gid, float px, float py, float pz, float& r, float& g,
+                                          float& b) {
+    const float dx = __fsub_rn(px, s.cam[0]), dy = __fsub_rn(py, s.cam[1]), dz = __fsub_rn(pz, s.cam[2]);
+    const float len = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
+    float rest[3] = {0.0f, 0.0f, 0.0f};
+    if (len != 0.0f) {
+        const float inv = __fdiv_rn(1.0f, len);
+        const float x = __fmul_rn(dx, inv), y = __fmul_rn(dy, inv), z = __fmul_rn(dz, inv);
+        const float4* c = s.sh + gid * s.vec4;
+        if (s.degree == 1) sh_rest<1>(c, x, y, z, rest);
+        else if (s.degree == 2) sh_rest<2>(c, x, y, z, rest);
+        else sh_rest<3>(c, x, y, z, rest);
+    }
+    r = __fadd_rn(r, rest[0]); g = __fadd_rn(g, rest[1]); b = __fadd_rn(b, rest[2]);
+    r = r < 0.0f ? 0.0f : r; g = g < 0.0f ? 0.0f : g; b = b < 0.0f ? 0.0f : b;
+}
+
+// kDepth: the prepass with the mesh depth test (map: dw x dh floats as m2s_mesh_depth writes them); kSh: the colour of
+// render modes 0 and 6 from the SH rest coefficients (sh)
+template <bool kStage, bool kDepth, bool kSh = false>
+__device__ __forceinline__ void prepass_body(const PrepassArgs& a, const float* map, uint32_t dw, uint32_t dh,
+                                             const PrepassShArgs* sh = nullptr) {
     __shared__ float4 stage[kPrepassThreads / 32][32 * 6];   // 3 KB per warp: the warp's surviving quads
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     unsigned long long n = a.count;
@@ -147,7 +208,10 @@ __device__ __forceinline__ void prepass_body(const PrepassArgs& a, const float* 
             n0 = r0 * 0.5f + 0.5f; n1 = r1 * 0.5f + 0.5f; n2 = r2 * 0.5f + 0.5f; n3 = ca;
         }
         float o0 = 0.f, o1 = 0.f, o2 = 0.f, o3 = 0.f;                    // :132-148
-        if (a.render_mode == 0 || a.render_mode == 6) { o0 = cr; o1 = cg; o2 = cb; o3 = ca; }
+        if (a.render_mode == 0 || a.render_mode == 6) {
+            o0 = cr; o1 = cg; o2 = cb; o3 = ca;
+            if (kSh) sh_colour(*sh, gid, px, py, pz, o0, o1, o2);   // survivors of the frustum cull only
+        }
         else if (a.render_mode == 1) {
             const float d = clamp01(expf(-20.0f * clamp01((-vs2 - a.near_far[0]) / (a.near_far[1] - a.near_far[0]))));   // common.glsl:80-84
             o0 = o1 = o2 = d; o3 = ca;
@@ -215,6 +279,11 @@ __global__ void __launch_bounds__(kPrepassThreads) prepass_depth_kernel(const __
     prepass_body<kStage, true>(a.p, a.map, a.width, a.height);
 }
 
+template <bool kStage>
+__global__ void __launch_bounds__(kPrepassThreads) prepass_sh_kernel(const __grid_constant__ PrepassShArgs a) {
+    prepass_body<kStage, false, true>(a.p, nullptr, 0, 0, &a);
+}
+
 cudaError_t prepass_launch(const PrepassArgs& args, cudaStream_t stream) {
     if (args.count == 0) return cudaSuccess;
     const unsigned long long blocks = (args.count + kPrepassThreads - 1) / kPrepassThreads;
@@ -228,6 +297,14 @@ cudaError_t prepass_depth_launch(const PrepassDepthArgs& args, cudaStream_t stre
     const unsigned long long blocks = (args.p.count + kPrepassThreads - 1) / kPrepassThreads;
     if (args.p.count >= (2ull << 20)) prepass_depth_kernel<true><<<(unsigned)blocks, kPrepassThreads, 0, stream>>>(args);
     else prepass_depth_kernel<false><<<(unsigned)blocks, kPrepassThreads, 0, stream>>>(args);
+    return cudaGetLastError();
+}
+
+cudaError_t prepass_sh_launch(const PrepassShArgs& args, cudaStream_t stream) {
+    if (args.p.count == 0) return cudaSuccess;
+    const unsigned long long blocks = (args.p.count + kPrepassThreads - 1) / kPrepassThreads;
+    if (args.p.count >= (2ull << 20)) prepass_sh_kernel<true><<<(unsigned)blocks, kPrepassThreads, 0, stream>>>(args);
+    else prepass_sh_kernel<false><<<(unsigned)blocks, kPrepassThreads, 0, stream>>>(args);
     return cudaGetLastError();
 }
 

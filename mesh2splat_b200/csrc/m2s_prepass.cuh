@@ -30,7 +30,17 @@ struct PrepassDepthArgs {
     uint32_t width, height;
 };
 
+// the prepass with view-dependent colour (m2s_prepass_sh): sh holds vec4 float4 per gaussian (M2S_SH_FLOATS / 4), the
+// coefficients of degree 1..degree are evaluated; cam is the camera position in model space
+struct PrepassShArgs {
+    PrepassArgs p;
+    const float4* sh;
+    uint32_t vec4, degree;
+    float cam[3];
+};
+
 cudaError_t prepass_launch(const PrepassArgs& args, cudaStream_t stream);
+cudaError_t prepass_sh_launch(const PrepassShArgs& args, cudaStream_t stream);
 cudaError_t prepass_depth_launch(const PrepassDepthArgs& args, cudaStream_t stream);
 
 }  // namespace m2s

@@ -196,6 +196,62 @@ M2S_EXPORT m2s_status m2s_prepass_mesh_depth(m2s_ctx* ctx, const void* d_records
     });
 }
 
+// ---- the prepass with view-dependent colour (beyond the reference): m2s_prepass plus a loaded .ply's SH rest coefficients
+static m2s_status prepass_sh_check(const m2s_ctx* ctx, const void* d_records, uint64_t count, const m2s_prepass_params* p, const float* d_sh,
+                                   uint32_t buffer_degree, uint32_t sh_degree, const void* d_quads, const float* d_depths, bool has_valid) {
+    const char* fn = "m2s_prepass_sh";
+    m2s_status st = prepass_check(ctx, d_records, count, p, d_quads, d_depths, has_valid);
+    if (st != M2S_OK) return st;
+    if (p->layout != M2S_VIEW_PLY && p->layout != M2S_VIEW_PLY_PBR) return invalid(fn, "layouts VIEW_PLY and VIEW_PLY_PBR only");
+    if (buffer_degree > 3 || sh_degree > buffer_degree) return invalid(fn, "buffer_degree must be 0..3, sh_degree 0..buffer_degree");
+    if (sh_degree && !d_sh) return invalid(fn, "NULL d_sh");
+    return aligned_ok(fn, "the SH buffer must be 16-byte aligned", {{d_sh, 16}}) ? M2S_OK : M2S_E_INVALID;
+}
+
+// the camera position in model space: the translation column of inverse(V M), in fp64 from the fp32 matrices, rounded once
+// to fp32; false for a singular V M
+static bool sh_camera(const m2s_prepass_params* p, float cam[3]) {
+    const float *V = p->world_to_view, *M = p->model_to_world;
+    double VM[16], inv[16];
+    for (int c = 0; c < 4; ++c)
+        for (int r = 0; r < 4; ++r)
+            VM[c * 4 + r] = (((double)V[r] * M[c * 4] + (double)V[4 + r] * M[c * 4 + 1]) + (double)V[8 + r] * M[c * 4 + 2]) +
+                            (double)V[12 + r] * M[c * 4 + 3];
+    if (!invert4(VM, inv) || !std::isfinite(inv[12]) || !std::isfinite(inv[13]) || !std::isfinite(inv[14])) return false;
+    for (int k = 0; k < 3; ++k) cam[k] = (float)inv[12 + k];
+    return true;
+}
+
+M2S_EXPORT m2s_status m2s_prepass_sh_enqueue(m2s_ctx* ctx, const void* d_records, uint64_t count, const uint64_t* d_count,
+                                             const m2s_prepass_params* p, const float* d_sh, uint32_t buffer_degree, uint32_t sh_degree,
+                                             void* d_quads, float* d_depths, uint32_t* d_valid, void* stream_) {
+    m2s_status st = prepass_sh_check(ctx, d_records, count, p, d_sh, buffer_degree, sh_degree, d_quads, d_depths, d_valid != nullptr);
+    if (st != M2S_OK) return st;
+    PrepassShArgs a;
+    std::memset(&a, 0, sizeof(a));
+    st = prepass_fill(d_records, count, d_count, p, d_quads, d_depths, d_valid, a.p);
+    if (st != M2S_OK) return st;
+    if (!sh_camera(p, a.cam)) return invalid("m2s_prepass_sh", "world_to_view * model_to_world is singular");
+    a.sh = reinterpret_cast<const float4*>(d_sh);
+    a.vec4 = M2S_SH_FLOATS(buffer_degree) / 4;
+    a.degree = sh_degree;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    cudaStream_t stream = pick_stream(ctx, stream_);
+    CUDA_TRY(cudaMemsetAsync(d_valid, 0, sizeof(uint32_t), stream));
+    CUDA_TRY(sh_degree ? prepass_sh_launch(a, stream) : prepass_launch(a.p, stream));   // degree 0: m2s_prepass's kernel
+    return M2S_OK;
+}
+
+M2S_EXPORT m2s_status m2s_prepass_sh(m2s_ctx* ctx, const void* d_records, uint64_t count, const m2s_prepass_params* p, const float* d_sh,
+                                     uint32_t buffer_degree, uint32_t sh_degree, void* d_quads, float* d_depths, uint32_t* valid) {
+    m2s_status st = prepass_sh_check(ctx, d_records, count, p, d_sh, buffer_degree, sh_degree, d_quads, d_depths, true);
+    if (st != M2S_OK) return st;
+    return prepass_sync(ctx, valid, [&](uint32_t* d_valid) {
+        return m2s_prepass_sh_enqueue(ctx, d_records, count, nullptr, p, d_sh, buffer_degree, sh_degree, d_quads, d_depths, d_valid,
+                                      ctx->stream);
+    });
+}
+
 // ---- the viewer's depth sort (SURVEY 8 f-5): RadixSortPass::execute = radixSortPrepass.glsl + glu::RadixSort + radixSortGather.glsl
 M2S_EXPORT m2s_status m2s_depth_sort_enqueue(m2s_ctx* ctx, const void* d_quads, const float* d_depths, uint64_t count,
                                              const uint32_t* d_count, void* d_sorted_quads, uint32_t* d_order, uint32_t* d_draw,
