@@ -43,6 +43,9 @@
  *      src/parsers/parsers.cpp:516-629)                          as the viewer passes' input
  *   beyond the reference: a loaded .ply's view-dependent colour  m2s_ply_read_sh, m2s_ply_decode_sh_enqueue,
  *     (the SH rest coefficients, graphdeco's computeColorFromSH) m2s_prepass_sh, m2s_prepass_sh_enqueue
+ *   beyond the reference: how closely the splats reproduce       m2s_image_compare, m2s_image_compare_enqueue
+ *     their mesh (SSIM, PSNR, coverage of the split screen's
+ *     two images, GaussianRelightingPass.cpp:90-135)
  *
  * Plain pointers and sizes only; no C++/torch types.  All functions return an
  * m2s_status; m2s_last_error() gives the thread-local message of the last
@@ -614,6 +617,42 @@ m2s_status m2s_deferred_light_split_enqueue(m2s_ctx* ctx, const m2s_gbuffer* spl
                                             void* stream);
 m2s_status m2s_deferred_light_split(m2s_ctx* ctx, const m2s_gbuffer* splat, const m2s_gbuffer* mesh, const float* d_cube,
                                     const m2s_light_params* params, float split_position, uint8_t* d_image);
+
+/* ---- how closely the splats reproduce their mesh (beyond the reference) -----------------------------------------------
+ * The split screen (GaussianRelightingPass.cpp:90-135) shows the lit mesh beside the lit splats and leaves the judgement
+ * to the eye; this call puts numbers on it.  It compares two RGBA8 images A and B of width x height pixels (row 0 at
+ * the bottom, as every pass writes them) on R, G and B; alpha is ignored.
+ *   SSIM  Wang et al. 2004 with an 11 x 11 Gaussian window (sigma 1.5), L = 255, over the valid windows only: centres
+ *         x in [5, width - 6], y in [5, height - 6], (width - 10) (height - 10) windows.  The value of a window is the
+ *         mean of its three channel values.  The fp32 operation order is DESIGN §2: identical images give exactly 1 in
+ *         every window.
+ *   SE    the squared error of every pixel and channel, summed exactly.
+ *   cover optional RGBA8 images of the same size (typically the albedo targets of the mesh and the splat G-buffer): a
+ *         pixel is covered in A (B) when the alpha of cover_a (cover_b) is >= cover_min; a NULL cover covers nothing.
+ *         The covered totals take the pixels covered in A or B, and the windows whose centre is.
+ * PSNR = 10 log10(255^2 3 N / sum_c sq_err[c]) with N the pixel count (+inf when the sum is 0); SSIM = sum_c ssim[c] /
+ * (3 windows); the covered forms with the covered counts. */
+typedef struct m2s_compare_params {
+    uint32_t width, height;    /* 11..4096 each */
+    uint32_t cover_min;        /* 1..255 */
+} m2s_compare_params;
+typedef struct m2s_compare_result {
+    uint64_t windows, covered_windows, pixels_both, pixels_a_only, pixels_b_only;
+    uint64_t sq_err[3], sq_err_covered[3];     /* per channel R, G, B, over all pixels / the pixels covered in A or B */
+    double ssim[3], ssim_covered[3];           /* sums over windows; mean = sum / count */
+} m2s_compare_result;
+/* Enqueue-only.  d_a, d_b, d_cover_a, d_cover_b (each cover optional): width x height x 4 bytes, 4-byte aligned.
+ * d_result: device, 8-byte aligned, written whole.  d_ssim_map (optional): (width - 10) x (height - 10) floats, 4-byte
+ * aligned, row 0 = window y 5.  Two calls on the same inputs give identical bits.  A size or cover_min out of range, a
+ * NULL image or result, or a misaligned pointer is M2S_E_INVALID with nothing written.  Scratch is stream-ordered
+ * context memory grown on `stream` (NULL = context stream); nothing is synchronised. */
+m2s_status m2s_image_compare_enqueue(m2s_ctx* ctx, const uint8_t* d_a, const uint8_t* d_b, const uint8_t* d_cover_a,
+                                     const uint8_t* d_cover_b, const m2s_compare_params* params, m2s_compare_result* d_result,
+                                     float* d_ssim_map, void* stream);
+/* Synchronous form on the context stream: *h_result on the host; the same bits as the enqueue form. */
+m2s_status m2s_image_compare(m2s_ctx* ctx, const uint8_t* d_a, const uint8_t* d_b, const uint8_t* d_cover_a,
+                             const uint8_t* d_cover_b, const m2s_compare_params* params, m2s_compare_result* h_result,
+                             float* d_ssim_map);
 
 #ifdef __cplusplus
 }

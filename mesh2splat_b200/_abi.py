@@ -5,6 +5,7 @@ No compute here: this is the marshalling layer between numpy arrays and the C AB
 from __future__ import annotations
 
 import ctypes as C
+import math
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -182,6 +183,40 @@ def make_mesh_render_params(world_to_view, view_to_clip, model_to_world, width: 
     p.near_far = (C.c_float * 2)(float(near_far[0]), float(near_far[1]))
     p.width, p.height, p.render_mode = int(width), int(height), int(render_mode)
     return p
+
+
+class m2s_compare_params(C.Structure):
+    _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("cover_min", C.c_uint32)]
+
+
+class m2s_compare_result(C.Structure):
+    """include/m2s.h: the totals of m2s_image_compare."""
+    _fields_ = [("windows", C.c_uint64), ("covered_windows", C.c_uint64), ("pixels_both", C.c_uint64), ("pixels_a_only", C.c_uint64),
+                ("pixels_b_only", C.c_uint64), ("sq_err", C.c_uint64 * 3), ("sq_err_covered", C.c_uint64 * 3), ("ssim", C.c_double * 3),
+                ("ssim_covered", C.c_double * 3)]
+
+
+def psnr(sq_err_sum: int, samples: int) -> float:
+    """10 log10(255^2 samples / sq_err_sum), samples = 3 N channel values; +inf for no error, nan for no samples."""
+    if samples == 0:
+        return float("nan")
+    return float("inf") if sq_err_sum == 0 else 10.0 * math.log10(255.0 * 255.0 * samples / sq_err_sum)
+
+
+def compare_result_dict(r: m2s_compare_result, pixels: int) -> dict:
+    """The totals of an m2s_compare_result as a dict, plus psnr, ssim (sum over channels / 3 windows) and the covered
+    forms (nan with nothing covered)."""
+    d = {n: int(getattr(r, n)) for n in ("windows", "covered_windows", "pixels_both", "pixels_a_only", "pixels_b_only")}
+    for n in ("sq_err", "sq_err_covered"):
+        d[n] = [int(v) for v in getattr(r, n)]
+    for n in ("ssim_sum", "ssim_covered_sum"):
+        d[n] = [float(v) for v in getattr(r, n.replace("_sum", ""))]
+    covered = d["pixels_both"] + d["pixels_a_only"] + d["pixels_b_only"]
+    d["psnr"] = psnr(sum(d["sq_err"]), 3 * pixels)
+    d["psnr_covered"] = psnr(sum(d["sq_err_covered"]), 3 * covered)
+    d["ssim"] = math.fsum(d["ssim_sum"]) / (3 * d["windows"])
+    d["ssim_covered"] = math.fsum(d["ssim_covered_sum"]) / (3 * d["covered_windows"]) if d["covered_windows"] else float("nan")
+    return d
 
 
 class m2s_peers(C.Structure):

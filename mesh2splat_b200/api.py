@@ -434,6 +434,32 @@ class Context:
         torch.cuda.synchronize(dev)
         return image.view(torch.uint8)[: width * height * 4].cpu().numpy().reshape(height, width, 4).copy()
 
+    def compare_images(self, a, b, width: int, height: int, cover_a=None, cover_b=None, cover_min: int = 128, ssim_map=None,
+                       enqueue: bool = False) -> dict:
+        """How closely image b reproduces image a (m2s_image_compare): SSIM over the valid 11 x 11 windows, squared error
+        and coverage of two RGBA8 device tensors of width * height * 4 bytes (e.g. the lit mesh and the lit splats of one
+        frame).  cover_a / cover_b: optional RGBA8 device tensors whose alpha >= cover_min marks a pixel covered (e.g. the
+        albedo targets of the two G-buffers).  ssim_map: optional float32 device tensor of at least (width - 10) *
+        (height - 10) values, filled with the per-window SSIM (row 0 = window y 5).  enqueue: m2s_image_compare_enqueue on
+        torch's current stream instead of the synchronous call.  Returns the totals (windows, covered_windows,
+        pixels_both, pixels_a_only, pixels_b_only, sq_err, sq_err_covered, ssim_sum, ssim_covered_sum) and the derived
+        psnr, ssim, psnr_covered and ssim_covered."""
+        torch = _torch()
+        dev = a.device
+        p = _abi.m2s_compare_params(width, height, cover_min)
+        ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+        args = (self.handle, ptr(a), ptr(b), ptr(cover_a), ptr(cover_b), C.byref(p))
+        if enqueue:
+            d_result = torch.zeros(C.sizeof(_abi.m2s_compare_result), dtype=torch.uint8, device=dev)
+            check(lib().m2s_image_compare_enqueue(*args, d_result.data_ptr(), ptr(ssim_map), torch.cuda.current_stream(dev).cuda_stream))
+            torch.cuda.synchronize(dev)
+            r = _abi.m2s_compare_result.from_buffer_copy(d_result.cpu().numpy().tobytes())
+        else:
+            r = _abi.m2s_compare_result()
+            torch.cuda.synchronize(dev)   # the images torch filled are ready before the context stream reads them
+            check(lib().m2s_image_compare(*args, C.byref(r), ptr(ssim_map)))
+        return _abi.compare_result_dict(r, width * height)
+
     def convert_timed(self, dscene: DeviceScene, params: _abi.m2s_params, out, capacity: int):
         """One conversion with an event between the two kernels (they do not overlap): (raster_ms, fragment_ms)."""
         a, b = C.c_float(0), C.c_float(0)
