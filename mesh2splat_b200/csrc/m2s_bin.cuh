@@ -62,12 +62,7 @@ __global__ void __launch_bounds__(kBinBlock) bin_count_kernel(B b) {
     if ((uint64_t)blockIdx.x * kBinBlock >= n) return;   // blocks at or past n are never read
     const uint32_t cnt = i < n ? b.visit((uint32_t)i, [](uint32_t, uint32_t) {}) : 0u;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t x = cnt;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
-        if (lane >= o) x += y;
-    }
+    const uint32_t x = warp_inclusive_scan(cnt, lane);
     if (lane == 31) s_warp[warp] = x;
     __syncthreads();
     uint32_t before = 0, total = 0;
@@ -93,12 +88,7 @@ __global__ void __launch_bounds__(kBinScanThreads) bin_scan_kernel(B b) {
     for (uint32_t base = 0; base < nb; base += kBinScanThreads) {
         const uint32_t k = base + threadIdx.x;
         const unsigned long long v = k < nb ? blocks[k] : 0ull;
-        unsigned long long x = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
-            if (lane >= o) x += y;
-        }
+        const unsigned long long x = warp_inclusive_scan(v, lane);
         if (lane == 31) s_warp[warp] = x;
         __syncthreads();
         unsigned long long before = s_carry, chunk = 0;

@@ -45,6 +45,9 @@ struct FragSmem {
     static constexpr size_t kBytes = kStageAligned + (size_t)kFragWarps * kWarpStage;
 };
 
+// FragItem::first from the low and high words of the item's first 16 bytes, loaded as one uint4 h0: item_first(h0.x, h0.y)
+__device__ __forceinline__ unsigned long long item_first(uint32_t lo, uint32_t hi) { return (unsigned long long)lo | ((unsigned long long)hi << 32); }
+
 // A micro item (kItMicro): <= 32 fragments listed in the item itself, shaded by one warp with direct loads.  Out of line:
 // the second copy of the shading code must not add to the register pressure of the main loop.
 template <int LAYOUT>
@@ -52,7 +55,7 @@ __device__ __noinline__ void micro_item(const ConvertArgs& a, uint32_t it, uint4
                                         unsigned long long goff, const uint32_t* __restrict__ texb, unsigned char* stage, int lane) {
     using Rec = typename FragSmem<LAYOUT>::Rec;
     constexpr int kStride = Cfg<LAYOUT>::kStride;
-    const unsigned long long first = (unsigned long long)h0.x | ((unsigned long long)h0.y << 32);
+    const unsigned long long first = item_first(h0.x, h0.y);
     const uint32_t t0 = h0.z * a.unit_tris;
     const uint32_t w32 = __ldg(reinterpret_cast<const uint32_t*>((a.items + it)->blocks) + min((uint32_t)lane, nfr - 1u));  // idle lanes shadow the last fragment
     const uint32_t slot = w32 & 31u;
@@ -118,7 +121,7 @@ __global__ void __launch_bounds__(kFragThreads, (LAYOUT == 1 ? M2S_FRAG_THREADS_
         return h;
     };
     auto live = [&](const Hdr& h) {  // uniform over the CTA: does the item emit anything?
-        const unsigned long long first = (unsigned long long)h.h0.x | ((unsigned long long)h.h0.y << 32);
+        const unsigned long long first = item_first(h.h0.x, h.h0.y);
         return h.h1.y > h.h1.x && first + h.h1.x < room;
     };
     auto issue = [&](const Hdr& h, uint32_t buf) {  // thread 0: stage the unit's records: one TMA bulk copy
@@ -150,7 +153,7 @@ __global__ void __launch_bounds__(kFragThreads, (LAYOUT == 1 ? M2S_FRAG_THREADS_
             continue;
         }
         // ---- the item: a unit's small triangles (implicit: one block per triangle) or queued row blocks ----
-        const unsigned long long first = (unsigned long long)cur.h0.x | ((unsigned long long)cur.h0.y << 32);
+        const unsigned long long first = item_first(cur.h0.x, cur.h0.y);
         const uint32_t unit = cur.h0.z, fb = cur.h1.x, fe = cur.h1.y;
         const bool unit_item = (cur.h0.w & 0x80000000u) != 0;
         const uint32_t nblocks = cur.h0.w & 0xffu;
@@ -197,12 +200,7 @@ __global__ void __launch_bounds__(kFragThreads, (LAYOUT == 1 ? M2S_FRAG_THREADS_
                     int h;
                     n = span_row(row_state(recs[slot], h), (int)(row_begin + lane), xl);
                 }
-                uint32_t incl = n;
-#pragma unroll
-                for (int d = 1; d < 32; d <<= 1) {
-                    const uint32_t t = __shfl_up_sync(0xffffffffu, incl, d);
-                    if (lane >= d) incl += t;
-                }
+                const uint32_t incl = warp_inclusive_scan(n, lane);
                 // rows past the block's last one repeat the block end: the table stays sorted, they are never selected
                 span[b * 32 + lane] = make_uint2(bp + incl - n, (uint32_t)xl | ((row_begin + lane) << 12) | (slot << 24));
             }

@@ -1,10 +1,22 @@
 // m2s_ptx.cuh — the PTX the conversion kernels use directly: mbarrier + 1-D bulk async copy (TMA engine; SASS UBLKCP),
-// system-scope release / acquire, and the bounded wait of the fused gather.
+// system-scope release / acquire, and the bounded wait of the fused gather; and the warp scan of the kernels' and the
+// viewer's prefix sums.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
 
 namespace m2s {
+
+// inclusive prefix sum of v over the lanes of each `width`-lane segment of the warp (width: a power of two <= 32)
+template <typename T>
+__device__ __forceinline__ T warp_inclusive_scan(T v, int lane, int width = 32) {
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const T y = __shfl_up_sync(0xffffffffu, v, d, width);
+        if ((lane & (width - 1)) >= d) v += y;
+    }
+    return v;
+}
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));

@@ -99,13 +99,31 @@ struct Tables {
     uint32_t nranges;
 };
 constexpr uint32_t kTableSmemBytes = 16 * 1024;
+// the CTA's threads copy the tables to `base` when they fit (kTableSmemBytes; the CTA barrier that follows publishes them)
+__device__ __forceinline__ Tables copy_tables(const ConvertArgs& a, unsigned char* base) {
+    Tables tabs{a.ranges, a.prims, a.texs, a.nranges};
+    const uint32_t br = a.nranges * (uint32_t)sizeof(DRange), bp = a.nprims * (uint32_t)sizeof(DPrim), bt = a.ntex * (uint32_t)sizeof(DTexture);
+    if (br + bp + bt <= kTableSmemBytes) {  // uniform across the grid
+        uint32_t* dst = reinterpret_cast<uint32_t*>(base);  // word-wise: the structs are 16, 56 and 48 bytes
+        const uint32_t* s0 = reinterpret_cast<const uint32_t*>(a.ranges);
+        const uint32_t* s1 = reinterpret_cast<const uint32_t*>(a.prims);
+        const uint32_t* s2 = reinterpret_cast<const uint32_t*>(a.texs);
+        const uint32_t n0 = br / 4, n1 = bp / 4, n2 = bt / 4;
+        for (uint32_t i = threadIdx.x; i < n0 + n1 + n2; i += blockDim.x)
+            dst[i] = i < n0 ? s0[i] : (i < n0 + n1 ? s1[i - n0] : s2[i - n0 - n1]);
+        tabs.ranges = reinterpret_cast<const DRange*>(base);
+        tabs.prims = reinterpret_cast<const DPrim*>(base + br);
+        tabs.texs = reinterpret_cast<const DTexture*>(base + br + bp);
+    }
+    return tabs;
+}
 
 // what the raster kernel itself keeps of a triangle after the set-up (registers of the owning lane)
 struct TriSetup {
-    long long E0[3];
-    int A[3], B[3];
-    int w, h;
-    unsigned incl;
+    long long E0[3] = {0, 0, 0};
+    int A[3] = {0, 0, 0}, B[3] = {0, 0, 0};
+    int w = 1, h = 0;
+    unsigned incl = 0;
 };
 
 // ------------------------------------------------------------------------------------------
@@ -317,13 +335,13 @@ __device__ __forceinline__ uint32_t block_ref(uint32_t slot, uint32_t row_begin,
 // A warp collects the work items of its current unit in shared memory (WarpBlock::pend / it*) and publishes them
 // with ONE 64-bit atomicAdd that reserves both the output range (low 40 bits: fragments) and the queue slots
 // (high 24 bits) — the reference does one atomicCounterIncrement per fragment (converterFS.glsl:46).
-struct Stash {            // warp-uniform registers
-    uint32_t n_it;        // closed items
-    uint32_t cur_nb;      // blocks of the open item
-    uint32_t cur_total;   // fragments of the open item
-    uint32_t frags;       // fragments of the closed items
-    uint32_t slots;       // queue slots of the closed items
-    unsigned long long seen;  // a lower bound of the global fragment counter (from this warp's last reservation)
+struct Stash {                // warp-uniform registers
+    uint32_t n_it = 0;        // closed items
+    uint32_t cur_nb = 0;      // blocks of the open item
+    uint32_t cur_total = 0;   // fragments of the open item
+    uint32_t frags = 0;       // fragments of the closed items
+    uint32_t slots = 0;       // queue slots of the closed items
+    unsigned long long seen = 0;  // a lower bound of the global fragment counter (from this warp's last reservation)
 };
 
 template <int RK>
@@ -494,6 +512,52 @@ struct CtaQueue {
     CtaEntry q[kCtaQueueCap];
 };
 
+// A post of n entries: cta_reserve reserves [base, base + n), the first `fit` of them in the queue (the poster keeps the
+// rest); cta_publish fills entry base + i, i < fit, through fill(entry, i) and marks it ready.  Two steps: a direct pass
+// sets WarpBlock::left in between.
+struct CtaPost {
+    uint32_t base, fit;
+};
+__device__ __forceinline__ CtaPost cta_reserve(CtaQueue& cq, uint32_t n, int lane) {
+    uint32_t base = 0;
+    if (lane == 0) base = atomicAdd_block(&cq.tail, n);
+    base = __shfl_sync(0xffffffffu, base, 0);
+    return {base, base < kCtaQueueCap ? min(n, kCtaQueueCap - base) : 0u};
+}
+template <class Fill>
+__device__ __forceinline__ void cta_publish(CtaQueue& cq, uint32_t base, uint32_t fit, int lane, Fill&& fill) {
+    if ((uint32_t)lane < fit) {
+        CtaEntry& e = cq.q[base + lane];
+        fill(e, (uint32_t)lane);
+        __threadfence_block();
+        e.ready = 1u;
+    }
+}
+
+// takes the shading piece of entry t unless another warp has: `won` becomes 1 on every lane if this warp took it, else 0
+__device__ __forceinline__ void cta_take(CtaQueue& cq, uint32_t t, uint32_t& won, int lane) {
+    if (lane == 0) won = atomicExch(&cq.q[t].taken, 1u) == 0u;
+    won = __shfl_sync(0xffffffffu, won, 0);
+}
+
+// a warp that is out of units waits for the entry of its ticket t: true once the entry is posted and ready, false once no
+// warp of the CTA can post it any more
+__device__ __forceinline__ bool cta_ticket_wait(CtaQueue& cq, uint32_t t, int lane) {
+    bool have = false;
+    if (lane == 0) {
+        unsigned ns = 64;   // the waiters must not take issue slots from the warps still working
+        for (;;) {
+            if (*reinterpret_cast<volatile uint32_t*>(&cq.tail) > t) { have = true; break; }
+            if (*reinterpret_cast<volatile uint32_t*>(&cq.active) == 0 && *reinterpret_cast<volatile uint32_t*>(&cq.tail) <= t) break;
+            __nanosleep(ns);
+            ns = min(ns * 2u, 256u);
+        }
+        if (have) while (cq.q[t].ready == 0u) __nanosleep(20);
+        __threadfence_block();
+    }
+    return __shfl_sync(0xffffffffu, (int)have, 0);
+}
+
 // ------------------------------------------------------------------------------------------
 // DIRECT path: the fragments of a light unit's small triangles, listed in the unit's shared-memory slice, are shaded
 // by the warp that rasterised them, in groups of 32.  Used when the warps have several units each (n_units > resident
@@ -543,6 +607,134 @@ __device__ __noinline__ uint32_t direct_run(const WarpBlock<1>& src, uint32_t f0
     return par;
 }
 
+// The sharing of a direct pass of `owner`, this warp: the pass's list [0, dsum) is cut into groups of 32 from 0, across
+// the boundary of its two units: only the last group can be partial.  This warp shades the first kShareFirst fragments at
+// once; the rest goes to the CTA's help queue in pieces of kSharePiece, which this warp then shades in order unless
+// another warp has taken them: a warp that is out of units takes the pieces this warp has not reached (the late claim
+// cannot balance a pass's weight).  Returns the pieces posted and how many of them this warp shaded itself.
+struct DirectShare {
+    uint32_t fit, done;
+};
+template <class Shade>
+__device__ __forceinline__ DirectShare direct_share(CtaQueue& cq, WarpBlock<1>& wb, uint32_t owner, uint32_t dsum, unsigned long long dfirst,
+                                                    uint32_t tri0, Shade&& shade, int lane) {
+    const uint32_t npiece = dsum > kShareFirst ? (dsum - kShareFirst + kSharePiece - 1) / kSharePiece : 0u;
+    CtaPost q{0, 0};
+    if (npiece) {
+        q = cta_reserve(cq, npiece, lane);
+        if (lane == 0) wb.left = q.fit;
+        __threadfence_block();   // the count, the records and the list, before the pieces are posted
+        __syncwarp();
+        cta_publish(cq, q.base, q.fit, lane, [&](CtaEntry& e, uint32_t i) {
+            e.h = -1;
+            e.sp.first = dfirst; e.sp.owner = owner; e.sp.tri0 = tri0;
+            e.sp.f0 = kShareFirst + i * kSharePiece; e.sp.f1 = min(dsum, e.sp.f0 + kSharePiece);
+        });
+    }
+    shade(wb, 0, min(dsum, kShareFirst), dfirst, tri0);
+    uint32_t done = 0;
+    for (uint32_t p = 0; p < npiece; ++p) {
+        uint32_t won = 1;
+        if (p < q.fit) {
+            cta_take(cq, q.base + p, won, lane);
+            done += won;
+        }
+        const uint32_t f0 = kShareFirst + p * kSharePiece;
+        if (won) shade(wb, f0, min(dsum, f0 + kSharePiece), dfirst, tri0);
+    }
+    return {q.fit, done};
+}
+
+// other warps may still read the records and the list of this warp's slice: wait until they have shaded the pieces
+// they took, before the slice is rewritten
+__device__ __forceinline__ void direct_share_wait(WarpBlock<1>& wb, DirectShare sh, int lane) {
+    if (sh.fit) {
+        if (lane == 0) {
+            if (sh.done) atomicSub_block(&wb.left, sh.done);
+            while (*reinterpret_cast<volatile uint32_t*>(&wb.left) != 0u) __nanosleep(32);
+            __threadfence_block();
+        }
+        __syncwarp();
+    }
+}
+
+// help: tickets on the CTA's queue until no warp of the CTA can post any more.  A tall triangle's row blocks are counted
+// into this warp's stash; a shading piece is shaded from its owner's slice of `smem`, unless its owner got there first
+template <int RK, class Shade>
+__device__ __forceinline__ void help_cta(const ConvertArgs& a, unsigned char* smem, WarpBlock<RK>& wb, Stash& st, CtaQueue& cq,
+                                         Shade&& shade, int lane) {
+    if (lane == 0) atomicSub_block(&cq.active, 1u);
+    for (;;) {
+        uint32_t t = 0;
+        if (lane == 0) t = atomicAdd_block(&cq.head, 1u);
+        t = __shfl_sync(0xffffffffu, t, 0);
+        if (t >= kCtaQueueCap) break;  // beyond the capacity nothing is ever posted
+        if (!cta_ticket_wait(cq, t, lane)) break;
+        const CtaEntry& e = cq.q[t];
+        if (e.h < 0) {
+            if constexpr (RK == 1) {
+                uint32_t won = 0;
+                cta_take(cq, t, won, lane);
+                if (won) {
+                    WarpBlock<RK>& src = *reinterpret_cast<WarpBlock<RK>*>(smem + (size_t)e.sp.owner * sizeof(WarpBlock<RK>));
+                    cp_async_wait_all();   // this warp's wb.logtab, if it never shaded a unit of its own
+                    __syncwarp();
+                    shade(src, e.sp.f0, e.sp.f1, e.sp.first, e.sp.tri0);
+                    __syncwarp();
+                    if (lane == 0) { __threadfence_block(); atomicSub_block(&src.left, 1u); }   // its slice may be rewritten
+                }
+            }
+            continue;
+        }
+        const RowState rs = e.rs;
+        const int h = e.h;
+        const uint32_t eu = e.unit, es = e.slot;
+        const int rb0 = (int)e.rb0, rb1 = (int)e.rb1;
+        count_blocks<RK>(a, wb, eu, st, rs, h, es, rb0, rb1, lane);
+        stash_close_item<RK>(a, wb, eu, st, lane);
+        stash_flush<RK>(a, wb, eu, st, lane);
+    }
+}
+
+// the last CTA out publishes the counts and re-arms the scheduler for the next launch
+__device__ __forceinline__ void raster_last_cta(const ConvertArgs& a, int warp, int lane) {
+    __syncthreads();
+    if (warp == 0) {
+        uint32_t last = 0;
+        unsigned long long tot = 0;
+        if (lane == 0) {
+            __threadfence();
+            const uint32_t done = atomicAdd(SCHED(a, 4), 1u);
+            if (done == gridDim.x - 1) {
+                __threadfence();
+                last = 1;
+                const unsigned long long packed = *reinterpret_cast<volatile unsigned long long*>(a.counter);
+                tot = packed & kFragMask;                       // fragments generated
+                *a.total_out = tot;
+                *a.n_items_out = (uint32_t)(packed >> 40);      // work items queued
+                *a.counter = 0ull;
+                if (a.host_total) {  // zero-copy count for the host (PCIe posted write, ~1 us)
+                    *reinterpret_cast<volatile unsigned long long*>(a.host_total) = tot;
+                    __threadfence_system();
+                    *reinterpret_cast<volatile unsigned long long*>(a.host_total + 1) = a.host_tag;
+                }
+                *SCHED(a, 0) = 0; *SCHED(a, 4) = 0;
+                __threadfence();
+            }
+        }
+        if (a.world > 1) {  // fused gather: tell every peer how many records this rank will write, one lane per peer
+            last = __shfl_sync(0xffffffffu, last, 0);
+            tot = __shfl_sync(0xffffffffu, tot, 0);
+            if (last && (uint32_t)lane < a.world) {
+                const unsigned long long mine = tot < a.cap ? tot : a.cap;
+                a.peer_xch[lane][a.rank * 4 + 0] = mine;
+                __threadfence_system();
+                st_release_sys(a.peer_xch[lane] + a.rank * 4 + 1, a.epoch);
+            }
+        }
+    }
+}
+
 // ------------------------------------------------------------------------------------------
 // raster_kernel
 // ------------------------------------------------------------------------------------------
@@ -581,30 +773,14 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         mbar_arrive_expect_tx(&wb.bar, bytes);
         tma_load_1d(wb.tri, tri_bytes + ((size_t)a.tri_first + t0) * kTriBytes, bytes, &wb.bar);
     };
+    auto claim = [&]() { return claim_base + atomicAdd(SCHED(a, 0), 1u); };   // lane 0 only: the next unit
     if (lane == 0 && unit < a.n_units) issue_load(unit, pair ? 2 * a.unit_tris : a.unit_tris);
     // ref_logf's table for the direct path's opacities -> the warp's slice, as an asynchronous copy that lands while the
     // first unit is set up (waited for before the first shading; a CTA-wide copy would wait at the barrier below: ~1 us
     // more per warp, measured on the H100)
     if constexpr (kDirectOK) cp_async_8(wb.logtab + lane, kLogfTab + lane);
 
-    // descriptor tables -> shared memory (once per CTA) when they fit
-    Tables tabs{a.ranges, a.prims, a.texs, a.nranges};
-    {
-        const uint32_t br = a.nranges * (uint32_t)sizeof(DRange), bp = a.nprims * (uint32_t)sizeof(DPrim), bt = a.ntex * (uint32_t)sizeof(DTexture);
-        if (br + bp + bt <= kTableSmemBytes) {  // uniform across the grid
-            unsigned char* base = smem + (size_t)C::kWarps * sizeof(WarpBlock<RK>);
-            uint32_t* dst = reinterpret_cast<uint32_t*>(base);  // word-wise: the structs are 16, 56 and 48 bytes
-            const uint32_t* s0 = reinterpret_cast<const uint32_t*>(a.ranges);
-            const uint32_t* s1 = reinterpret_cast<const uint32_t*>(a.prims);
-            const uint32_t* s2 = reinterpret_cast<const uint32_t*>(a.texs);
-            const uint32_t n0 = br / 4, n1 = bp / 4, n2 = bt / 4;
-            for (uint32_t i = threadIdx.x; i < n0 + n1 + n2; i += blockDim.x)
-                dst[i] = i < n0 ? s0[i] : (i < n0 + n1 ? s1[i - n0] : s2[i - n0 - n1]);
-            tabs.ranges = reinterpret_cast<const DRange*>(base);
-            tabs.prims = reinterpret_cast<const DPrim*>(base + br);
-            tabs.texs = reinterpret_cast<const DTexture*>(base + br + bp);
-        }
-    }
+    const Tables tabs = copy_tables(a, smem + (size_t)C::kWarps * sizeof(WarpBlock<RK>));
     CtaQueue& cq = *reinterpret_cast<CtaQueue*>(smem + (size_t)C::kWarps * sizeof(WarpBlock<RK>) + kTableSmemBytes);
     if (threadIdx.x == 0) { cq.tail = 0; cq.head = 0; cq.active = blockDim.x >> 5; }
     if (threadIdx.x < kCtaQueueCap) { cq.q[threadIdx.x].ready = 0u; cq.q[threadIdx.x].taken = 0u; }
@@ -613,7 +789,6 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
     uint32_t phase = 0;
     uint32_t spar = 0;   // the half of this warp's output stage that its next group of direct records goes to
     Stash st;
-    st.n_it = 0; st.cur_nb = 0; st.cur_total = 0; st.frags = 0; st.slots = 0; st.seen = 0;
     // the listed fragments [f0, f1) of the unit(s) in slice `src`, shaded by this warp through its own stage (direct_run)
     auto shade = [&](const WarpBlock<RK>& src, uint32_t f0, uint32_t f1, unsigned long long first, uint32_t tri0) {
         if constexpr (kDirectOK) {
@@ -638,7 +813,7 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         // weights average out and the claim stays up front.  The host decides (ConvertPlan::claim_late).
         const bool claim_late = kDirectOK && a.claim_late != 0;
         if (lane == 0) {
-            if (a.n_units > nwarps_total && !claim_late) next = claim_base + atomicAdd(SCHED(a, 0), 1u);  // needed only after the set-up
+            if (a.n_units > nwarps_total && !claim_late) next = claim();  // needed only after the set-up
             tma_store_wait_read();  // the previous unit's record store has finished reading wb.rec
         }
         mbar_wait(&wb.bar, phase);
@@ -650,8 +825,6 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         // ---- per-triangle stage: one lane per triangle ----
         uint32_t cnt = 0;
         TriSetup ts;
-        ts.w = 1; ts.h = 0; ts.incl = 0;
-        ts.A[0] = ts.A[1] = ts.A[2] = ts.B[0] = ts.B[1] = ts.B[2] = 0; ts.E0[0] = ts.E0[1] = ts.E0[2] = 0;
         Rec& myrec = wb.rec[lane];
         if ((uint32_t)lane < ntri) cnt = setup_triangle<RK>(wb.tri + lane * 9, a.tri_first + t0 + lane, a, tabs, ts, myrec);
         __syncwarp();
@@ -681,21 +854,11 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         const unsigned long long hits = box_mask(e0, e1, e2, a0, a1, a2, b0, b1, b2, w, mine, __reduce_max_sync(0xffffffffu, mine));
         const uint32_t nh = (uint32_t)__popcll(hits);
         // the scans run over the lanes of one unit: TriRec::first is relative to the triangle's own unit
-        uint32_t incl_scan = nh;  // inclusive scan
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const uint32_t v = __shfl_up_sync(0xffffffffu, incl_scan, d, sw);
-            if ((lane & (sw - 1)) >= d) incl_scan += v;
-        }
+        const uint32_t incl_scan = warp_inclusive_scan(nh, lane, sw);
         const uint32_t tot0 = __shfl_sync(0xffffffffu, incl_scan, sw - 1);   // small-triangle fragments of the first unit
         const uint32_t tot1 = __shfl_sync(0xffffffffu, incl_scan, 31);       // ... and of the second (paired pass)
         const uint32_t myrows = small ? (uint32_t)ts.h : 0u;  // rows this triangle contributes to the unit item's span table
-        uint32_t rows_scan = myrows;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const uint32_t v = __shfl_up_sync(0xffffffffu, rows_scan, d, sw);
-            if ((lane & (sw - 1)) >= d) rows_scan += v;
-        }
+        const uint32_t rows_scan = warp_inclusive_scan(myrows, lane, sw);
         if ((uint32_t)lane < ntri) {
             myrec.hits = hits;
             myrec.first = (incl_scan - nh) | ((rows_scan - myrows) << 16);
@@ -715,11 +878,11 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         const unsigned hmask = sw == 32 ? 0xffffffffu : 0xffffu << (hf * 16);   // the lanes of that unit
         const bool my_direct = hf ? direct1 : direct0;
         const uint32_t dfr0 = direct0 ? tot0 : 0u, dsum = dfr0 + (direct1 ? tot1 : 0u);   // the pass's list: unit 0's, then unit 1's
-        auto claim = [&]() {   // the next unit, claimed once this one's work is known
-            if (lane == 0) next = claim_base + atomicAdd(SCHED(a, 0), 1u);
+        auto claim_now = [&]() {   // the next unit, claimed once this one's work is known
+            if (lane == 0) next = claim();
             next = __shfl_sync(0xffffffffu, next, 0);
         };
-        if (claim_late && !direct) claim();
+        if (claim_late && !direct) claim_now();
         if (!direct && lane == 0 && next < a.n_units) issue_load(next, a.unit_tris);
 
         // ---- all other triangles: the warp counts one triangle at a time, one lane per pixel row; the tall triangles of
@@ -742,18 +905,12 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
                     int h;
                     const RowState rs = row_state(wb.rec[s], h);
                     const uint32_t nb = (uint32_t)(h + 31) / 32u, nent = (nb + kDeferBlocks - 1) / kDeferBlocks;
-                    uint32_t base = 0;
-                    if (lane == 0) base = atomicAdd_block(&cq.tail, nent);
-                    base = __shfl_sync(0xffffffffu, base, 0);
-                    const uint32_t fit = base < kCtaQueueCap ? min(nent, kCtaQueueCap - base) : 0u;  // the first `fit` pieces go to the queue
-                    if ((uint32_t)lane < fit) {
-                        CtaEntry& e = cq.q[base + lane];
+                    const CtaPost q = cta_reserve(cq, nent, lane);   // the first q.fit pieces go to the queue
+                    cta_publish(cq, q.base, q.fit, lane, [&](CtaEntry& e, uint32_t i) {
                         e.rs = rs; e.h = h; e.unit = u; e.slot = (uint32_t)s - lo;
-                        e.rb0 = lane * kDeferBlocks; e.rb1 = min(nb, (lane + 1) * kDeferBlocks);
-                        __threadfence_block();
-                        e.ready = 1u;
-                    }
-                    if (fit < nent) count_blocks<RK>(a, wb, u, st, rs, h, (uint32_t)s - lo, (int)(fit * kDeferBlocks), 1 << 20, lane);  // the rest stays here
+                        e.rb0 = i * kDeferBlocks; e.rb1 = min(nb, (i + 1) * kDeferBlocks);
+                    });
+                    if (q.fit < nent) count_blocks<RK>(a, wb, u, st, rs, h, (uint32_t)s - lo, (int)(q.fit * kDeferBlocks), 1 << 20, lane);  // the rest stays here
                     gm &= ~(1u << s);
                 }
             }
@@ -784,57 +941,15 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
                 cp_async_wait_all();   // wb.logtab has landed (a no-op after the first direct unit)
                 __syncwarp();
                 TR_PHASE(a, kTrList);
-                const uint32_t tri0 = a.tri_first + t0;
-                // the pass's list [0, dsum) is cut into groups of 32 from 0, across the boundary of its two units: only the
-                // last group can be partial.  This warp shades the first kShareFirst fragments at once; the rest goes to the
-                // CTA's help queue in pieces of kSharePiece, which this warp then shades in order unless another warp has
-                // taken them: a warp that is out of units takes the pieces this warp has not reached (the late claim cannot
-                // balance a pass's weight)
-                const uint32_t npiece = dsum > kShareFirst ? (dsum - kShareFirst + kSharePiece - 1) / kSharePiece : 0u;
-                uint32_t qbase = 0, fit = 0;
-                if (npiece) {
-                    if (lane == 0) qbase = atomicAdd_block(&cq.tail, npiece);
-                    qbase = __shfl_sync(0xffffffffu, qbase, 0);
-                    fit = qbase < kCtaQueueCap ? min(npiece, kCtaQueueCap - qbase) : 0u;   // the rest is this warp's own
-                    if (lane == 0) wb.left = fit;
-                    __threadfence_block();   // the count, the records and the list, before the pieces are posted
-                    __syncwarp();
-                    if ((uint32_t)lane < fit) {
-                        CtaEntry& e = cq.q[qbase + lane];
-                        e.h = -1;
-                        e.sp.first = dfirst; e.sp.owner = (uint32_t)warp; e.sp.tri0 = tri0;
-                        e.sp.f0 = kShareFirst + lane * kSharePiece; e.sp.f1 = min(dsum, e.sp.f0 + kSharePiece);
-                        __threadfence_block();
-                        e.ready = 1u;
-                    }
-                }
-                shade(wb, 0, min(dsum, kShareFirst), dfirst, tri0);
-                uint32_t done = 0;   // posted pieces this warp shaded itself
-                for (uint32_t p = 0; p < npiece; ++p) {
-                    uint32_t won = 1;
-                    if (p < fit) {
-                        if (lane == 0) won = atomicExch(&cq.q[qbase + p].taken, 1u) == 0u;
-                        won = __shfl_sync(0xffffffffu, won, 0);
-                        done += won;
-                    }
-                    const uint32_t f0 = kShareFirst + p * kSharePiece;
-                    if (won) shade(wb, f0, min(dsum, f0 + kSharePiece), dfirst, tri0);
-                }
+                const DirectShare sh = direct_share(cq, wb, (uint32_t)warp, dsum, dfirst, a.tri_first + t0, shade, lane);
                 TR_PHASE(a, kTrShade);
                 // the stage was written through the generic proxy: every writer fences before the TMA engine writes there again
                 fence_proxy_async();
                 __syncwarp();
-                if (claim_late) claim();
+                if (claim_late) claim_now();
                 if (lane == 0) tma_store_wait_read();   // the last groups' copies have read the stage
                 if (lane == 0 && next < a.n_units) issue_load(next, a.unit_tris);
-                if (fit) {   // other warps may still read this slice's records and list: wait before they are rewritten
-                    if (lane == 0) {
-                        if (done) atomicSub_block(&wb.left, done);
-                        while (*reinterpret_cast<volatile uint32_t*>(&wb.left) != 0u) __nanosleep(32);
-                        __threadfence_block();
-                    }
-                    __syncwarp();
-                }
+                direct_share_wait(wb, sh, lane);
             }
         }
 
@@ -854,88 +969,10 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         pair = false;
         TR_PHASE(a, kTrUnitEnd);
     }
-    // ---- help: tickets on the CTA's queue until no warp of the CTA can post any more ----
-    if (lane == 0) atomicSub_block(&cq.active, 1u);
-    for (;;) {
-        uint32_t t = 0;
-        if (lane == 0) t = atomicAdd_block(&cq.head, 1u);
-        t = __shfl_sync(0xffffffffu, t, 0);
-        if (t >= kCtaQueueCap) break;  // beyond the capacity nothing is ever posted
-        bool have = false;
-        if (lane == 0) {
-            unsigned ns = 64;   // the waiters must not take issue slots from the warps still working
-            for (;;) {
-                if (*reinterpret_cast<volatile uint32_t*>(&cq.tail) > t) { have = true; break; }
-                if (*reinterpret_cast<volatile uint32_t*>(&cq.active) == 0 && *reinterpret_cast<volatile uint32_t*>(&cq.tail) <= t) break;
-                __nanosleep(ns);
-                ns = min(ns * 2u, 256u);
-            }
-            if (have) while (cq.q[t].ready == 0u) __nanosleep(20);
-            __threadfence_block();
-        }
-        if (!__shfl_sync(0xffffffffu, (int)have, 0)) break;
-        const CtaEntry& e = cq.q[t];
-        if (e.h < 0) {   // a shading piece: unless its owner got there first
-            if constexpr (kDirectOK) {
-                uint32_t won = 0;
-                if (lane == 0) won = atomicExch(&cq.q[t].taken, 1u) == 0u;
-                if (__shfl_sync(0xffffffffu, won, 0)) {
-                    WarpBlock<RK>& src = *reinterpret_cast<WarpBlock<RK>*>(smem + (size_t)e.sp.owner * sizeof(WarpBlock<RK>));
-                    cp_async_wait_all();   // this warp's wb.logtab, if it never shaded a unit of its own
-                    __syncwarp();
-                    shade(src, e.sp.f0, e.sp.f1, e.sp.first, e.sp.tri0);
-                    __syncwarp();
-                    if (lane == 0) { __threadfence_block(); atomicSub_block(&src.left, 1u); }   // its slice may be rewritten
-                }
-            }
-            continue;
-        }
-        const RowState rs = e.rs;
-        const int h = e.h;
-        const uint32_t eu = e.unit, es = e.slot;
-        const int rb0 = (int)e.rb0, rb1 = (int)e.rb1;
-        count_blocks<RK>(a, wb, eu, st, rs, h, es, rb0, rb1, lane);
-        stash_close_item<RK>(a, wb, eu, st, lane);
-        stash_flush<RK>(a, wb, eu, st, lane);
-    }
+    help_cta<RK>(a, smem, wb, st, cq, shade, lane);
     if (lane == 0) tma_store_wait_all();  // record stores are complete (not just read) before the kernel ends
     if constexpr (kDirectOK) cp_async_wait_all();   // a warp without a direct unit never waited for its wb.logtab
-    // ---- last CTA out publishes the counts and re-arms the scheduler for the next launch ---------
-    __syncthreads();
-    if (warp == 0) {
-        uint32_t last = 0;
-        unsigned long long tot = 0;
-        if (lane == 0) {
-            __threadfence();
-            const uint32_t done = atomicAdd(SCHED(a, 4), 1u);
-            if (done == gridDim.x - 1) {
-                __threadfence();
-                last = 1;
-                const unsigned long long packed = *reinterpret_cast<volatile unsigned long long*>(a.counter);
-                tot = packed & kFragMask;                       // fragments generated
-                *a.total_out = tot;
-                *a.n_items_out = (uint32_t)(packed >> 40);      // work items queued
-                *a.counter = 0ull;
-                if (a.host_total) {  // zero-copy count for the host (PCIe posted write, ~1 us)
-                    *reinterpret_cast<volatile unsigned long long*>(a.host_total) = tot;
-                    __threadfence_system();
-                    *reinterpret_cast<volatile unsigned long long*>(a.host_total + 1) = a.host_tag;
-                }
-                *SCHED(a, 0) = 0; *SCHED(a, 4) = 0;
-                __threadfence();
-            }
-        }
-        if (a.world > 1) {  // fused gather: tell every peer how many records this rank will write, one lane per peer
-            last = __shfl_sync(0xffffffffu, last, 0);
-            tot = __shfl_sync(0xffffffffu, tot, 0);
-            if (last && (uint32_t)lane < a.world) {
-                const unsigned long long mine = tot < a.cap ? tot : a.cap;
-                a.peer_xch[lane][a.rank * 4 + 0] = mine;
-                __threadfence_system();
-                st_release_sys(a.peer_xch[lane] + a.rank * 4 + 1, a.epoch);
-            }
-        }
-    }
+    raster_last_cta(a, warp, lane);
 #ifdef M2S_TRACE
     TR_PHASE(a, kTrTail);
     TR_ADD(a, kTrCycles, clock64() - tr_c0_);   // with kTrNanos: the SM clock the cycles convert at

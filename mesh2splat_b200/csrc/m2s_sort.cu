@@ -45,12 +45,7 @@ __device__ __forceinline__ uint32_t load_acquire(uint32_t* p) {
 // exclusive prefix of one value per thread over the CTA (thread order); s_warp: kSortWarps words
 __device__ __forceinline__ uint32_t cta_exclusive_scan(uint32_t v, uint32_t* s_warp) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t x = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
-        if (lane >= o) x += y;
-    }
+    const uint32_t x = warp_inclusive_scan(v, lane);
     if (lane == 31) s_warp[warp] = x;
     __syncthreads();
     uint32_t before = 0;

@@ -5,6 +5,8 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "m2s_ptx.cuh"
+
 namespace m2s {
 
 constexpr int kSortThreads = 256;                              // one thread per digit in the per-digit steps
