@@ -229,7 +229,7 @@ m2s_status m2s_convert_timed(m2s_ctx* ctx, const m2s_dscene* scene, const m2s_pa
  * the texture rows the converted triangle range can sample.  With >= 16384 triangles the call is pipelined: the
  * triangle range is converted in chunks (each bringing its triangles and texture rows with it) whose records are
  * appended on the device, and each chunk's download overlaps the next chunk's upload and kernels (pass pinned host
- * memory to benefit; M2S_HOST_CHUNKS=n overrides the chunk count, 1 = unpipelined).  The cap and the returned total
+ * memory to benefit).  The cap and the returned total
  * behave as in one launch. */
 m2s_status m2s_convert_host(m2s_ctx* ctx, const m2s_scene* scene, const m2s_params* params,
                             void* h_out, uint64_t out_capacity, uint64_t* h_keys,

@@ -176,12 +176,13 @@ class Context:
         return DeviceScene(self, h.value, scene)
 
     # ---- the hot path ----
-    def default_capacity(self, dscene: DeviceScene, resolution: int, max_gaussians: int, flags: int) -> int:
+    @staticmethod
+    def default_capacity(primitive_count: int, resolution: int, max_gaussians: int, flags: int) -> int:
         if max_gaussians:
             return max_gaussians
         if flags & _abi.FLAG_UNCAPPED:
-            return 6 * resolution * resolution * max(1, dscene.primitive_count)
-        return _abi.reference_capacity(resolution, dscene.primitive_count)
+            return 6 * resolution * resolution * max(1, primitive_count)
+        return _abi.reference_capacity(resolution, primitive_count)
 
     def convert(self, dscene: DeviceScene, resolution: int, layout: int = _abi.LAYOUT_REF96,
                 gaussian_std: float = 0.65, max_gaussians: int = 0, flags: int = 0, first_triangle: int = 0,
@@ -190,7 +191,7 @@ class Context:
         torch = _torch()
         stride = _abi.STRIDES[layout]
         if capacity is None:
-            capacity = self.default_capacity(dscene, resolution, max_gaussians, flags)
+            capacity = self.default_capacity(dscene.primitive_count, resolution, max_gaussians, flags)
         dev = torch.device("cuda", self.device)
         if out is None:
             out = torch.empty(max(1, capacity) * stride, dtype=torch.uint8, device=dev)
@@ -473,12 +474,7 @@ class Context:
         out / keys: optional caller-owned host arrays (uint8, >= capacity * stride bytes / uint64, >= capacity)."""
         stride = _abi.STRIDES[layout]
         if capacity is None:
-            if max_gaussians:
-                capacity = max_gaussians
-            elif flags & _abi.FLAG_UNCAPPED:
-                capacity = 6 * resolution * resolution * max(1, len(scene.primitives))
-            else:
-                capacity = _abi.reference_capacity(resolution, len(scene.primitives))
+            capacity = self.default_capacity(len(scene.primitives), resolution, max_gaussians, flags)
         if out is None:
             out = np.empty(max(1, capacity) * stride, np.uint8)
         if want_keys and keys is None:

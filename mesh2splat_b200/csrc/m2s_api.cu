@@ -47,8 +47,7 @@ M2S_EXPORT void m2s_params_default(m2s_params* p) {
 
 // everything a context owns beyond its device and SM count; on failure m2s_ctx_destroy releases what was made so far
 static m2s_status ctx_init(m2s_ctx* c) {
-    for (cudaStream_t* s : {&c->stream, &c->stream2, &c->stream3, &c->stream4, &c->stream5}) CUDA_TRY(cudaStreamCreateWithFlags(s, cudaStreamNonBlocking));
-    c->up = c->tex_up = c->mip = c->aux = c->stream;
+    CUDA_TRY(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
     cudaMemPool_t pool;
     CUDA_TRY(cudaDeviceGetDefaultMemPool(&pool, c->device));
     uint64_t thresh = UINT64_MAX;  // keep freed blocks cached: uploads in steady state never hit cudaMalloc
@@ -62,12 +61,9 @@ static m2s_status ctx_init(m2s_ctx* c) {
     *c->h_status = 0;
     CUDA_TRY(cudaHostGetDevicePointer((void**)&c->d_status, c->h_status, 0));
     for (cudaEvent_t* ev : {&c->ev0, &c->ev1}) CUDA_TRY(cudaEventCreate(ev));
-    CUDA_TRY(cudaEventCreateWithFlags(&c->ev_alloc, cudaEventDisableTiming));
-    for (int i = 0; i < m2s_ctx::kMaxChunks; ++i)
-        for (cudaEvent_t* ev : {&c->ev_tri[i], &c->ev_up[i], &c->ev_chunk[i]}) CUDA_TRY(cudaEventCreateWithFlags(ev, cudaEventDisableTiming));
-    CUDA_TRY(cudaMalloc(&c->d_chunk_tot, m2s_ctx::kMaxChunks * sizeof(unsigned long long)));
-    CUDA_TRY(cudaHostAlloc(&c->h_chunk_tot, 2 * m2s_ctx::kMaxChunks * sizeof(unsigned long long), cudaHostAllocMapped));
-    std::memset(c->h_chunk_tot, 0, 2 * m2s_ctx::kMaxChunks * sizeof(unsigned long long));
+    for (cudaEvent_t* ev : {&c->ev_stage[0], &c->ev_stage[1]}) CUDA_TRY(cudaEventCreateWithFlags(ev, cudaEventDisableTiming));
+    const m2s_status st = c->pipeline.create();
+    if (st != M2S_OK) return st;
     for (int l = 0; l < m2s_ctx::kLayouts; ++l) {
         CUDA_TRY(raster_configure(l, &c->blocks_per_sm[l]));
         CUDA_TRY(fragment_configure(l, &c->frag_blocks_per_sm[l]));
@@ -110,17 +106,10 @@ M2S_EXPORT void m2s_ctx_destroy(m2s_ctx* c) {
     cudaFree(c->d_sched); cudaFree(c->d_counter); cudaFree(c->d_total); cudaFree(c->d_nitems);
     if (c->h_total) cudaFreeHost(c->h_total);
     if (c->h_status) cudaFreeHost(c->h_status);
-    cudaFree(c->d_chunk_tot);
-    if (c->h_chunk_tot) cudaFreeHost(c->h_chunk_tot);
     for (int i = 0; i < 2; ++i) if (c->h_stage[i]) cudaFreeHost(c->h_stage[i]);
-    for (auto& v : c->vr) { if (v.d_minmax) cudaFree(v.d_minmax); if (v.h_minmax) cudaFreeHost(v.h_minmax); if (v.ev) cudaEventDestroy(v.ev); }
-    for (int i = 0; i < m2s_ctx::kMaxChunks; ++i) {
-        if (c->ev_chunk[i]) cudaEventDestroy(c->ev_chunk[i]);
-        if (c->ev_tri[i]) cudaEventDestroy(c->ev_tri[i]);
-        if (c->ev_up[i]) cudaEventDestroy(c->ev_up[i]);
-    }
-    for (cudaEvent_t ev : {c->ev0, c->ev1, c->ev_mid, c->ev_alloc}) if (ev) cudaEventDestroy(ev);
-    for (cudaStream_t s : {c->stream2, c->stream3, c->stream4, c->stream5, c->stream}) if (s) cudaStreamDestroy(s);
+    c->pipeline.release();
+    for (cudaEvent_t ev : {c->ev0, c->ev1, c->ev_mid, c->ev_stage[0], c->ev_stage[1]}) if (ev) cudaEventDestroy(ev);
+    if (c->stream) cudaStreamDestroy(c->stream);
     delete c;
 }
 

@@ -1,9 +1,7 @@
 // m2s_convert.cu — C-ABI implementation (include/m2s.h): the conversion.  Its launch plan, the enqueue and synchronous
 // forms, the pipelined host-to-host conversion (m2s_convert_host), and the .ply outputs.
-#include <chrono>
 #include <cmath>
 #include <cstdio>
-#include <cstdlib>
 
 #include "m2s_ctx.cuh"
 
@@ -248,202 +246,237 @@ M2S_EXPORT m2s_status m2s_convert_timed(m2s_ctx* ctx, const m2s_dscene* s, const
     return M2S_OK;
 }
 
+// ---- host buffers in, host buffers out: the pipelined conversion ------------------------------------------------------
+m2s_status m2s::HostPipeline::create() {
+    for (cudaStream_t* s : {&tri_stream, &tex_stream, &vr_stream, &dl_stream}) CUDA_TRY(cudaStreamCreateWithFlags(s, cudaStreamNonBlocking));
+    CUDA_TRY(cudaEventCreateWithFlags(&ev_alloc, cudaEventDisableTiming));
+    for (int i = 0; i < kMaxChunks; ++i)
+        for (cudaEvent_t* ev : {&ev_tri[i], &ev_up[i], &ev_chunk[i]}) CUDA_TRY(cudaEventCreateWithFlags(ev, cudaEventDisableTiming));
+    CUDA_TRY(cudaMalloc(&d_chunk_tot, kMaxChunks * sizeof(unsigned long long)));
+    CUDA_TRY(cudaHostAlloc(&h_chunk_tot, 2 * kMaxChunks * sizeof(unsigned long long), cudaHostAllocMapped));
+    std::memset(h_chunk_tot, 0, 2 * kMaxChunks * sizeof(unsigned long long));
+    return M2S_OK;
+}
+
+void m2s::HostPipeline::release() {
+    cudaFree(d_chunk_tot);
+    if (h_chunk_tot) cudaFreeHost(h_chunk_tot);
+    for (VRangeSlot& v : vr) { if (v.d_minmax) cudaFree(v.d_minmax); if (v.h_minmax) cudaFreeHost(v.h_minmax); if (v.ev) cudaEventDestroy(v.ev); }
+    for (int i = 0; i < kMaxChunks; ++i)
+        for (cudaEvent_t ev : {ev_tri[i], ev_up[i], ev_chunk[i]}) if (ev) cudaEventDestroy(ev);
+    if (ev_alloc) cudaEventDestroy(ev_alloc);
+    for (cudaStream_t s : {tri_stream, tex_stream, vr_stream, dl_stream}) if (s) cudaStreamDestroy(s);
+}
+
+namespace {
+
+constexpr int kMaxChunks = HostPipeline::kMaxChunks;
+// triangle chunks (and their v-range reductions) queued ahead of the chunk whose texture rows go up: the first records
+// exist after ~kLookahead/nchunks of the triangles and 1/nchunks of the texture rows (the downloads of the records are
+// the longest leg of the call: they must start early; queueing every triangle chunk up front delays them)
+constexpr int kLookahead = 2;
+
+// M2S_OK, or M2S_E_CUDA with the error "<what>: <e>"
+m2s_status cuda_status(const char* what, cudaError_t e) {
+    if (e == cudaSuccess) return M2S_OK;
+    set_error(std::string(what) + ": " + cudaGetErrorString(e));
+    return M2S_E_CUDA;
+}
+
+// One m2s_convert_host call: a pipeline over the chunks of its triangle range.  Chunk c's records are appended after
+// chunk c-1's on the device (the fragment kernel adds the earlier chunks' counts, prev_totals).  (1) The triangle chunks
+// go up back to back on the triangle stream, kLookahead ahead of the chunk being converted, each followed on the v-range
+// stream by the reduction of its v-range per texture and an 8-byte-per-texture copy back.  (2) Per chunk, as soon as its
+// v-range is on the host: the texture row groups it samples (not yet resident) go up on the texture stream, and the
+// compute stream (the context's) generates their mip rows and runs the two kernels.  (3) A chunk's records start
+// crossing PCIe on the download stream as soon as its count has arrived (zero-copy, from the raster kernel's last CTA),
+// while later chunks are still being uploaded and converted.  The first records exist after ~1/nchunks of the upload; a
+// shard (first_triangle/triangle_count) never uploads texture rows it does not sample.
+struct HostConvert {
+    m2s_ctx* ctx;
+    HostPipeline& hp;                           // ctx->pipeline
+    const m2s_scene* sc;                        // the call's arguments
+    const m2s_params* p;
+    unsigned char* h_out;
+    uint64_t* h_keys;
+    uint64_t out_capacity;
+    uint32_t stride;                            // record bytes of p->layout
+    m2s_dscene* ds = nullptr;
+    uint64_t cap = 0;                           // the effective cap
+    uint64_t first = 0, end = 0, per = 0;       // the triangle range [first, end), in chunks of `per` triangles
+    int nchunks = 0, uploaded = 0, launched = 0, downloaded = 0;  // chunks planned; with triangles, kernels, downloads enqueued
+    unsigned long long tags[kMaxChunks] = {};   // the tag each chunk's count arrives with
+    uint64_t base = 0, written = 0;             // records of the downloaded chunks: generated, and stored
+
+    uint64_t lo(int c) const { return first + (uint64_t)c * per; }
+    uint64_t hi(int c) const { return std::min(end, lo(c) + per); }
+
+    // the chunk plan: under 16384 triangles one chunk, otherwise count / 16384 chunks, 2 to 4.  Every chunk shortens the
+    // tail (the last chunk's kernels and download) and costs ~25 us of kernel latency on the compute stream, hidden behind
+    // the uploads; chunks of >= 8 k triangles keep the GPU filled.  No chunk is empty unless the range is.
+    void plan(const TriRange& tr) {
+        first = tr.first;
+        end = tr.first + tr.count;
+        nchunks = tr.count < 16384 ? 1 : (int)std::clamp<uint64_t>(tr.count / 16384, 2, kMaxChunks);
+        per = (tr.count + nchunks - 1) / nchunks;
+    }
+
+    // the start event, and the upload streams behind the allocations and table copies made on the compute stream
+    m2s_status start() {
+        cudaError_t e = cudaEventRecord(ctx->ev0, ctx->stream);
+        if (e == cudaSuccess) e = cudaEventRecord(hp.ev_alloc, ctx->stream);
+        for (cudaStream_t s : {hp.tri_stream, hp.tex_stream, hp.vr_stream})
+            if (e == cudaSuccess) e = cudaStreamWaitEvent(s, hp.ev_alloc, 0);
+        return cuda_status("convert_host", e);
+    }
+
+    // (1) chunk c's triangles, then the reduction of its v-range behind "chunk c is resident"
+    m2s_status upload_tris(int c) {
+        const uint64_t n = hi(c) - lo(c);
+        cudaError_t e = cudaSuccess;
+        if (n) {
+            e = cudaMemcpyAsync(reinterpret_cast<unsigned char*>(ds->d_tris) + lo(c) * (size_t)kTriBytes,
+                                reinterpret_cast<const unsigned char*>(sc->triangles) + lo(c) * (size_t)kTriBytes,
+                                n * (size_t)kTriBytes, cudaMemcpyHostToDevice, hp.tri_stream);
+            ds->h2d_bytes += n * (uint64_t)kTriBytes;
+        }
+        if (e == cudaSuccess) e = cudaEventRecord(hp.ev_tri[c], hp.tri_stream);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(hp.vr_stream, hp.ev_tri[c], 0);
+        if (e != cudaSuccess) return cuda_status("convert_host upload", e);
+        return vrange_enqueue(ctx, ds, hp.vr_stream, lo(c), hi(c), c);
+    }
+
+    // (2) chunk c's texture rows once its v-range has arrived (the downloads that are ready are enqueued meanwhile), then
+    // their mip rows on the compute stream, behind the rows and the chunk's triangles
+    m2s_status texture_rows(int c) {
+        std::vector<MipRun> runs;
+        const m2s_status st = upload_groups_from_vrange(ctx, ds, hp.tex_stream, c, [&] { return downloads(false); }, &runs);
+        if (st != M2S_OK) return st;
+        cudaError_t e = cudaEventRecord(hp.ev_up[c], hp.tex_stream);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(ctx->stream, hp.ev_up[c], 0);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(ctx->stream, hp.ev_tri[c], 0);
+        if (e != cudaSuccess) return cuda_status("convert_host", e);
+        for (const MipRun& r : runs) {
+            e = mip_groups_launch(ds->d_arena, ds->h_texs[r.t], r.g0, r.g1, ctx->stream);
+            if (e != cudaSuccess) return cuda_status("convert_host mips", e);
+        }
+        return M2S_OK;
+    }
+
+    // (2) chunk c's kernels, appending after the earlier chunks' records; the count reaches its mapped slot with a fresh tag
+    m2s_status launch(int c) {
+        unsigned long long* h_dev = nullptr;  // device view of the mapped count slot
+        cudaError_t e = cudaHostGetDevicePointer((void**)&h_dev, hp.h_chunk_tot + 2 * c, 0);
+        if (e != cudaSuccess) return cuda_status("convert_host", e);
+        tags[c] = ++hp.host_seq;
+        if (hi(c) > lo(c)) {
+            m2s_params pc = *p;
+            pc.first_triangle = lo(c);
+            pc.triangle_count = hi(c) - lo(c);
+            const m2s_status st = convert_enqueue_impl(ctx, ds, &pc, ctx->out.p, out_capacity, h_keys ? (uint64_t*)ctx->keys.p : nullptr,
+                                                       (uint64_t*)(hp.d_chunk_tot + c), ctx->stream, nullptr, hp.d_chunk_tot,
+                                                       (uint32_t)c, h_dev, tags[c]);
+            if (st != M2S_OK) return st;
+        } else {  // empty range: nothing to launch, the count is zero
+            e = cudaMemsetAsync(hp.d_chunk_tot + c, 0, sizeof(unsigned long long), ctx->stream);
+            if (e != cudaSuccess) return cuda_status("convert_host", e);
+            hp.h_chunk_tot[2 * c] = 0;
+            __atomic_store_n(&hp.h_chunk_tot[2 * c + 1], tags[c], __ATOMIC_RELEASE);
+        }
+        e = cudaEventRecord(hp.ev_chunk[c], ctx->stream);
+        if (e != cudaSuccess) return cuda_status("convert_host", e);
+        ++launched;
+        return M2S_OK;
+    }
+
+    // (3) the downloads of the launched chunks whose counts have arrived, in order; block: wait for every count
+    m2s_status downloads(bool block) {
+        for (; downloaded < launched; ++downloaded) {
+            const int c = downloaded;
+            volatile unsigned long long* slot = hp.h_chunk_tot + 2 * c;
+            for (;;) {
+                if (__atomic_load_n(&hp.h_chunk_tot[2 * c + 1], __ATOMIC_ACQUIRE) == tags[c]) break;  // count is ordered before the tag
+                if (!block) return M2S_OK;
+                const cudaError_t q = cudaEventQuery(hp.ev_chunk[c]);
+                if (q == cudaSuccess) break;             // finished: the tag is there
+                if (q != cudaErrorNotReady) return cuda_status("convert_host download", q);
+            }
+            if (__atomic_load_n(&hp.h_chunk_tot[2 * c + 1], __ATOMIC_ACQUIRE) != tags[c]) return cuda_status("convert_host download", cudaErrorUnknown);
+            const uint64_t tot = slot[0];
+            const uint64_t room = cap > base ? cap - base : 0, w = std::min(tot, room);
+            if (w) {
+                cudaError_t e = cudaStreamWaitEvent(hp.dl_stream, hp.ev_chunk[c], 0);
+                if (e == cudaSuccess)
+                    e = cudaMemcpyAsync(h_out + base * stride, reinterpret_cast<const unsigned char*>(ctx->out.p) + base * stride, w * stride,
+                                        cudaMemcpyDeviceToHost, hp.dl_stream);
+                if (e == cudaSuccess && h_keys)
+                    e = cudaMemcpyAsync(h_keys + base, static_cast<const uint64_t*>(ctx->keys.p) + base, w * 8, cudaMemcpyDeviceToHost, hp.dl_stream);
+                if (e != cudaSuccess) return cuda_status("convert_host download", e);
+            }
+            base += tot;
+            written += w;
+        }
+        return M2S_OK;
+    }
+
+    // the stop event, every download, and every stream idle
+    m2s_status drain() {
+        m2s_status st = cuda_status("convert_host", cudaEventRecord(ctx->ev1, ctx->stream));
+        if (st == M2S_OK) st = downloads(true);
+        if (st != M2S_OK) return st;
+        cudaError_t e = cudaSuccess;
+        for (cudaStream_t s : {hp.dl_stream, ctx->stream, hp.tri_stream, hp.tex_stream, hp.vr_stream})
+            if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        return cuda_status("convert_host download", e);
+    }
+
+    // the one failure path once the streams have work: all five streams are idle before the scene is freed, and the next
+    // call resets the scheduler state and re-arms the v-range slots
+    m2s_status fail(m2s_status st) {
+        for (cudaStream_t s : {hp.tri_stream, hp.tex_stream, hp.vr_stream, ctx->stream, hp.dl_stream}) cudaStreamSynchronize(s);
+        ctx->dirty = true;
+        hp.vr_dirty = true;
+        m2s_scene_free(ctx, ds);
+        return st;
+    }
+};
+
+}  // namespace
+
 M2S_EXPORT m2s_status m2s_convert_host(m2s_ctx* ctx, const m2s_scene* sc, const m2s_params* p, void* h_out, uint64_t out_capacity,
                                        uint64_t* h_keys, m2s_result* res) {
     if (!ctx || !sc || !p || (!h_out && out_capacity)) { set_error("m2s_convert_host: NULL argument"); return M2S_E_INVALID; }
     const uint32_t stride = m2s_record_stride(p->layout);
     if (!stride) { set_error("m2s_convert_host: unknown layout"); return M2S_E_INVALID; }
     CUDA_TRY(cudaSetDevice(ctx->device));
-    SlimScene slim_holder(sc, p->layout);
-    const m2s_scene& slim = slim_holder.scene;
-    // Pipeline (REF96 / PACKED56, meshes large enough to split): the triangle range is cut into chunks; chunk c's
-    // records are appended after chunk c-1's on the device (fragment kernel: prev_totals) and start crossing
-    // PCIe on a second stream while chunk c+1 is still being uploaded and converted — H2D and D2H overlap.
+    HostConvert hc{ctx, ctx->pipeline, sc, p, static_cast<unsigned char*>(h_out), h_keys, out_capacity, stride};
+    // the tables on the compute stream; the triangles and the texture rows come with the chunks
+    const SlimScene slim(sc, p->layout);
     const TriRange tr = tri_range(p->first_triangle, p->triangle_count, sc->triangle_count);
-    const uint64_t first = tr.first, count = tr.count;
-    int nchunks = 1;
-    if (count >= 16384) {  // every layout: the fragment kernel appends after the earlier chunks' records itself
-        // every chunk shortens the tail (the last chunk's kernels and download) and costs ~25 us of kernel latency on the
-        // compute stream, hidden behind the uploads; chunks of >= 8 k triangles keep the GPU filled
-        nchunks = (int)std::max<uint64_t>(2, std::min<uint64_t>(4, count / 16384));
-        if (const char* e = std::getenv("M2S_HOST_CHUNKS")) nchunks = std::max(1, std::min(m2s_ctx::kMaxChunks, std::atoi(e)));
-    }
-    const uint64_t per = (count + nchunks - 1) / nchunks;
-    m2s_dscene* ds = nullptr;
-    // Pipeline: (1) the triangle chunks go up back to back, each followed by a reduction of its v-range per texture and
-    // a 8-byte-per-texture copy back; (2) per chunk, as soon as its v-range is on the host: the texture row groups it
-    // samples (not yet resident) go up, the two kernels are enqueued; (3) a chunk's records start crossing PCIe on a
-    // second stream as soon as its count has arrived (zero-copy, from the raster kernel's last CTA) while later chunks
-    // are still being uploaded and converted.  The first records exist after ~1/nchunks of the upload; a shard
-    // (first_triangle/triangle_count) never uploads texture rows it does not sample.
-    m2s_status st = scene_upload_impl(ctx, &slim, &ds, 0, false, first, true);
+    m2s_status st = scene_upload_impl(ctx, &slim.scene, &hc.ds, 0, false, tr.first, true);
     if (st != M2S_OK) return st;
     st = grow(ctx, ctx->out, std::max<uint64_t>(out_capacity, 1) * stride);
     if (st == M2S_OK && h_keys) st = grow(ctx, ctx->keys, std::max<uint64_t>(out_capacity, 1) * 8);
-    if (st != M2S_OK) { cudaStreamSynchronize(ctx->stream); m2s_scene_free(ctx, ds); return st; }
-    unsigned long long* const d_keys = static_cast<unsigned long long*>(ctx->keys.p);
+    if (st != M2S_OK) { cudaStreamSynchronize(ctx->stream); m2s_scene_free(ctx, hc.ds); return st; }
+    hc.cap = effective_cap(hc.ds, p, out_capacity);
+    hc.plan(tr);
+    st = hc.start();
+    while (st == M2S_OK && hc.uploaded < std::min(hc.nchunks, kLookahead)) st = hc.upload_tris(hc.uploaded++);
+    for (int c = 0; st == M2S_OK && c < hc.nchunks; ++c) {
+        st = hc.texture_rows(c);
+        if (st == M2S_OK && hc.uploaded < hc.nchunks) st = hc.upload_tris(hc.uploaded++);  // the next look-ahead chunk
+        if (st == M2S_OK) st = hc.launch(c);
+        if (st == M2S_OK) st = hc.downloads(false);  // whatever is ready
+    }
+    if (st == M2S_OK) st = hc.drain();
+    if (st != M2S_OK) return hc.fail(st);
     m2s_result r;
     std::memset(&r, 0, sizeof(r));
-    const uint64_t cap = effective_cap(ds, p, out_capacity);
-    auto fail_with = [&](m2s_status code) {
-        cudaStreamSynchronize(ctx->stream3); cudaStreamSynchronize(ctx->stream4); cudaStreamSynchronize(ctx->stream5);
-        cudaStreamSynchronize(ctx->stream); cudaStreamSynchronize(ctx->stream2);
-        ctx->dirty = true; ctx->vr_dirty = true;
-        m2s_scene_free(ctx, ds);
-        return code;
-    };
-    auto bail = [&](const char* what, cudaError_t e) {
-        set_error(std::string(what) + ": " + cudaGetErrorString(e));
-        return fail_with(M2S_E_CUDA);
-    };
-    static const bool host_trace = std::getenv("M2S_HOST_TRACE") != nullptr;  // debug: phase times on stderr
-    const auto t_start = std::chrono::steady_clock::now();
-    auto since = [&]() { return std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t_start).count(); };
-    cudaError_t e = cudaEventRecord(ctx->ev0, ctx->stream);
-    if (e != cudaSuccess) return bail("convert_host", e);
-    // uploads run on their own stream (behind the allocations and table copies made above on the context stream): the
-    // copy engine streams triangles and texture rows continuously while the chunks' kernels run on the context stream
-    e = cudaEventRecord(ctx->ev_alloc, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamWaitEvent(ctx->stream3, ctx->ev_alloc, 0);
-    if (e == cudaSuccess) e = cudaStreamWaitEvent(ctx->stream4, ctx->ev_alloc, 0);
-    if (e == cudaSuccess) e = cudaStreamWaitEvent(ctx->stream5, ctx->ev_alloc, 0);
-    if (e != cudaSuccess) return bail("convert_host", e);
-    // triangles on one copy stream, texture rows on another (two copy engines), the v-range
-    // reductions on a third, the mip rows on the compute stream: no copy ever queues behind a kernel
-    struct UpGuard { m2s_ctx* c; ~UpGuard() { c->up = c->tex_up = c->mip = c->aux = c->stream; } } up_guard{ctx};
-    ctx->up = ctx->stream3; ctx->tex_up = ctx->stream4; ctx->aux = ctx->stream5; ctx->mip = ctx->stream;
-    uint64_t lo_[m2s_ctx::kMaxChunks], hi_[m2s_ctx::kMaxChunks];
-    int planned = 0, uploaded = 0;
-    for (int c = 0; c < nchunks; ++c) {
-        const uint64_t lo = first + (uint64_t)c * per, hi = std::min(first + count, lo + per);
-        if (lo >= hi && c > 0) break;
-        lo_[c] = lo; hi_[c] = hi;
-        ++planned;
-    }
-    // (1) triangle chunk c goes up (its own copy stream), followed by the reduction of its v-range per texture (a kernel behind
-    // "chunk c is resident" on the aux stream, results through mapped memory)
-    auto upload_tris = [&](int c) -> m2s_status {
-        cudaError_t e1 = cudaSuccess;
-        if (hi_[c] > lo_[c]) {
-            e1 = cudaMemcpyAsync(reinterpret_cast<unsigned char*>(ds->d_tris) + lo_[c] * (size_t)kTriBytes,
-                                 reinterpret_cast<const unsigned char*>(sc->triangles) + lo_[c] * (size_t)kTriBytes,
-                                 (hi_[c] - lo_[c]) * (size_t)kTriBytes, cudaMemcpyHostToDevice, ctx->up);
-            ds->h2d_bytes += (hi_[c] - lo_[c]) * (uint64_t)kTriBytes;
-        }
-        if (e1 == cudaSuccess) e1 = cudaEventRecord(ctx->ev_tri[c], ctx->up);
-        if (e1 == cudaSuccess) e1 = cudaStreamWaitEvent(ctx->aux, ctx->ev_tri[c], 0);
-        if (e1 != cudaSuccess) { set_error(std::string("convert_host upload: ") + cudaGetErrorString(e1)); return M2S_E_CUDA; }
-        return vrange_enqueue(ctx, ds, lo_[c], hi_[c], c);
-    };
-    // look-ahead: triangle chunks (and their v-range reductions) queued ahead of the chunk whose texture rows go up: the
-    // first records exist after ~lookahead/nchunks of the triangles and 1/nchunks of the texture rows (the downloads of the
-    // records are the longest leg of the call: they must start early; queueing every triangle chunk up front delays them)
-    int lookahead = 2;
-    if (const char* e = std::getenv("M2S_HOST_LOOKAHEAD")) lookahead = std::max(1, std::atoi(e));
-    for (; uploaded < std::min(planned, lookahead); ++uploaded) {
-        st = upload_tris(uploaded);
-        if (st != M2S_OK) return fail_with(st);
-    }
-    unsigned long long tags[m2s_ctx::kMaxChunks] = {};
-    uint64_t base = 0, written = 0;
-    int next_dl = 0;
-    // enqueue the downloads of the chunks whose counts have arrived (in order); block: wait for them
-    auto downloads = [&](int upto, bool block) -> cudaError_t {
-        while (next_dl < upto) {
-            const int c = next_dl;
-            volatile unsigned long long* slot = ctx->h_chunk_tot + 2 * c;
-            for (;;) {
-                if (__atomic_load_n(&ctx->h_chunk_tot[2 * c + 1], __ATOMIC_ACQUIRE) == tags[c]) break;  // count is ordered before the tag
-                if (!block) return cudaSuccess;
-                const cudaError_t q = cudaEventQuery(ctx->ev_chunk[c]);
-                if (q == cudaSuccess) break;             // finished: the tag is there
-                if (q != cudaErrorNotReady) return q;
-            }
-            if (__atomic_load_n(&ctx->h_chunk_tot[2 * c + 1], __ATOMIC_ACQUIRE) != tags[c]) return cudaErrorUnknown;
-            const uint64_t tot = slot[0];
-            if (host_trace) std::fprintf(stderr, "[m2s host] chunk %d rasterised at %.0f us (%llu records)\n", c, since(), (unsigned long long)tot);
-            const uint64_t room = cap > base ? cap - base : 0, w = std::min(tot, room);
-            if (w) {
-                cudaError_t e2 = cudaStreamWaitEvent(ctx->stream2, ctx->ev_chunk[c], 0);
-                if (e2 == cudaSuccess)
-                    e2 = cudaMemcpyAsync(reinterpret_cast<unsigned char*>(h_out) + base * stride,
-                                         reinterpret_cast<const unsigned char*>(ctx->out.p) + base * stride, w * stride,
-                                         cudaMemcpyDeviceToHost, ctx->stream2);
-                if (e2 == cudaSuccess && h_keys)
-                    e2 = cudaMemcpyAsync(h_keys + base, d_keys + base, w * 8, cudaMemcpyDeviceToHost, ctx->stream2);
-                if (e2 != cudaSuccess) return e2;
-            }
-            base += tot;
-            written += w;
-            ++next_dl;
-        }
-        return cudaSuccess;
-    };
-    int launched = 0;
-    for (int c = 0; c < planned; ++c) {  // (2)
-        std::vector<MipRun> runs;
-        const double t_it0 = host_trace ? since() : 0.0;
-        st = upload_groups_from_vrange(ctx, ds, c, [&] { return downloads(launched, false); }, &runs);  // (3) while waiting: whatever is ready
-        if (st != M2S_OK) return fail_with(st);
-        const double t_it1 = host_trace ? since() : 0.0;
-        e = cudaEventRecord(ctx->ev_up[c], ctx->tex_up);   // chunk c's texture rows are resident (level 0)
-        if (e == cudaSuccess) e = cudaStreamWaitEvent(ctx->stream, ctx->ev_up[c], 0);
-        if (e == cudaSuccess) e = cudaStreamWaitEvent(ctx->stream, ctx->ev_tri[c], 0);
-        if (e != cudaSuccess) return bail("convert_host", e);
-        for (const MipRun& r : runs) {   // their mip rows: on the compute stream, right before the kernels that sample them
-            e = mip_groups_launch(ds->d_arena, ds->h_texs[r.t], r.g0, r.g1, ctx->stream);
-            if (e != cudaSuccess) return bail("convert_host mips", e);
-        }
-        if (uploaded < planned) {  // the next look-ahead chunk
-            st = upload_tris(uploaded++);
-            if (st != M2S_OK) return fail_with(st);
-        }
-        m2s_params pc = *p;
-        pc.first_triangle = lo_[c];
-        pc.triangle_count = hi_[c] - lo_[c];
-        unsigned long long* h_dev = nullptr;  // device view of the mapped count slot
-        e = cudaHostGetDevicePointer((void**)&h_dev, ctx->h_chunk_tot + 2 * c, 0);
-        if (e != cudaSuccess) return bail("convert_host", e);
-        tags[c] = ++ctx->host_seq;
-        if (hi_[c] > lo_[c]) {
-            st = convert_enqueue_impl(ctx, ds, &pc, ctx->out.p, out_capacity, h_keys ? (uint64_t*)d_keys : nullptr,
-                                      (uint64_t*)(ctx->d_chunk_tot + c), ctx->stream, nullptr, ctx->d_chunk_tot, (uint32_t)c,
-                                      h_dev, tags[c]);
-            if (st != M2S_OK) return fail_with(st);
-        } else {  // empty range: nothing to launch, the count is zero
-            e = cudaMemsetAsync(ctx->d_chunk_tot + c, 0, sizeof(unsigned long long), ctx->stream);
-            if (e != cudaSuccess) return bail("convert_host", e);
-            ctx->h_chunk_tot[2 * c] = 0;
-            __atomic_store_n(&ctx->h_chunk_tot[2 * c + 1], tags[c], __ATOMIC_RELEASE);
-        }
-        e = cudaEventRecord(ctx->ev_chunk[c], ctx->stream);
-        if (e != cudaSuccess) return bail("convert_host", e);
-        ++launched;
-        const double t_it2 = host_trace ? since() : 0.0;
-        e = downloads(launched, false);  // (3) whatever is ready
-        if (e != cudaSuccess) return bail("convert_host download", e);
-        if (host_trace) std::fprintf(stderr, "[m2s host] chunk %d: v-range wait + rows enqueued %.0f us, tris/mips/kernels enqueued %.0f us, downloads %.0f us (at %.0f us)\n",
-                                     c, t_it1 - t_it0, t_it2 - t_it1, since() - t_it2, since());
-    }
-    e = cudaEventRecord(ctx->ev1, ctx->stream);
-    if (e != cudaSuccess) return bail("convert_host", e);
-    if (host_trace) std::fprintf(stderr, "[m2s host] enqueued %d chunks at %.0f us\n", launched, since());
-    e = downloads(launched, true);
-    if (e != cudaSuccess) return bail("convert_host download", e);
-    e = cudaStreamSynchronize(ctx->stream2);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream3);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream4);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream5);
-    if (e != cudaSuccess) return bail("convert_host download", e);
-    if (host_trace) std::fprintf(stderr, "[m2s host] downloads done at %.0f us\n", since());
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
-    r.total = base; r.cap = cap; r.written = written; r.device_ms = ms;
-    st = base > cap ? capacity_error(base, cap) : M2S_OK;
+    cudaEventElapsedTime(&r.device_ms, ctx->ev0, ctx->ev1);
+    r.total = hc.base; r.cap = hc.cap; r.written = hc.written;
     if (res) *res = r;
-    m2s_scene_free(ctx, ds);
-    return st;
+    m2s_scene_free(ctx, hc.ds);
+    return hc.base > hc.cap ? capacity_error(hc.base, hc.cap) : M2S_OK;
 }
 
 // ---- scene -> .ply file: rows encoded on the GPU, streamed to disk through two pinned buffers -------------
@@ -482,10 +515,10 @@ m2s_status m2s::convert_scene_to_ply(m2s_ctx* ctx, const m2s_scene* sc, const m2
         if (b < nblocks) {  // start the download of block b ...
             e = cudaMemcpyAsync(ctx->h_stage[b & 1], reinterpret_cast<const unsigned char*>(ctx->out.p) + b * rows_per_block * stride,
                                 block_bytes(b), cudaMemcpyDeviceToHost, ctx->stream);
-            if (e == cudaSuccess) e = cudaEventRecord(ctx->ev_chunk[b & 1], ctx->stream);
+            if (e == cudaSuccess) e = cudaEventRecord(ctx->ev_stage[b & 1], ctx->stream);
         }
         if (b > 0 && e == cudaSuccess) {  // ... and write block b-1 while it crosses PCIe
-            e = cudaEventSynchronize(ctx->ev_chunk[(b - 1) & 1]);
+            e = cudaEventSynchronize(ctx->ev_stage[(b - 1) & 1]);
             if (e == cudaSuccess) ok = std::fwrite(ctx->h_stage[(b - 1) & 1], 1, block_bytes(b - 1), f) == block_bytes(b - 1);
         }
     }

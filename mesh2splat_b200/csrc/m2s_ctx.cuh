@@ -40,6 +40,31 @@ struct VRangeSlot {        // v-range reduction of one pipeline chunk: device bu
     cudaEvent_t ev = nullptr;    // recorded behind the publish kernel (error path: a failed launch never writes the tag)
 };
 
+// The per-context state of the host pipeline (m2s_convert_host, m2s_convert.cu): its streams, its per-chunk events and
+// counts, and the v-range slots (also used by m2s_scene_upload_range).  The pipeline keeps TWO copy engines busy in the
+// upload direction (two streams deliver more than one: scripts/pcie_probe.py measures it) and never puts a kernel
+// between two copies of a stream (a copy behind a kernel of its own stream waits for it: with the v-range and mip
+// kernels on the copy stream every chunk cost ~40 us of bubbles).  The kernels run on the context's stream.
+struct HostPipeline {
+    static constexpr int kMaxChunks = 4;         // the chunk plan's bound
+    cudaStream_t tri_stream = nullptr;           // triangle chunks
+    cudaStream_t tex_stream = nullptr;           // texture rows
+    cudaStream_t vr_stream = nullptr;            // v-range reductions and their 8-byte results
+    cudaStream_t dl_stream = nullptr;            // record downloads
+    cudaEvent_t ev_alloc = nullptr;              // "the allocations and table copies on the context's stream are done"
+    cudaEvent_t ev_tri[kMaxChunks] = {};         // "chunk c's triangles are resident"
+    cudaEvent_t ev_up[kMaxChunks] = {};          // "chunk c's texture rows are resident"
+    cudaEvent_t ev_chunk[kMaxChunks] = {};       // "chunk c's kernels are done"
+    unsigned long long* d_chunk_tot = nullptr;   // [kMaxChunks]
+    unsigned long long* h_chunk_tot = nullptr;   // pinned + mapped: {count, tag} per chunk, written by the raster kernel
+    unsigned long long host_seq = 0;             // tag generator
+    VRangeSlot vr[kMaxChunks];                   // v-range reductions (lazy texture upload)
+    uint32_t vr_ntex = 0;                        // textures the slots are sized for
+    bool vr_dirty = false;                       // a pipeline was abandoned half way: the device copies must be re-armed
+    m2s_status create();
+    void release();                              // also after a create() that failed half way
+};
+
 }  // namespace m2s
 
 struct m2s_ctx {
@@ -55,32 +80,12 @@ struct m2s_ctx {
     uint32_t* h_status = nullptr;            // pinned + mapped: raised by device-side waits that timed out (fused gather)
     uint32_t* d_status = nullptr;            // its device view
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev_mid = nullptr;
-    // convert_host pipeline: a second stream for the downloads, per-chunk counts and events
-    static constexpr int kMaxChunks = 8;
-    cudaStream_t stream2 = nullptr;
-    cudaStream_t stream3 = nullptr;              // uploads of the host pipeline: the copy engine keeps going while chunk kernels run
-    cudaStream_t up = nullptr;                   // stream triangle chunks are uploaded on (= stream, or stream3 inside the pipeline)
-    // the host pipeline keeps TWO copy engines busy in the upload direction (two streams deliver more than one:
-    // scripts/pcie_probe.py measures it) and never puts a kernel between two copies of a stream (a copy behind a kernel of
-    // its own stream waits for it: with the v-range and mip kernels on the copy stream every chunk cost ~40 us of bubbles)
-    cudaStream_t stream4 = nullptr;              // texture rows
-    cudaStream_t stream5 = nullptr;              // v-range reductions and their 8-byte results
-    cudaStream_t tex_up = nullptr;               // stream texture rows are uploaded on (= up, or stream4 inside the pipeline)
-    cudaStream_t mip = nullptr;                  // stream their mip rows are generated on (= tex_up, or the compute stream inside the pipeline)
-    cudaStream_t aux = nullptr;                  // stream the v-range reductions run on (= up, or stream5 inside the pipeline)
-    cudaEvent_t ev_tri[kMaxChunks] = {};         // "chunk c's triangles are resident"
-    cudaEvent_t ev_up[kMaxChunks] = {};          // "chunk c's texture rows are resident"
-    cudaEvent_t ev_alloc = nullptr;
-    unsigned long long* d_chunk_tot = nullptr;   // [kMaxChunks]
-    unsigned long long* h_chunk_tot = nullptr;   // pinned + mapped: {count, tag} per chunk, written by the raster kernel
-    unsigned long long host_seq = 0;             // tag generator
-    // file writer: two pinned staging buffers (download of block i overlaps the write of block i-1)
+    m2s::HostPipeline pipeline;              // m2s_convert_host
+    // .ply writer and reader: two pinned staging buffers (the copy of block i overlaps the file access of block i-1), and
+    // the events that say when each is free again
     static constexpr size_t kStageBytes = 32u << 20;
     unsigned char* h_stage[2] = {nullptr, nullptr};
-    cudaEvent_t ev_chunk[kMaxChunks] = {};
-    m2s::VRangeSlot vr[kMaxChunks];          // v-range reductions of the host pipeline (lazy texture upload)
-    uint32_t vr_ntex = 0;                    // textures the slots are sized for
-    bool vr_dirty = false;                   // a pipeline was abandoned half way: the device copies must be re-armed
+    cudaEvent_t ev_stage[2] = {};
     static constexpr int kLayouts = 5;
     int blocks_per_sm[kLayouts] = {};       // raster kernel (persistent)
     int frag_blocks_per_sm[kLayouts] = {};  // fragment kernel
@@ -170,11 +175,11 @@ struct MipRun { uint32_t t, g0, g1; };   // levels 1.. of the row groups [g0, g1
 // m2s_scene_upload_range uploads what one shard needs).
 m2s_status scene_upload_impl(m2s_ctx* ctx, const m2s_scene* sc, m2s_dscene** out, uint64_t first_tris, bool sync,
                              uint64_t tri_offset = 0, bool lazy_tex = false);
-// enqueue on ctx->aux: reduce the v-range of triangles [lo, hi) (already on the device) per texture, copy it to the
+// enqueue on `stream`: reduce the v-range of triangles [lo, hi) (already on the device) per texture, copy it to the
 // slot's pinned buffer, record the slot's event
-m2s_status vrange_enqueue(m2s_ctx* ctx, m2s_dscene* d, uint64_t lo, uint64_t hi, int slot);
-// rows [g0, g1) x kTexGroupRows of texture t go up; their mip rows are generated, or appended to *deferred
-m2s_status upload_texture_groups(m2s_ctx* ctx, m2s_dscene* d, uint32_t t, uint32_t g0, uint32_t g1, std::vector<MipRun>* deferred = nullptr);
+m2s_status vrange_enqueue(m2s_ctx* ctx, m2s_dscene* d, cudaStream_t stream, uint64_t lo, uint64_t hi, int slot);
+// rows [g0, g1) x kTexGroupRows of texture t go up on `stream`; their mip rows are generated there, or appended to *deferred
+m2s_status upload_texture_groups(m2s_dscene* d, cudaStream_t stream, uint32_t t, uint32_t g0, uint32_t g1, std::vector<MipRun>* deferred = nullptr);
 
 // Which texture rows can the triangles [lo, hi) sample?  The v-range per texture is reduced ON THE GPU from the triangles
 // already uploaded (vrange_kernel, m2s_scene.cu: the host would have to stream the same 144 B/triangle through one core — ~1 ms for
@@ -182,23 +187,25 @@ m2s_status upload_texture_groups(m2s_ctx* ctx, m2s_dscene* d, uint32_t t, uint32
 // footprints of all five mip levels (level l reaches 2^(l+1) level-0 rows beyond the sample point, plus the drift of
 // non-power-of-two chains) and the REPEAT wrap at both ends; a range whose v spans a whole period (or is not finite)
 // takes the whole image.
-// `idle` (optional) is called while the host waits for the reduction: the host pipeline enqueues ready downloads there
+// `idle` is called while the host waits for the reduction (the host pipeline enqueues ready downloads there); a status
+// other than M2S_OK ends the wait and is returned.  The rows go up on `stream`.
 inline float sortable_to_float(int i) { i ^= (i >> 31) & 0x7fffffff; float f; std::memcpy(&f, &i, 4); return f; }
 template <class Idle>
-m2s_status upload_groups_from_vrange(m2s_ctx* ctx, m2s_dscene* d, int slot, Idle idle, std::vector<MipRun>* deferred = nullptr) {
+m2s_status upload_groups_from_vrange(m2s_ctx* ctx, m2s_dscene* d, cudaStream_t stream, int slot, Idle idle, std::vector<MipRun>* deferred = nullptr) {
     const uint32_t nt = d->ntex;
     if (!nt) return M2S_OK;
+    const VRangeSlot& v = ctx->pipeline.vr[slot];
     for (uint32_t spin = 0;; ++spin) {
-        if (__atomic_load_n(ctx->vr[slot].h_tag, __ATOMIC_ACQUIRE) == ctx->vr[slot].tag) break;   // the values are ordered before the tag
+        if (__atomic_load_n(v.h_tag, __ATOMIC_ACQUIRE) == v.tag) break;   // the values are ordered before the tag
         if ((spin & 255u) == 255u) {  // a failed launch never writes the tag: ask the stream now and then
-            const cudaError_t q = cudaEventQuery(ctx->vr[slot].ev);
-            if (q == cudaSuccess) { if (__atomic_load_n(ctx->vr[slot].h_tag, __ATOMIC_ACQUIRE) == ctx->vr[slot].tag) break; }
+            const cudaError_t q = cudaEventQuery(v.ev);
+            if (q == cudaSuccess) { if (__atomic_load_n(v.h_tag, __ATOMIC_ACQUIRE) == v.tag) break; }
             else if (q != cudaErrorNotReady) { set_error(std::string("v-range reduction: ") + cudaGetErrorString(q)); return M2S_E_CUDA; }
         }
-        const cudaError_t ie = idle();
-        if (ie != cudaSuccess) { set_error(std::string("convert_host download: ") + cudaGetErrorString(ie)); return M2S_E_CUDA; }
+        const m2s_status ist = idle();
+        if (ist != M2S_OK) return ist;
     }
-    const int* mm = ctx->vr[slot].h_minmax;
+    const int* mm = v.h_minmax;
     const bool finite = mm[2 * nt] == 0;
     for (uint32_t t = 0; t < nt; ++t) {
         if (mm[t] > mm[nt + t]) continue;  // no triangle of the range samples this texture
@@ -218,7 +225,7 @@ m2s_status upload_groups_from_vrange(m2s_ctx* ctx, m2s_dscene* d, int slot, Idle
             if (!need[g] || d->present[t][g]) { ++g; continue; }
             uint32_t e = g;
             while (e < ng && need[e] && !d->present[t][e]) ++e;
-            m2s_status st = upload_texture_groups(ctx, d, t, g, e, deferred);
+            m2s_status st = upload_texture_groups(d, stream, t, g, e, deferred);
             if (st != M2S_OK) return st;
             g = e;
         }

@@ -426,7 +426,7 @@ M2S_EXPORT m2s_status m2s_ply_read_sh(m2s_ctx* ctx, const char* path, void* d_re
         const int slot = (int)(b & 1);
         const uint64_t first = b * rows_per_block, rows = std::min(rows_per_block, n - first);
         const size_t bytes = (size_t)rows * stride;
-        if (b >= 2) e = cudaEventSynchronize(ctx->ev_chunk[slot]);
+        if (b >= 2) e = cudaEventSynchronize(ctx->ev_stage[slot]);
         if (e != cudaSuccess) break;
         if (std::fread(ctx->h_stage[slot], 1, bytes, f) != bytes) {
             set_error(std::string("m2s_ply_read: short read of ") + path);
@@ -438,7 +438,7 @@ M2S_EXPORT m2s_status m2s_ply_read_sh(m2s_ctx* ctx, const char* path, void* d_re
         if (e == cudaSuccess)
             e = ply_decode_launch(info, d, rows, static_cast<unsigned char*>(d_ref96) + first * 96, sh_floats ? d_sh + first * sh_floats : nullptr,
                                   ctx->stream);
-        if (e == cudaSuccess) e = cudaEventRecord(ctx->ev_chunk[slot], ctx->stream);
+        if (e == cudaSuccess) e = cudaEventRecord(ctx->ev_stage[slot], ctx->stream);
         if (e == cudaSuccess) ctx->ply_h2d += bytes;
     }
     const cudaError_t es = cudaStreamSynchronize(ctx->stream);   // the pinned buffers are idle before the call returns

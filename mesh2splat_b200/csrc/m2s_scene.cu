@@ -163,33 +163,34 @@ M2S_EXPORT void m2s_scene_free(m2s_ctx* ctx, m2s_dscene* s) {
 }
 
 // one contiguous H2D copy, then the rows of levels 1.. that they determine
-m2s_status m2s::upload_texture_groups(m2s_ctx* ctx, m2s_dscene* d, uint32_t t, uint32_t g0, uint32_t g1, std::vector<MipRun>* deferred) {
+m2s_status m2s::upload_texture_groups(m2s_dscene* d, cudaStream_t stream, uint32_t t, uint32_t g0, uint32_t g1, std::vector<MipRun>* deferred) {
     const DTexture& dt = d->h_texs[t];
     const uint32_t H = dt.h[0], W = dt.w[0];
     const uint32_t r0 = g0 * kTexGroupRows, r1 = std::min<uint32_t>(H, g1 * kTexGroupRows);
     if (r0 >= r1) return M2S_OK;
     CUDA_TRY(cudaMemcpyAsync(d->d_arena + dt.off[0] + (size_t)r0 * W, d->h_rgba[t] + (size_t)r0 * W * 4, (size_t)(r1 - r0) * W * 4,
-                             cudaMemcpyHostToDevice, ctx->tex_up));
+                             cudaMemcpyHostToDevice, stream));
     // level-l row j needs level-(l-1) rows 2j, 2j+1: inside the same 16-row group — all levels in one launch; inside the
     // host pipeline the launch is left to the caller (on the compute stream, behind an event: no kernel on the copy stream)
     const uint32_t ge = std::min<uint32_t>(g1, (H + kTexGroupRows - 1) / kTexGroupRows);
     if (deferred) deferred->push_back({t, g0, ge});
-    else CUDA_TRY(mip_groups_launch(d->d_arena, dt, g0, ge, ctx->tex_up));
+    else CUDA_TRY(mip_groups_launch(d->d_arena, dt, g0, ge, stream));
     for (uint32_t g = g0; g < g1 && g < d->present[t].size(); ++g) d->present[t][g] = 1;
     d->h2d_bytes += (uint64_t)(r1 - r0) * W * 4;
     return M2S_OK;
 }
 
-m2s_status m2s::vrange_enqueue(m2s_ctx* ctx, m2s_dscene* d, uint64_t lo, uint64_t hi, int slot) {
+m2s_status m2s::vrange_enqueue(m2s_ctx* ctx, m2s_dscene* d, cudaStream_t stream, uint64_t lo, uint64_t hi, int slot) {
     const uint32_t nt = d->ntex;
     if (!nt) return M2S_OK;
-    if (ctx->vr_ntex != nt) {  // (re)size and arm every slot: the armed layout (min block | max block | flag) depends on the texture count
-        for (auto& v : ctx->vr) {
+    HostPipeline& hp = ctx->pipeline;
+    if (hp.vr_ntex != nt) {  // (re)size and arm every slot: the armed layout (min block | max block | flag) depends on the texture count
+        for (auto& v : hp.vr) {
             if (v.d_minmax) { cudaFree(v.d_minmax); v.d_minmax = nullptr; }
             if (v.h_minmax) { cudaFreeHost(v.h_minmax); v.h_minmax = nullptr; }
         }
-        ctx->vr_ntex = 0;
-        for (auto& v : ctx->vr) {
+        hp.vr_ntex = 0;
+        for (auto& v : hp.vr) {
             const size_t nints = 2 * (size_t)nt + 1, tag_off = (nints * sizeof(int) + 7) & ~(size_t)7;
             CUDA_TRY(cudaMalloc(&v.d_minmax, nints * sizeof(int)));
             std::vector<int> arm(nints, 0);
@@ -202,28 +203,28 @@ m2s_status m2s::vrange_enqueue(m2s_ctx* ctx, m2s_dscene* d, uint64_t lo, uint64_
             v.h_tag_dev = reinterpret_cast<unsigned long long*>(reinterpret_cast<unsigned char*>(v.h_minmax_dev) + tag_off);
             if (!v.ev) CUDA_TRY(cudaEventCreateWithFlags(&v.ev, cudaEventDisableTiming));
         }
-        ctx->vr_ntex = nt;
+        hp.vr_ntex = nt;
     }
-    VRangeSlot& v = ctx->vr[slot];
+    VRangeSlot& v = hp.vr[slot];
     // min <- 0x7f7f7f7f (above every finite float's key), max <- 0x80808080 (below), flag <- 0
     // d_minmax is armed (at allocation, then by every publish kernel); a conversion that failed in between re-arms it
-    if (ctx->vr_dirty) {
-        for (auto& w : ctx->vr) {
-            CUDA_TRY(cudaMemsetAsync(w.d_minmax, 0x7f, nt * sizeof(int), ctx->aux));
-            CUDA_TRY(cudaMemsetAsync(w.d_minmax + nt, 0x80, nt * sizeof(int), ctx->aux));
-            CUDA_TRY(cudaMemsetAsync(w.d_minmax + 2 * nt, 0, sizeof(int), ctx->aux));
+    if (hp.vr_dirty) {
+        for (auto& w : hp.vr) {
+            CUDA_TRY(cudaMemsetAsync(w.d_minmax, 0x7f, nt * sizeof(int), stream));
+            CUDA_TRY(cudaMemsetAsync(w.d_minmax + nt, 0x80, nt * sizeof(int), stream));
+            CUDA_TRY(cudaMemsetAsync(w.d_minmax + 2 * nt, 0, sizeof(int), stream));
         }
-        ctx->vr_dirty = false;
+        hp.vr_dirty = false;
     }
     if (hi > lo) {
-        vrange_kernel<<<(uint32_t)(hi - lo + 255) / 256, 256, 0, ctx->aux>>>(d->d_tris, (uint32_t)lo, (uint32_t)(hi - lo), d->d_ranges,
-                                                                           d->nranges, d->d_prims, nt, v.d_minmax);
+        vrange_kernel<<<(uint32_t)(hi - lo + 255) / 256, 256, 0, stream>>>(d->d_tris, (uint32_t)lo, (uint32_t)(hi - lo), d->d_ranges,
+                                                                        d->nranges, d->d_prims, nt, v.d_minmax);
         CUDA_TRY(cudaGetLastError());
     }
-    v.tag = ++ctx->host_seq;
-    vrange_publish_kernel<<<1, 128, 0, ctx->aux>>>(v.d_minmax, nt, v.h_minmax_dev, v.h_tag_dev, v.tag);
+    v.tag = ++hp.host_seq;
+    vrange_publish_kernel<<<1, 128, 0, stream>>>(v.d_minmax, nt, v.h_minmax_dev, v.h_tag_dev, v.tag);
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaEventRecord(v.ev, ctx->aux));
+    CUDA_TRY(cudaEventRecord(v.ev, stream));
     return M2S_OK;
 }
 
@@ -325,7 +326,7 @@ m2s_status m2s::scene_upload_impl(m2s_ctx* ctx, const m2s_scene* sc, m2s_dscene*
         d->h_rgba[t] = sc->textures[t].rgba;
         d->present[t].assign(ngroups, 0);
         if (!lazy_tex) {
-            m2s_status st = upload_texture_groups(ctx, d, t, 0, ngroups);
+            m2s_status st = upload_texture_groups(d, ctx->stream, t, 0, ngroups);
             if (st != M2S_OK) return fail(st);
         }
     }
@@ -369,8 +370,8 @@ M2S_EXPORT m2s_status m2s_scene_upload_range(m2s_ctx* ctx, const m2s_scene* sc, 
     m2s_dscene* ds = nullptr;
     m2s_status st = scene_upload_impl(ctx, &slim.scene, &ds, r.count, false, r.first, true);
     if (st != M2S_OK) return st;
-    st = vrange_enqueue(ctx, ds, r.first, r.first + r.count, 0);
-    if (st == M2S_OK) st = upload_groups_from_vrange(ctx, ds, 0, [] { return cudaSuccess; });
+    st = vrange_enqueue(ctx, ds, ctx->stream, r.first, r.first + r.count, 0);
+    if (st == M2S_OK) st = upload_groups_from_vrange(ctx, ds, ctx->stream, 0, [] { return M2S_OK; });
     cudaError_t e = cudaStreamSynchronize(ctx->stream);
     if (st == M2S_OK && e != cudaSuccess) { set_error(std::string("m2s_scene_upload_range: ") + cudaGetErrorString(e)); st = M2S_E_CUDA; }
     if (st != M2S_OK) { m2s_scene_free(ctx, ds); return st; }

@@ -1,5 +1,4 @@
-"""m2s_convert_host on the bench scene (pinned buffers), a few repetitions; prints the mean time.  With M2S_HOST_TRACE=1 the
-library prints its phase times; M2S_HOST_CHUNKS=n sets the pipeline depth."""
+"""m2s_convert_host on the bench scene (pinned buffers), a few repetitions; prints the mean time."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -17,7 +16,6 @@ h = torch.empty(cap * stride, dtype=torch.uint8).pin_memory().numpy()
 for _ in range(3):
     ctx.convert_host(ps, 512, layout, flags=_abi.FLAG_UNCAPPED, capacity=cap, out=h, c_scene=cs)
 torch.cuda.synchronize()
-os.environ.pop("M2S_HOST_TRACE", None)
 t0 = time.perf_counter()
 n = 10
 for _ in range(n):

@@ -1,5 +1,5 @@
-"""PCIe probe: H2D and D2H alone and concurrently (pinned memory, two streams), and the phase times of
-m2s_convert_host (M2S_HOST_TRACE=1).  Explains the e2e number of bench.py."""
+"""PCIe probe: H2D and D2H alone and concurrently (pinned memory, two streams), and with the argument `host` the
+per-call times of m2s_convert_host.  Explains the e2e number of bench.py."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -66,7 +66,6 @@ except Exception as e:  # noqa: BLE001
     print("write-combined probe unavailable:", e)
 
 if len(sys.argv) > 1 and sys.argv[1] == "host":
-    os.environ["M2S_HOST_TRACE"] = "1"
     import numpy as np
     from mesh2splat_b200 import synth, _abi
     from mesh2splat_b200.api import Context
