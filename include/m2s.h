@@ -654,6 +654,47 @@ m2s_status m2s_image_compare(m2s_ctx* ctx, const uint8_t* d_a, const uint8_t* d_
                              const uint8_t* d_cover_b, const m2s_compare_params* params, m2s_compare_result* h_result,
                              float* d_ssim_map);
 
+/* ---- the standard 3DGS render (beyond the reference) ------------------------------------------------------------------
+ * The picture a graphdeco-style rasteriser (Kerbl et al. 2023, diff-gaussian-rasterization's forward pass, which SIBR,
+ * gsplat and most viewers copy) makes of converted or loaded gaussians, for the project's GL camera: per gaussian the
+ * 3-D covariance from scale and normalised rotation, the EWA projection with +0.3 on the diagonal, the conic, a 3-sigma
+ * radius and its 16 x 16 tile rectangle; per pixel the gaussians of its tile front to back in (view depth, record index)
+ * order, alpha = min(0.99, opacity exp(power)), skipped below 1/255, the pixel stopped before the gaussian that would
+ * take its transmittance T below 1e-4.  Colour C + T background, alpha 1 - T.  DESIGN §2 fixes every fp32 operation
+ * (no contraction, exp = the project's rn_exp), so the image is deterministic.  Row 0 is the bottom row.
+ * Records: M2S_LAYOUT_REF96 (scale * std_dev), M2S_LAYOUT_PACKED56, M2S_VIEW_PLY or M2S_VIEW_PLY_PBR (scale as stored);
+ * colour max(colour + SH rest, 0) per channel, the rest as m2s_prepass_sh evaluates it (VIEW_PLY* with d_sh only). */
+typedef struct m2s_3dgs_params {
+    float world_to_view[16];   /* column-major, finite */
+    float view_to_clip[16];    /* finite; [0] and [5] > 0 (the focal lengths fx = P00 W / 2, fy = P11 H / 2) */
+    float model_to_world[16];  /* finite; world_to_view * model_to_world non-singular */
+    uint32_t width, height;    /* 1..4096 each */
+    float near;                /* > 0: a gaussian is culled unless its view depth d = -z > near (graphdeco: 0.2) */
+    float std_dev;             /* the REF96 scale multiplier (gaussianStd / resolutionTarget); unused by other layouts */
+    float scale_modifier;      /* every scale times this (graphdeco's scale_modifier, 1 by default) */
+    float background[3];       /* RGB behind the gaussians */
+    uint32_t layout;           /* M2S_LAYOUT_REF96, M2S_LAYOUT_PACKED56, M2S_VIEW_PLY or M2S_VIEW_PLY_PBR */
+    uint32_t reserved;
+} m2s_3dgs_params;
+/* Enqueue-only.  d_records: count records of the layout (16-byte aligned); d_count (optional, device): n = min(count,
+ * *d_count).  d_sh / buffer_degree / sh_degree as m2s_prepass_sh (VIEW_PLY* only; sh_degree 0 = no SH).  Targets, each
+ * optional but not both NULL, every pixel written once: d_rgba32f width x height x 4 floats (16-byte aligned), d_rgba8
+ * width x height x 4 bytes (4-byte aligned), unorm8 of each value (clamp to [0, 1], round-half-even(v 255)).
+ * max_pairs (< 2^30) is the budget of (16 x 16 tile, gaussian) pairs: when the survivors need more, the longest prefix in
+ * depth order (the nearest gaussians) whose pairs fit is drawn.  d_drawn (optional, device uint32) receives the prefix
+ * length, d_pairs (optional, device uint64) the pairs all survivors need.  count < 2^30.  M2S_E_INVALID before any launch,
+ * with nothing written, for a bad size or layout, no target, a misaligned pointer, SH arguments m2s_prepass_sh rejects,
+ * non-finite matrices, near <= 0, view_to_clip[0] or [5] <= 0, or a singular world_to_view * model_to_world.  Scratch is
+ * stream-ordered context memory grown on `stream` (NULL = context stream); nothing is synchronised. */
+m2s_status m2s_3dgs_render_enqueue(m2s_ctx* ctx, const void* d_records, uint64_t count, const uint64_t* d_count,
+                                   const m2s_3dgs_params* params, const float* d_sh, uint32_t buffer_degree, uint32_t sh_degree,
+                                   float* d_rgba32f, uint8_t* d_rgba8, uint64_t max_pairs, uint64_t* d_pairs, uint32_t* d_drawn,
+                                   void* stream);
+/* Synchronous form on the context stream: counts the pairs, reads the count back once, grows the scratch and draws every
+ * survivor.  *pairs (optional, host) receives the pair count. */
+m2s_status m2s_3dgs_render(m2s_ctx* ctx, const void* d_records, uint64_t count, const m2s_3dgs_params* params, const float* d_sh,
+                           uint32_t buffer_degree, uint32_t sh_degree, float* d_rgba32f, uint8_t* d_rgba8, uint64_t* pairs);
+
 #ifdef __cplusplus
 }
 #endif

@@ -185,6 +185,29 @@ def make_mesh_render_params(world_to_view, view_to_clip, model_to_world, width: 
     return p
 
 
+class m2s_3dgs_params(C.Structure):
+    """include/m2s.h: the camera, image and records of the standard 3DGS render; matrices column-major (glm::mat4)."""
+    _fields_ = [("world_to_view", C.c_float * 16), ("view_to_clip", C.c_float * 16), ("model_to_world", C.c_float * 16),
+                ("width", C.c_uint32), ("height", C.c_uint32), ("near", C.c_float), ("std_dev", C.c_float), ("scale_modifier", C.c_float),
+                ("background", C.c_float * 3), ("layout", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+GS3D_SPLAT_FLOATS = 12   # the preprocess kernel's splat record (m2s_debug_3dgs_preprocess): 48 B
+GS3D_CULLED = 0xFFFFFFFF  # the depth key of a culled record
+
+
+def make_3dgs_params(world_to_view, view_to_clip, model_to_world, width: int, height: int, near: float, std_dev: float,
+                     scale_modifier: float, background, layout: int):
+    p = m2s_3dgs_params()
+    for name, m in (("world_to_view", world_to_view), ("view_to_clip", view_to_clip), ("model_to_world", model_to_world)):
+        setattr(p, name, (C.c_float * 16)(*[float(v) for v in np.asarray(m, np.float32).ravel()]))
+    p.width, p.height = int(width), int(height)
+    p.near, p.std_dev, p.scale_modifier = float(near), float(std_dev), float(scale_modifier)
+    p.background = (C.c_float * 3)(*[float(v) for v in background])
+    p.layout, p.reserved = int(layout), 0
+    return p
+
+
 class m2s_compare_params(C.Structure):
     _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("cover_min", C.c_uint32)]
 

@@ -26,7 +26,7 @@ SYMBOLS = [
     "m2s_deferred_light_split", "m2s_deferred_light_split_enqueue",
     "m2s_ply_parse_header", "m2s_ply_decode_enqueue", "m2s_ply_read", "m2s_ply_h2d_bytes",
     "m2s_ply_decode_sh_enqueue", "m2s_ply_read_sh", "m2s_prepass_sh", "m2s_prepass_sh_enqueue",
-    "m2s_image_compare", "m2s_image_compare_enqueue",
+    "m2s_image_compare", "m2s_image_compare_enqueue", "m2s_3dgs_render", "m2s_3dgs_render_enqueue",
 ]
 
 
@@ -167,6 +167,10 @@ def lib() -> C.CDLL:
     L.m2s_image_compare_enqueue.argtypes = [vp, vp, vp, vp, vp, C.POINTER(_abi.m2s_compare_params), vp, vp, vp]
     L.m2s_image_compare.restype = i32
     L.m2s_image_compare.argtypes = [vp, vp, vp, vp, vp, C.POINTER(_abi.m2s_compare_params), C.POINTER(_abi.m2s_compare_result), vp]
+    L.m2s_3dgs_render_enqueue.restype = i32
+    L.m2s_3dgs_render_enqueue.argtypes = [vp, vp, u64, vp, C.POINTER(_abi.m2s_3dgs_params), vp, u32, u32, vp, vp, u64, vp, vp, vp]
+    L.m2s_3dgs_render.restype = i32
+    L.m2s_3dgs_render.argtypes = [vp, vp, u64, C.POINTER(_abi.m2s_3dgs_params), vp, u32, u32, vp, vp, C.POINTER(u64)]
     _lib = L
     return L
 

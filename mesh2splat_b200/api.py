@@ -461,6 +461,69 @@ class Context:
             check(lib().m2s_image_compare(*args, C.byref(r), ptr(ssim_map)))
         return _abi.compare_result_dict(r, width * height)
 
+    def render_3dgs(self, records, count: int, layout: int, world_to_view, view_to_clip, model_to_world, width: int, height: int,
+                    near: float = 0.2, std_dev: float = 1.0, scale_modifier: float = 1.0, background=(0.0, 0.0, 0.0), sh=None,
+                    sh_degree: int | None = None, targets=("rgba8", "rgba32f"), max_pairs: int | None = None, d_count=None,
+                    images=None):
+        """The standard 3DGS render (m2s_3dgs_render, graphdeco's forward pass) of device-resident records (a torch uint8
+        tensor, e.g. ConvertOutput.data or ply_read's): returns ({target: device tensor}, drawn, pairs).  "rgba8" is a uint8
+        tensor of width * height * 4 bytes (it feeds compare_images directly), "rgba32f" a float32 tensor of width * height
+        * 4 values; row 0 = the bottom row.  targets: the names to draw.  sh / sh_degree: a loaded .ply's SH rest
+        coefficients, as prepass (layouts VIEW_PLY and VIEW_PLY_PBR).  max_pairs None: m2s_3dgs_render (every survivor
+        drawn).  Otherwise m2s_3dgs_render_enqueue on torch's current stream with that pair budget and d_count (optional
+        uint64 device tensor) limiting n.  images: optional {target: caller-owned device tensor}."""
+        torch = _torch()
+        dev = records.device
+        images = dict(images or {})
+        for name, dt in (("rgba8", torch.uint8), ("rgba32f", torch.float32)):
+            if name in targets and name not in images:
+                images[name] = torch.empty(width * height * 4, dtype=dt, device=dev)
+        images = {k: v for k, v in images.items() if k in targets}
+        buffer_degree, sh_ptr = self._sh_buffer(sh, dev)
+        degree = buffer_degree if sh_degree is None else int(sh_degree)
+        p = _abi.make_3dgs_params(world_to_view, view_to_clip, model_to_world, width, height, near, std_dev, scale_modifier, background, layout)
+        ptr = lambda name: images[name].data_ptr() if name in images else None  # noqa: E731
+        drawn, npairs = _binned_pass(
+            dev, max_pairs, count,
+            lambda pairs: lib().m2s_3dgs_render(self.handle, records.data_ptr(), count, C.byref(p), sh_ptr, buffer_degree, degree,
+                                                ptr("rgba32f"), ptr("rgba8"), pairs),
+            lambda *budget: lib().m2s_3dgs_render_enqueue(self.handle, records.data_ptr(), count,
+                                                          d_count.data_ptr() if d_count is not None else None, C.byref(p), sh_ptr,
+                                                          buffer_degree, degree, ptr("rgba32f"), ptr("rgba8"), *budget))
+        return images, drawn, npairs
+
+    def gs3d_preprocess(self, records, count: int, layout: int, world_to_view, view_to_clip, model_to_world, width: int, height: int,
+                        near: float = 0.2, std_dev: float = 1.0, scale_modifier: float = 1.0, sh=None, sh_degree: int | None = None):
+        """The 3DGS render's preprocess kernel alone (m2s_debug_3dgs_preprocess, not in m2s.h): (splat records [count, 12]
+        float32, depth keys [count] uint32 (GS3D_CULLED for a culled record), survivors) as numpy values."""
+        torch = _torch()
+        dev = records.device
+        fn = lib().m2s_debug_3dgs_preprocess
+        fn.restype = C.c_int
+        fn.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(_abi.m2s_3dgs_params), C.c_void_p, C.c_uint32, C.c_uint32,
+                       C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32)]
+        splats = torch.empty(max(1, count) * _abi.GS3D_SPLAT_FLOATS, dtype=torch.float32, device=dev)
+        keys = torch.empty(max(1, count), dtype=torch.int32, device=dev)
+        buffer_degree, sh_ptr = self._sh_buffer(sh, dev)
+        p = _abi.make_3dgs_params(world_to_view, view_to_clip, model_to_world, width, height, near, std_dev, scale_modifier, (0, 0, 0), layout)
+        survivors = C.c_uint32(0)
+        torch.cuda.synchronize(dev)
+        check(fn(self.handle, records.data_ptr(), count, C.byref(p), sh_ptr, buffer_degree, buffer_degree if sh_degree is None else int(sh_degree),
+                 splats.data_ptr(), keys.data_ptr(), C.byref(survivors)))
+        return (splats[: count * _abi.GS3D_SPLAT_FLOATS].cpu().numpy().reshape(count, _abi.GS3D_SPLAT_FLOATS).copy(),
+                keys[:count].cpu().numpy().view(np.uint32).copy(), int(survivors.value))
+
+    @staticmethod
+    def _sh_buffer(sh, dev):
+        """(buffer degree, device pointer) of an SH tensor as ply_read_sh returns it, (0, None) for None."""
+        if sh is None:
+            return 0, None
+        torch = _torch()
+        degrees = {f: d for d, f in _abi.SH_FLOATS.items() if f}
+        if sh.dim() != 2 or sh.shape[1] not in degrees or sh.dtype != torch.float32 or sh.device != dev or not sh.is_contiguous():
+            raise ValueError("sh must be a contiguous (count, 12 | 24 | 48) float32 tensor on the records' device")
+        return degrees[sh.shape[1]], sh.data_ptr()
+
     def convert_timed(self, dscene: DeviceScene, params: _abi.m2s_params, out, capacity: int):
         """One conversion with an event between the two kernels (they do not overlap): (raster_ms, fragment_ms)."""
         a, b = C.c_float(0), C.c_float(0)

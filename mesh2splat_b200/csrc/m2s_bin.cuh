@@ -1,7 +1,8 @@
 // m2s_bin.cuh — the tile binning of the viewer's tiled rasterisers: the splat draw (m2s_splat.cu), the shadow pass's
-// cube raster (m2s_light.cu), the mesh depth pre-pass (m2s_depth.cu) and the mesh G-buffer pass (m2s_mesh.cu).  Each
-// pass bins its items (quads, light records, source triangles) into 16 x 16 tiles and then runs its own tile kernel
-// over each tile's run of pairs (bin_draw_launch, in the frame of tile_frame and tile_batches):
+// cube raster (m2s_light.cu), the mesh depth pre-pass (m2s_depth.cu) and the mesh G-buffer pass (m2s_mesh.cu), and of
+// the standard 3DGS render (m2s_3dgs.cu).  Each pass bins its items (quads, light records, source triangles, gaussians)
+// into 16 x 16 tiles and then runs its own tile kernel over each tile's run of pairs (bin_draw_launch, in the frame of
+// tile_frame and tile_batches):
 //   bin_count_kernel     per item: the number of its (tile, value) pairs, scanned within the block of kBinBlock items
 //   bin_scan_kernel      one CTA: exclusive prefix over the block sums; the total number of pairs
 //   bin_emit_kernel      per item of the longest prefix whose pairs fit the budget: its pairs at its scan offset, so the
@@ -20,6 +21,7 @@
 #include <algorithm>
 #include <cstddef>
 #include <cstdint>
+#include <type_traits>
 #include <cuda_runtime.h>
 
 #include "m2s_sort.cuh"
@@ -171,13 +173,17 @@ __device__ __forceinline__ TileFrame tile_frame(const unsigned char* scratch, co
 }
 
 // the tile's pairs in batches of kTileThreads: thread `slot` calls stage(slot, value) for pair `slot` of the batch, then
-// every thread calls test(j) for each staged slot j in pair order
-template <typename Stage, typename Test>
-__device__ __forceinline__ void tile_batches(const TileFrame& f, const uint32_t* __restrict__ vals, Stage&& stage, Test&& test) {
+// every thread calls test(j) for each staged slot j in pair order.  done (optional): a per-thread predicate; the tile
+// stops before the next batch once it holds for every thread of the CTA
+struct NeverDone {};
+template <typename Stage, typename Test, typename Done = NeverDone>
+__device__ __forceinline__ void tile_batches(const TileFrame& f, const uint32_t* __restrict__ vals, Stage&& stage, Test&& test,
+                                             Done&& done = Done()) {
     const int tid = threadIdx.x;
     for (uint32_t base = f.r0; base < f.r1; base += kTileThreads) {
         const uint32_t nb = min(f.r1 - base, (uint32_t)kTileThreads);
-        __syncthreads();
+        if constexpr (std::is_same_v<std::decay_t<Done>, NeverDone>) __syncthreads();
+        else if (__syncthreads_and(done())) break;
         if ((uint32_t)tid < nb) stage(tid, vals[base + tid]);
         __syncthreads();
         for (uint32_t j = 0; j < nb; ++j) test(j);

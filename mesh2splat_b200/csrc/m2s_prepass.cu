@@ -10,6 +10,7 @@
 // m2s_ply_read loads from a .ply (u_format 1, u_plyHasPbr 0 or 1): the record layout and u_format are separate arguments.
 // Beyond the reference, prepass_sh_kernel gives those loaded records their view-dependent colour from the SH rest
 // coefficients m2s_ply_read_sh keeps (render modes 0 and 6).
+#include "m2s_gauss.cuh"
 #include "m2s_prepass.cuh"
 
 namespace m2s {
@@ -50,63 +51,6 @@ __device__ __forceinline__ bool prepass_behind_mesh(const PrepassArgs& a, const 
     return my > __fadd_rn(depth, 0.00002f);
 }
 
-// ---- view-dependent colour (m2s_prepass_sh, beyond the reference): graphdeco's computeColorFromSH with its constants and
-// the signs folded into the basis; every operation one round-to-nearest fp32 step without contraction, as
-// oracle/m2s_sh_oracle.c restates it ----
-// rest = sum over k = 1..K of B_k coeff_k, in k order per channel; c: the gaussian's block (coefficient-major r g b)
-template <int D>
-__device__ __forceinline__ void sh_rest(const float4* c, float x, float y, float z, float rest[3]) {
-    constexpr int K = (D + 1) * (D + 1) - 1;
-    const float C1 = 0.4886025119029199f;
-    float B[15];
-    B[0] = __fmul_rn(-C1, y); B[1] = __fmul_rn(C1, z); B[2] = __fmul_rn(-C1, x);
-    if (D >= 2) {
-        const float xx = __fmul_rn(x, x), yy = __fmul_rn(y, y), zz = __fmul_rn(z, z);
-        const float xy = __fmul_rn(x, y), yz = __fmul_rn(y, z), xz = __fmul_rn(x, z);
-        B[3] = __fmul_rn(1.0925484305920792f, xy);
-        B[4] = __fmul_rn(-1.0925484305920792f, yz);
-        B[5] = __fmul_rn(0.31539156525252005f, __fsub_rn(__fsub_rn(__fmul_rn(2.0f, zz), xx), yy));
-        B[6] = __fmul_rn(-1.0925484305920792f, xz);
-        B[7] = __fmul_rn(0.5462742152960396f, __fsub_rn(xx, yy));
-        if (D >= 3) {
-            B[8] = __fmul_rn(__fmul_rn(-0.5900435899266435f, y), __fsub_rn(__fmul_rn(3.0f, xx), yy));
-            B[9] = __fmul_rn(__fmul_rn(2.890611442640554f, xy), z);
-            B[10] = __fmul_rn(__fmul_rn(-0.4570457994644658f, y), __fsub_rn(__fsub_rn(__fmul_rn(4.0f, zz), xx), yy));
-            B[11] = __fmul_rn(__fmul_rn(0.3731763325901154f, z), __fsub_rn(__fsub_rn(__fmul_rn(2.0f, zz), __fmul_rn(3.0f, xx)), __fmul_rn(3.0f, yy)));
-            B[12] = __fmul_rn(__fmul_rn(-0.4570457994644658f, x), __fsub_rn(__fsub_rn(__fmul_rn(4.0f, zz), xx), yy));
-            B[13] = __fmul_rn(__fmul_rn(1.445305721320277f, z), __fsub_rn(xx, yy));
-            B[14] = __fmul_rn(__fmul_rn(-0.5900435899266435f, x), __fsub_rn(xx, __fmul_rn(3.0f, yy)));
-        }
-    }
-    rest[0] = rest[1] = rest[2] = 0.0f;
-#pragma unroll
-    for (int v = 0; v < (3 * K + 3) / 4; ++v) {   // every load of the block first: one round trip to memory
-        const float4 q = __ldg(c + v);
-        const float e[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-            if (4 * v + j < 3 * K) rest[(4 * v + j) % 3] = __fadd_rn(rest[(4 * v + j) % 3], __fmul_rn(B[(4 * v + j) / 3], e[j]));
-    }
-}
-
-// the colour of gaussian gid at model-space position p seen from s.cam: max(colour + rest, 0) per channel (glm::max: NaN kept)
-__device__ __forceinline__ void sh_colour(const PrepassShArgs& s, unsigned long long gid, float px, float py, float pz, float& r, float& g,
-                                          float& b) {
-    const float dx = __fsub_rn(px, s.cam[0]), dy = __fsub_rn(py, s.cam[1]), dz = __fsub_rn(pz, s.cam[2]);
-    const float len = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
-    float rest[3] = {0.0f, 0.0f, 0.0f};
-    if (len != 0.0f) {
-        const float inv = __fdiv_rn(1.0f, len);
-        const float x = __fmul_rn(dx, inv), y = __fmul_rn(dy, inv), z = __fmul_rn(dz, inv);
-        const float4* c = s.sh + gid * s.vec4;
-        if (s.degree == 1) sh_rest<1>(c, x, y, z, rest);
-        else if (s.degree == 2) sh_rest<2>(c, x, y, z, rest);
-        else sh_rest<3>(c, x, y, z, rest);
-    }
-    r = __fadd_rn(r, rest[0]); g = __fadd_rn(g, rest[1]); b = __fadd_rn(b, rest[2]);
-    r = r < 0.0f ? 0.0f : r; g = g < 0.0f ? 0.0f : g; b = b < 0.0f ? 0.0f : b;
-}
-
 // kDepth: the prepass with the mesh depth test (map: dw x dh floats as m2s_mesh_depth writes them); kSh: the colour of
 // render modes 0 and 6 from the SH rest coefficients (sh)
 template <bool kStage, bool kDepth, bool kSh = false>
@@ -137,24 +81,22 @@ __device__ __forceinline__ void prepass_body(const PrepassArgs& a, const float* 
     // ---- the gaussian as the shader sees it (GaussianVertex) ----
     float px = 0, py = 0, pz = 0, cr = 0, cg = 0, cb = 0, ca = 0, sx = 0, sy = 0, sz = 0, nx = 0, ny = 0, nz = 0, qx = 1, qy = 0, qz = 0, qw = 0, pb0 = 0, pb1 = 0;
     if (alive) {
+        GaussFields g;
         if (a.layout == 0) {   // REF96: position color scale normal rotation pbr
             const float4* gs = stage[warp] + lane * 6;
             const float4* gg = reinterpret_cast<const float4*>(a.records) + gid * 6;
-            const float4 p = kStage ? gs[0] : __ldg(gg), c = kStage ? gs[1] : __ldg(gg + 1), s = kStage ? gs[2] : __ldg(gg + 2),
-                         nn = kStage ? gs[3] : __ldg(gg + 3), q = kStage ? gs[4] : __ldg(gg + 4), pb = kStage ? gs[5] : __ldg(gg + 5);
-            px = p.x; py = p.y; pz = p.z; cr = c.x; cg = c.y; cb = c.z; ca = c.w; sx = s.x; sy = s.y; sz = s.z;
-            nx = nn.x; ny = nn.y; nz = nn.z; qx = q.x; qy = q.y; qz = q.z; qw = q.w; pb0 = pb.x; pb1 = pb.y;
-        } else {               // PACKED56: xyz | quat wxyz | log-scale | SH0 | opacity logit  (parsers.cpp:560-622 on load)
+            ref96_fields(kStage ? gs[0] : __ldg(gg), kStage ? gs[1] : __ldg(gg + 1), kStage ? gs[2] : __ldg(gg + 2),
+                         kStage ? gs[3] : __ldg(gg + 3), kStage ? gs[4] : __ldg(gg + 4), kStage ? gs[5] : __ldg(gg + 5), g);
+            px = g.px; py = g.py; pz = g.pz; cr = g.cr; cg = g.cg; cb = g.cb; ca = g.ca; sx = g.sx; sy = g.sy; sz = g.sz;
+            nx = g.nx; ny = g.ny; nz = g.nz; qx = g.qx; qy = g.qy; qz = g.qz; qw = g.qw; pb0 = g.pb0; pb1 = g.pb1;
+        } else {               // PACKED56
             const float2* gs = reinterpret_cast<const float2*>(reinterpret_cast<const unsigned char*>(stage[warp]) + lane * 56u);
             const float2* gg = reinterpret_cast<const float2*>(a.records + gid * 56ull);
-            const float2 f0 = kStage ? gs[0] : __ldg(gg), f1 = kStage ? gs[1] : __ldg(gg + 1), f2 = kStage ? gs[2] : __ldg(gg + 2),
-                         f3 = kStage ? gs[3] : __ldg(gg + 3), f4 = kStage ? gs[4] : __ldg(gg + 4), f5 = kStage ? gs[5] : __ldg(gg + 5),
-                         f6 = kStage ? gs[6] : __ldg(gg + 6);
-            px = f0.x; py = f0.y; pz = f1.x; qx = f1.y; qy = f2.x; qz = f2.y; qw = f3.x;
-            sx = expf(f3.y); sy = expf(f4.x); sz = expf(f4.y);
-            const float kC0 = 0.28209479177387814f;
-            cr = f5.x * kC0 + 0.5f; cg = f5.y * kC0 + 0.5f; cb = f6.x * kC0 + 0.5f;
-            ca = 1.0f / (1.0f + expf(-f6.y));
+            packed56_fields<false>(kStage ? gs[0] : __ldg(gg), kStage ? gs[1] : __ldg(gg + 1), kStage ? gs[2] : __ldg(gg + 2),
+                                   kStage ? gs[3] : __ldg(gg + 3), kStage ? gs[4] : __ldg(gg + 4), kStage ? gs[5] : __ldg(gg + 5),
+                                   kStage ? gs[6] : __ldg(gg + 6), g);
+            px = g.px; py = g.py; pz = g.pz; qx = g.qx; qy = g.qy; qz = g.qz; qw = g.qw;
+            sx = g.sx; sy = g.sy; sz = g.sz; cr = g.cr; cg = g.cg; cb = g.cb; ca = g.ca;
         }
     }
     if (kStage) __syncwarp();   // every lane has its record: the stage is free for the warp's output
@@ -210,7 +152,7 @@ __device__ __forceinline__ void prepass_body(const PrepassArgs& a, const float* 
         float o0 = 0.f, o1 = 0.f, o2 = 0.f, o3 = 0.f;                    // :132-148
         if (a.render_mode == 0 || a.render_mode == 6) {
             o0 = cr; o1 = cg; o2 = cb; o3 = ca;
-            if (kSh) sh_colour(*sh, gid, px, py, pz, o0, o1, o2);   // survivors of the frustum cull only
+            if (kSh) sh_colour(sh->sh, sh->vec4, sh->degree, sh->cam, gid, px, py, pz, o0, o1, o2);   // survivors of the frustum cull only
         }
         else if (a.render_mode == 1) {
             const float d = clamp01(expf(-20.0f * clamp01((-vs2 - a.near_far[0]) / (a.near_far[1] - a.near_far[0]))));   // common.glsl:80-84

@@ -200,30 +200,36 @@ __global__ void __launch_bounds__(kGatherThreads) sort_gather_kernel(const float
     }
 }
 
+cudaError_t sort_order_launch(const uint32_t* keys, unsigned long long count, const uint32_t* d_count, uint32_t* order, uint32_t* scratch,
+                              int sm_count, cudaStream_t stream) {
+    if (count == 0) return cudaSuccess;
+    const SortLayout l = sort_layout(count);
+    uint32_t* hist = scratch;
+    uint32_t* counters = scratch + kSortPasses * 256;
+    uint32_t* status = counters + 32;
+    uint32_t* kb[2] = {scratch + l.ctrl_words, scratch + l.ctrl_words + 2 * l.buf_words};
+    uint32_t* vb[2] = {scratch + l.ctrl_words + l.buf_words, scratch + l.ctrl_words + 3 * l.buf_words};
+    cudaError_t e = cudaMemsetAsync(scratch, 0, l.ctrl_words * sizeof(uint32_t), stream);
+    if (e != cudaSuccess) return e;
+    const unsigned hist_grid = (unsigned)std::min<uint64_t>(l.tiles, 2ull * sm_count);
+    sort_hist_kernel<<<hist_grid, kSortThreads, 0, stream>>>(keys, count, d_count, hist);
+    sort_scan_kernel<<<1, kSortThreads, 0, stream>>>(hist);
+    const unsigned grid = (unsigned)l.tiles;
+    const size_t sw = l.tiles * 256;
+    sort_pass_kernel<true, false><<<grid, kSortThreads, 0, stream>>>(keys, nullptr, kb[0], vb[0], count, d_count, hist + 0 * 256,
+                                                                      counters + 0, status + 0 * sw, 0u);
+    sort_pass_kernel<false, false><<<grid, kSortThreads, 0, stream>>>(kb[0], vb[0], kb[1], vb[1], count, d_count, hist + 1 * 256,
+                                                                       counters + 1, status + 1 * sw, 8u);
+    sort_pass_kernel<false, false><<<grid, kSortThreads, 0, stream>>>(kb[1], vb[1], kb[0], vb[0], count, d_count, hist + 2 * 256,
+                                                                       counters + 2, status + 2 * sw, 16u);
+    sort_pass_kernel<false, true><<<grid, kSortThreads, 0, stream>>>(kb[0], vb[0], nullptr, order, count, d_count, hist + 3 * 256,
+                                                                      counters + 3, status + 3 * sw, 24u);
+    return cudaGetLastError();
+}
+
 cudaError_t sort_launch(const SortArgs& a, int sm_count, cudaStream_t stream) {
-    const SortLayout l = sort_layout(a.count);
-    if (a.count > 0) {
-        uint32_t* hist = a.scratch;
-        uint32_t* counters = a.scratch + kSortPasses * 256;
-        uint32_t* status = counters + 32;
-        uint32_t* kb[2] = {a.scratch + l.ctrl_words, a.scratch + l.ctrl_words + 2 * l.buf_words};
-        uint32_t* vb[2] = {a.scratch + l.ctrl_words + l.buf_words, a.scratch + l.ctrl_words + 3 * l.buf_words};
-        cudaError_t e = cudaMemsetAsync(a.scratch, 0, l.ctrl_words * sizeof(uint32_t), stream);
-        if (e != cudaSuccess) return e;
-        const unsigned hist_grid = (unsigned)std::min<uint64_t>(l.tiles, 2ull * sm_count);
-        sort_hist_kernel<<<hist_grid, kSortThreads, 0, stream>>>(a.depth_bits, a.count, a.d_count, hist);
-        sort_scan_kernel<<<1, kSortThreads, 0, stream>>>(hist);
-        const unsigned grid = (unsigned)l.tiles;
-        const size_t sw = l.tiles * 256;
-        sort_pass_kernel<true, false><<<grid, kSortThreads, 0, stream>>>(a.depth_bits, nullptr, kb[0], vb[0], a.count, a.d_count,
-                                                                          hist + 0 * 256, counters + 0, status + 0 * sw, 0u);
-        sort_pass_kernel<false, false><<<grid, kSortThreads, 0, stream>>>(kb[0], vb[0], kb[1], vb[1], a.count, a.d_count,
-                                                                           hist + 1 * 256, counters + 1, status + 1 * sw, 8u);
-        sort_pass_kernel<false, false><<<grid, kSortThreads, 0, stream>>>(kb[1], vb[1], kb[0], vb[0], a.count, a.d_count,
-                                                                           hist + 2 * 256, counters + 2, status + 2 * sw, 16u);
-        sort_pass_kernel<false, true><<<grid, kSortThreads, 0, stream>>>(kb[0], vb[0], nullptr, a.order, a.count, a.d_count,
-                                                                          hist + 3 * 256, counters + 3, status + 3 * sw, 24u);
-    }
+    const cudaError_t e = sort_order_launch(a.depth_bits, a.count, a.d_count, a.order, a.scratch, sm_count, stream);
+    if (e != cudaSuccess) return e;
     if (a.count > 0 || a.draw) {
         const uint64_t want = (a.count * 6ull + kGatherThreads - 1) / kGatherThreads;
         const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(want, 16ull * sm_count));

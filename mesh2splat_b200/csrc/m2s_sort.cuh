@@ -47,6 +47,10 @@ struct SortArgs {
 };
 
 cudaError_t sort_launch(const SortArgs& args, int sm_count, cudaStream_t stream);
+// The permutation alone: order[i] = the index of the i-th smallest of the n = min(count, *d_count) uint32 keys, ties in
+// index order (the depth sort without its gather; the 3DGS render's depth order).  scratch: SortLayout of `count`.
+cudaError_t sort_order_launch(const uint32_t* keys, unsigned long long count, const uint32_t* d_count, uint32_t* order, uint32_t* scratch,
+                              int sm_count, cudaStream_t stream);
 
 // The splat draw's (tile, quad) pairs: a stable sort of n = *d_n <= capacity (key < 2^16, value) pairs with the same
 // histogram, scan and onesweep pass kernels, two passes (digits 0 and 1).  The pairs go in, and come out, in key and

@@ -3,6 +3,7 @@
 // uniforms built on the host, and the launches.
 #include <cmath>
 
+#include "m2s_3dgs.cuh"
 #include "m2s_bin.cuh"
 #include "m2s_ctx.cuh"
 #include "m2s_depth.cuh"
@@ -209,9 +210,8 @@ static m2s_status prepass_sh_check(const m2s_ctx* ctx, const void* d_records, ui
 }
 
 // the camera position in model space: the translation column of inverse(V M), in fp64 from the fp32 matrices, rounded once
-// to fp32; false for a singular V M
-static bool sh_camera(const m2s_prepass_params* p, float cam[3]) {
-    const float *V = p->world_to_view, *M = p->model_to_world;
+// to fp32; false for a singular V M.  mv (optional): V M itself, rounded once to fp32
+static bool sh_camera(const float* V, const float* M, float cam[3], float* mv = nullptr) {
     double VM[16], inv[16];
     for (int c = 0; c < 4; ++c)
         for (int r = 0; r < 4; ++r)
@@ -219,6 +219,8 @@ static bool sh_camera(const m2s_prepass_params* p, float cam[3]) {
                             (double)V[12 + r] * M[c * 4 + 3];
     if (!invert4(VM, inv) || !std::isfinite(inv[12]) || !std::isfinite(inv[13]) || !std::isfinite(inv[14])) return false;
     for (int k = 0; k < 3; ++k) cam[k] = (float)inv[12 + k];
+    if (mv)
+        for (int k = 0; k < 16; ++k) mv[k] = (float)VM[k];
     return true;
 }
 
@@ -231,7 +233,7 @@ M2S_EXPORT m2s_status m2s_prepass_sh_enqueue(m2s_ctx* ctx, const void* d_records
     std::memset(&a, 0, sizeof(a));
     st = prepass_fill(d_records, count, d_count, p, d_quads, d_depths, d_valid, a.p);
     if (st != M2S_OK) return st;
-    if (!sh_camera(p, a.cam)) return invalid("m2s_prepass_sh", "world_to_view * model_to_world is singular");
+    if (!sh_camera(p->world_to_view, p->model_to_world, a.cam)) return invalid("m2s_prepass_sh", "world_to_view * model_to_world is singular");
     a.sh = reinterpret_cast<const float4*>(d_sh);
     a.vec4 = M2S_SH_FLOATS(buffer_degree) / 4;
     a.degree = sh_degree;
@@ -662,4 +664,121 @@ M2S_EXPORT m2s_status m2s_deferred_light_split_enqueue(m2s_ctx* ctx, const m2s_g
 M2S_EXPORT m2s_status m2s_deferred_light_split(m2s_ctx* ctx, const m2s_gbuffer* splat, const m2s_gbuffer* mesh, const float* d_cube,
                                                const m2s_light_params* p, float split_position, uint8_t* d_image) {
     return synced(ctx, m2s_deferred_light_split_enqueue(ctx, splat, mesh, d_cube, p, split_position, d_image, nullptr));
+}
+
+// ---- the standard 3DGS render (beyond the reference): graphdeco's forward pass, DESIGN §2 ----------------------------------
+// the argument checks and the kernels' arguments (a.count .. a.order and the targets; the scratch pointers are the caller's
+// to set); M2S_E_INVALID with the error "<fn>: ..." for anything m2s.h rejects
+static m2s_status gs3d_args(const char* fn, const m2s_ctx* ctx, const void* d_records, uint64_t count, const uint64_t* d_count,
+                            const m2s_3dgs_params* p, const float* d_sh, uint32_t buffer_degree, uint32_t sh_degree, Gs3dArgs& a) {
+    if (!ctx || !p) return invalid(fn, "NULL argument");
+    if (count && !d_records) return invalid(fn, "NULL records");
+    if (count >= kGs3dMaxCount) return invalid(fn, "too many gaussians (< 2^30 supported)");
+    if (!sizes_ok(fn, "width and height", kTileMaxSide, {p->width, p->height})) return M2S_E_INVALID;
+    ViewInput v;
+    if (!view_input(fn, p->layout, v)) return M2S_E_INVALID;
+    if (sh_degree || buffer_degree || d_sh) {
+        if (p->layout != M2S_VIEW_PLY && p->layout != M2S_VIEW_PLY_PBR) return invalid(fn, "SH with layouts VIEW_PLY and VIEW_PLY_PBR only");
+        if (buffer_degree > 3 || sh_degree > buffer_degree) return invalid(fn, "buffer_degree must be 0..3, sh_degree 0..buffer_degree");
+        if (sh_degree && !d_sh) return invalid(fn, "NULL d_sh");
+    }
+    if (!aligned_ok(fn, "the record and SH buffers must be 16-byte aligned", {{d_records, 16}, {d_sh, 16}})) return M2S_E_INVALID;
+    for (int k = 0; k < 16; ++k)
+        if (!std::isfinite(p->world_to_view[k]) || !std::isfinite(p->view_to_clip[k]) || !std::isfinite(p->model_to_world[k]))
+            return invalid(fn, "the matrices must be finite");
+    if (!(p->near > 0.0f)) return invalid(fn, "near must be > 0");
+    if (!(p->view_to_clip[0] > 0.0f) || !(p->view_to_clip[5] > 0.0f)) return invalid(fn, "view_to_clip[0] and [5] must be > 0");
+    std::memset(&a, 0, sizeof(a));
+    if (!sh_camera(p->world_to_view, p->model_to_world, a.cam, a.MV)) return invalid(fn, "world_to_view * model_to_world is singular");
+    std::memcpy(a.P, p->view_to_clip, 64);
+    a.near = p->near;
+    a.mult = p->layout == M2S_LAYOUT_REF96 ? p->std_dev : 1.0f;
+    a.scale_modifier = p->scale_modifier;
+    for (int k = 0; k < 3; ++k) a.bg[k] = p->background[k];
+    a.width = p->width; a.height = p->height;
+    a.layout = v.layout;
+    a.sh_vec4 = M2S_SH_FLOATS(buffer_degree) / 4;
+    a.sh_degree = sh_degree;
+    a.sh = reinterpret_cast<const float4*>(d_sh);
+    a.count = count;
+    a.d_count = reinterpret_cast<const unsigned long long*>(d_count);
+    a.records = static_cast<const unsigned char*>(d_records);
+    a.sm_count = ctx->sm_count;
+    return M2S_OK;
+}
+
+// the render's own scratch (splat records, keys, order, their sort), grown on stream
+static m2s_status gs3d_scratch(m2s_ctx* ctx, Gs3dArgs& a, cudaStream_t stream) {
+    const Gs3dLayout l = gs3d_layout(a.count);
+    m2s_status st = grow(ctx, ctx->gs3d, l.total_bytes, stream);
+    if (st == M2S_OK && a.count) st = grow(ctx, ctx->gs3d_sort, sort_layout(a.count).total_bytes, stream);
+    if (st != M2S_OK) return st;
+    unsigned char* base = static_cast<unsigned char*>(ctx->gs3d.p);
+    a.ctrl = reinterpret_cast<uint32_t*>(base);
+    a.splats = reinterpret_cast<Gs3dSplat*>(base + l.splats_off);
+    a.keys = reinterpret_cast<uint32_t*>(base + l.keys_off);
+    a.order = reinterpret_cast<uint32_t*>(base + l.order_off);
+    a.sort_scratch = static_cast<uint32_t*>(ctx->gs3d_sort.p);
+    return M2S_OK;
+}
+
+// both forms of the 3DGS render: the argument checks, the arguments, the scratch, then bin_pass
+static m2s_status gs3d_pass(m2s_ctx* ctx, const void* d_records, uint64_t count, const uint64_t* d_count, const m2s_3dgs_params* p,
+                            const float* d_sh, uint32_t buffer_degree, uint32_t sh_degree, float* d_rgba32f, uint8_t* d_rgba8, void* stream_,
+                            bool sync, uint64_t max_pairs, uint64_t* pairs, uint32_t* d_drawn) {
+    const char* fn = "m2s_3dgs_render";
+    Gs3dArgs a;
+    m2s_status st = gs3d_args(fn, ctx, d_records, count, d_count, p, d_sh, buffer_degree, sh_degree, a);
+    if (st != M2S_OK) return st;
+    if (!d_rgba32f && !d_rgba8) return invalid(fn, "no targets");
+    if (!aligned_ok(fn, "the RGBA32F target must be 16-byte aligned, the RGBA8 target 4-byte aligned", {{d_rgba32f, 16}, {d_rgba8, 4}}) ||
+        !pair_budget_ok(fn, max_pairs))
+        return M2S_E_INVALID;
+    a.rgba32f = reinterpret_cast<float4*>(d_rgba32f);
+    a.rgba8 = reinterpret_cast<uint32_t*>(d_rgba8);
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    cudaStream_t stream = pick_stream(ctx, stream_);
+    st = gs3d_scratch(ctx, a, stream);
+    if (st != M2S_OK) return st;
+    return bin_pass(ctx, ctx->gs3d_bins, bin_layout(count, tile_count(p->width, p->height)).total_bytes, a, gs3d_count_launch, gs3d_draw_launch,
+                    stream, sync, max_pairs, pairs, d_drawn, "m2s_3dgs_render: the gaussians need 2^30 or more (tile, gaussian) pairs");
+}
+
+M2S_EXPORT m2s_status m2s_3dgs_render_enqueue(m2s_ctx* ctx, const void* d_records, uint64_t count, const uint64_t* d_count,
+                                              const m2s_3dgs_params* p, const float* d_sh, uint32_t buffer_degree, uint32_t sh_degree,
+                                              float* d_rgba32f, uint8_t* d_rgba8, uint64_t max_pairs, uint64_t* d_pairs, uint32_t* d_drawn,
+                                              void* stream_) {
+    return gs3d_pass(ctx, d_records, count, d_count, p, d_sh, buffer_degree, sh_degree, d_rgba32f, d_rgba8, stream_, false, max_pairs, d_pairs,
+                     d_drawn);
+}
+
+M2S_EXPORT m2s_status m2s_3dgs_render(m2s_ctx* ctx, const void* d_records, uint64_t count, const m2s_3dgs_params* p, const float* d_sh,
+                                      uint32_t buffer_degree, uint32_t sh_degree, float* d_rgba32f, uint8_t* d_rgba8, uint64_t* pairs) {
+    return gs3d_pass(ctx, d_records, count, nullptr, p, d_sh, buffer_degree, sh_degree, d_rgba32f, d_rgba8, nullptr, true, 0, pairs, nullptr);
+}
+
+// Test aid (not part of m2s.h, like m2s_debug_codec_eval): the preprocess kernel alone on the context stream, synchronised.
+// d_splats: count x 48 B (Gs3dSplat, 16-byte aligned), d_keys: count uint32 depth keys (kGs3dCulled for a culled record);
+// *survivors (optional, host) the records not culled.
+M2S_EXPORT m2s_status m2s_debug_3dgs_preprocess(m2s_ctx* ctx, const void* d_records, uint64_t count, const m2s_3dgs_params* p,
+                                                const float* d_sh, uint32_t buffer_degree, uint32_t sh_degree, void* d_splats,
+                                                uint32_t* d_keys, uint32_t* survivors) {
+    const char* fn = "m2s_debug_3dgs_preprocess";
+    Gs3dArgs a;
+    m2s_status st = gs3d_args(fn, ctx, d_records, count, nullptr, p, d_sh, buffer_degree, sh_degree, a);
+    if (st != M2S_OK) return st;
+    if (count && (!d_splats || !d_keys)) return invalid(fn, "NULL output");
+    if (!aligned_ok(fn, "the splat buffer must be 16-byte aligned, the keys 4-byte aligned", {{d_splats, 16}, {d_keys, 4}})) return M2S_E_INVALID;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    st = grow(ctx, ctx->gs3d, 256, ctx->stream);
+    if (st != M2S_OK) return st;
+    a.ctrl = static_cast<uint32_t*>(ctx->gs3d.p);
+    a.splats = static_cast<Gs3dSplat*>(d_splats);
+    a.keys = d_keys;
+    CUDA_TRY(gs3d_preprocess_launch(a, ctx->stream));
+    uint32_t ctrl[2] = {0, 0};
+    CUDA_TRY(cudaMemcpyAsync(ctrl, a.ctrl, sizeof(ctrl), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    if (survivors) *survivors = ctrl[1];
+    return M2S_OK;
 }
