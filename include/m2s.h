@@ -190,7 +190,9 @@ m2s_status m2s_compute_bboxes(const float* triangles, m2s_primitive* primitives,
                               uint32_t primitive_count, int cumulative);
 
 /* Copies triangles + primitive table + textures to the device and builds mip levels 1..4
- * (2x2 box, round-to-nearest) on the GPU.  Host pointers may be pageable. */
+ * (2x2 box, round-to-nearest) on the GPU, and a 64-byte-per-triangle copy of the positions and uvs that PACKED56
+ * conversions read instead of the 144-byte triangles (device memory: 208 B per triangle in all).  Host pointers may be
+ * pageable. */
 m2s_status m2s_scene_upload(m2s_ctx* ctx, const m2s_scene* scene, m2s_dscene** out);
 /* One shard of a scene (multi-GPU: one contiguous triangle range per rank): copies the triangles
  * [first_triangle, first_triangle + triangle_count) to their global positions and, of the maps `layout` consumes, only

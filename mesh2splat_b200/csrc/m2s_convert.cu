@@ -13,6 +13,10 @@ M2S_EXPORT void m2s_debug_set_trace(void* p) { g_trace = (unsigned long long*)p;
 // records are compared against
 static bool g_direct_off = false;
 M2S_EXPORT void m2s_debug_set_direct_off(int off) { g_direct_off = off != 0; }
+// Test aid: PACKED56 conversions stage the 144-byte triangles even when the scene has the 64-byte position/uv stream, the
+// route the slim stream's records are compared against
+static bool g_slim_off = false;
+M2S_EXPORT void m2s_debug_set_slim_off(int off) { g_slim_off = off != 0; }
 
 // ---- the hot path -----------------------------------------------------------------------------
 uint64_t m2s::effective_cap(const m2s_dscene* s, const m2s_params* p, uint64_t out_capacity) {
@@ -144,6 +148,7 @@ m2s_status m2s::convert_enqueue_impl(m2s_ctx* ctx, const m2s_dscene* s, const m2
     ConvertArgs a;
     std::memset(&a, 0, sizeof(a));
     a.tris = s->d_tris;
+    a.tris_slim = (klayout == M2S_LAYOUT_PACKED56 && !g_slim_off) ? s->d_tris_slim : nullptr;   // only PACKED56's set-up reads it
     a.tri_first = (uint32_t)tr.first;
     a.tri_count = (uint32_t)tr.count;
     a.ranges = s->d_ranges; a.nranges = s->nranges;

@@ -114,6 +114,10 @@ struct m2s_ctx {
 struct m2s_dscene {
     float4* d_tris = nullptr;
     uint64_t ntri = 0;
+    // the positions and uvs of d_tris repacked into 4 float4 per triangle (ConvertArgs::tris_slim), derived at upload like
+    // the mip levels: the raster pass of a PACKED56 conversion reads 64 B per triangle instead of 144.  Only scenes uploaded
+    // whole in one call have it; partial and lazy uploads (the host pipeline, m2s_scene_upload_range) leave it null
+    float4* d_tris_slim = nullptr;
     m2s::DRange* d_ranges = nullptr;
     uint32_t nranges = 0;
     m2s::DPrim* d_prims = nullptr;

@@ -9,6 +9,7 @@ constexpr int kMaxPeers = 8;             // GPUs of one NVSwitch domain
 constexpr int kMaxLevels = 5;            // levels 0..4 (GL_TEXTURE_MAX_LEVEL 4, glUtils.cpp:313)
 constexpr int kUnitTris = 32;            // max triangles per work unit (one lane per triangle)
 constexpr int kTriBytes = 144;           // 36 floats
+constexpr int kSlimTriBytes = 64;        // the position/uv stream of PACKED56's raster pass: 4 float4 per triangle
 constexpr uint32_t kSmallCand = 64;      // <= this many candidate pixels (and <= 32 rows): coverage as a 64-bit mask
 constexpr int kItemBlocks = 32;          // row blocks (<= 32 pixel rows of one triangle) per fragment work item
 constexpr int kStashItems = 8;           // work items a raster warp publishes with one atomic
@@ -77,6 +78,8 @@ struct DRange {
 
 struct ConvertArgs {
     const float4* tris;   // 9 float4 per triangle (3 x {pos3 nrm3 tan4 uv2})
+    const float4* tris_slim;  // PACKED56 when the scene has it, else null: 4 float4 per triangle, {P0 u0} {P1 u1} {P2 u2}
+                              // {v0 v1 v2 0} (m2s_dscene::d_tris_slim), what the raster kernel stages instead of `tris`
     uint32_t tri_first;   // shard
     uint32_t tri_count;
     const DRange* ranges;

@@ -11,7 +11,8 @@
 //     claimed from a global counter; the next unit's triangles are in flight (TMA) while this one is processed.
 //     Launches of 16-triangle units (ConvertPlan::pair_first): the first pass sets up units 2g and 2g + 1 on the two
 //     half warps.  A pass's direct shading is shared with the CTA's other warps (CtaQueue)
-//   TMA (cp.async.bulk + mbarrier complete_tx) stages the unit's 144 B/triangle into shared memory
+//   TMA (cp.async.bulk + mbarrier complete_tx) stages the unit's 144 B/triangle into shared memory (PACKED56 on a scene
+//     uploaded whole: 64 B/triangle, only the positions and uvs the set-up reads)
 //   per-triangle stage, one LANE per triangle (converterGS.glsl:326-443): longest edge, face normal, dominant
 //     axis, orthographic uv, quaternion, UV->3D Jacobian scale; rasteriser set-up: 24.8 fixed-point window
 //     coords, int64 edge functions, top-left ownership bits, candidate pixel box (clamped to the call's
@@ -79,7 +80,7 @@ __device__ __forceinline__ f3 cross3(f3 x, f3 y) {
 
 template <int RK>
 struct __align__(128) WarpBlock {
-    float4 tri[kUnitTris * 9];                    // 4608 B, TMA destination
+    float4 tri[kUnitTris * 9];                    // 4608 B, TMA destination (the 64-byte stream uses 2048 B of it)
     TriRec<RCfg<RK>::kMaps> rec[kUnitTris];       // TMA source
     BlockRef pend[kStashItems * kItemBlocks];     // the stash: row blocks of up to kStashItems work items
     uint32_t itN[kStashItems];                    // blocks per item | kItUnit / kItSplit
@@ -88,6 +89,8 @@ struct __align__(128) WarpBlock {
     double logtab[RK == 1 ? 32 : 1];              // PACKED56: the direct path's copy of ref_logf's table (kLogfTab)
     uint32_t left;                                // posted pieces of this warp's direct pass not yet shaded (CtaQueue)
 };
+static_assert(offsetof(WarpBlock<1>, pend) % 16 == 0 && sizeof(WarpBlock<1>::pend) >= kUnitTris * kSlimTriBytes,
+              "PACKED56's 144-byte route restages a pass's triangles in their 64-byte form into the stash (restage_slim)");
 
 // The scene's descriptor tables as the set-up sees them: in shared memory when they fit (each CTA copies
 // them once — ~2100 warps (132 SMs x 16) chasing range -> primitive -> texture through the same few L2 lines pay a
@@ -126,8 +129,45 @@ struct TriSetup {
     unsigned incl = 0;
 };
 
+// The vertex values the set-up reads.  The set-up of PACKED56 (kSlim) reads a triangle in the 64-byte form of
+// ConvertArgs::tris_slim (4 float4: {P0 u0} {P1 u1} {P2 u2} {v0 v1 v2 0}), the three-map layouts read the 144-byte AoS
+// (9 float4: 3 x {pos3 nrm3 tan4 uv2}).  Both hold the same fp32 bits.
+struct TriVerts {
+    f3 P[3];
+    float u[3], v[3];
+};
+template <bool kSlim>
+__device__ __forceinline__ TriVerts tri_verts(const float4* __restrict__ t4) {
+    TriVerts tv;
+    if constexpr (kSlim) {
+        const float4 a = t4[0], b = t4[1], c = t4[2], d = t4[3];
+        tv.P[0] = {a.x, a.y, a.z}; tv.P[1] = {b.x, b.y, b.z}; tv.P[2] = {c.x, c.y, c.z};
+        tv.u[0] = a.w; tv.u[1] = b.w; tv.u[2] = c.w;
+        tv.v[0] = d.x; tv.v[1] = d.y; tv.v[2] = d.z;
+    } else {
+        const float4 q0 = t4[0], q3 = t4[3], q6 = t4[6];
+        const float4 q2 = t4[2], q5 = t4[5], q8 = t4[8];
+        tv.P[0] = {q0.x, q0.y, q0.z}; tv.P[1] = {q3.x, q3.y, q3.z}; tv.P[2] = {q6.x, q6.y, q6.z};
+        tv.u[0] = q2.z; tv.u[1] = q5.z; tv.u[2] = q8.z;
+        tv.v[0] = q2.w; tv.v[1] = q5.w; tv.v[2] = q8.w;
+    }
+    return tv;
+}
+// PACKED56 on a scene without the 64-byte stream (partial uploads, m2s_debug_set_slim_off): the lane's staged 144-byte
+// triangle `src` is rewritten into the 64-byte form at `dst`, which the set-up then reads: one form for the set-up.  `dst`
+// is the lane's slot in a free area of its warp's slice; the lane reads back only what it wrote itself.
+__device__ __forceinline__ const float4* restage_slim(const float4* __restrict__ src, float4* __restrict__ dst) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {   // vertex k: position = float4 3k, uv = the upper half of float4 3k + 2
+        const float4 p = src[3 * k];
+        dst[k] = make_float4(p.x, p.y, p.z, src[3 * k + 2].z);
+    }
+    dst[3] = make_float4(src[2].w, src[5].w, src[8].w, 0.0f);
+    return dst;
+}
+
 // ------------------------------------------------------------------------------------------
-// per-triangle stage + rasteriser set-up.  t4: 9 float4 in shared memory.
+// per-triangle stage + rasteriser set-up.  t4: the staged triangle in shared memory, in the form tri_verts<RK == 1> reads.
 // Returns the number of candidate pixels (0 => nothing to rasterise).
 // ------------------------------------------------------------------------------------------
 template <int RK>
@@ -146,10 +186,9 @@ __device__ __forceinline__ uint32_t setup_triangle(const float4* __restrict__ t4
     if (found < 0) return 0;
     const DPrim pr = tb.prims[found];
 
-    // vertex data: 3 x {pos3 nrm3 tan4 uv2} = 9 float4
-    const float4 q0 = t4[0], q3 = t4[3], q6 = t4[6];
-    const float4 q2 = t4[2], q5 = t4[5], q8 = t4[8];
-    const f3 P0 = {q0.x, q0.y, q0.z}, P1 = {q3.x, q3.y, q3.z}, P2 = {q6.x, q6.y, q6.z};
+    // vertex data: positions and uvs
+    const TriVerts tv = tri_verts<RK == 1>(t4);
+    const f3 P0 = tv.P[0], P1 = tv.P[1], P2 = tv.P[2];
 
     // converterGS.glsl:327-347
     f3 e1 = sub3(P1, P0), e2 = sub3(P2, P0), e3 = sub3(P2, P1);
@@ -203,7 +242,8 @@ __device__ __forceinline__ uint32_t setup_triangle(const float4* __restrict__ t4
     // origin; the per-pixel steps of the mesh uv (constant per triangle: uv is affine in window space)
     float dudx = 0.f, dvdx = 0.f, dudy = 0.f, dvdy = 0.f;
     {
-        const float uvx[3] = {q2.z, q5.z, q8.z}, uvy[3] = {q2.w, q5.w, q8.w};
+        const float* uvx = tv.u;
+        const float* uvy = tv.v;
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
             const int va = (k + 1) % 3, vb = (k + 2) % 3;
@@ -238,9 +278,9 @@ __device__ __forceinline__ uint32_t setup_triangle(const float4* __restrict__ t4
             tf.plane[at + stride] = (float)(lx0 * a0 + lx1 * a1 + lx2 * a2);
             tf.plane[at + 2 * stride] = (float)(ly0 * a0 + ly1 * a1 + ly2 * a2);
         };
-        put(0, 4, q0.x, q3.x, q6.x); put(1, 4, q0.y, q3.y, q6.y); put(2, 4, q0.z, q3.z, q6.z);   // position
-        put(3, 4, q2.z, q5.z, q8.z);                                                             // u
-        put(12, 1, q2.w, q5.w, q8.w);                                                            // v
+        put(0, 4, P0.x, P1.x, P2.x); put(1, 4, P0.y, P1.y, P2.y); put(2, 4, P0.z, P1.z, P2.z);   // position
+        put(3, 4, tv.u[0], tv.u[1], tv.u[2]);                                                    // u
+        put(12, 1, tv.v[0], tv.v[1], tv.v[2]);                                                   // v
     }
 
     // :399-407 rotation -> quaternion (w,x,y,z), quat_cast :131-183
@@ -745,8 +785,11 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
     extern __shared__ __align__(128) unsigned char smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     WarpBlock<RK>& wb = *reinterpret_cast<WarpBlock<RK>*>(smem + (size_t)warp * sizeof(WarpBlock<RK>));
-    const unsigned char* tri_bytes = reinterpret_cast<const unsigned char*>(a.tris);
     constexpr bool kDirectOK = (RK == 1);   // PACKED56: the records carry everything the shading needs
+    // PACKED56 stages only the positions and uvs when the scene has them repacked (64 B per triangle instead of 144).  Read
+    // from the kernel parameters where it is used: a pointer kept across the unit loop takes registers the loop needs
+    auto slim = [&]() { return RK == 1 && a.tris_slim != nullptr; };
+    auto tri_size = [&]() { return slim() ? (uint32_t)kSlimTriBytes : (uint32_t)kTriBytes; };
 #ifdef M2S_TRACE
     long long tr_prev_ = clock64();
     const long long tr_c0_ = tr_prev_;
@@ -759,8 +802,8 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
     }
     __syncwarp();
     // the first unit of every warp is static (unit = global warp id): no atomic, and nobody can grab two units
-    // while a neighbour gets none; its triangles start moving before the descriptor tables are copied.  Paired launches
-    // (ConvertPlan::pair_first): the first pass takes units 2g and 2g + 1, one per half warp, on one load
+    // while a neighbour gets none.  Paired launches (ConvertPlan::pair_first): the first pass takes units 2g and 2g + 1,
+    // one per half warp, on one load
     const uint32_t nwarps_total = gridDim.x * (blockDim.x >> 5);
     const uint32_t gwarp = blockIdx.x + gridDim.x * warp;  // warp w of every CTA before warp w+1 of any: SMs fill evenly
     bool pair = kDirectOK && a.pair_first != 0;
@@ -768,13 +811,13 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
     const uint32_t claim_base = pair ? 2 * nwarps_total : nwarps_total;   // the first unit the counter hands out
     auto issue_load = [&](uint32_t u, uint32_t n) {  // lane 0 only: up to n triangles from unit u on
         const uint32_t t0 = u * a.unit_tris;
-        const uint32_t bytes = min(n, a.tri_count - t0) * kTriBytes;
+        const uint32_t bytes = min(n, a.tri_count - t0) * tri_size();
+        const unsigned char* src = reinterpret_cast<const unsigned char*>(slim() ? a.tris_slim : a.tris);
         fence_proxy_async();
         mbar_arrive_expect_tx(&wb.bar, bytes);
-        tma_load_1d(wb.tri, tri_bytes + ((size_t)a.tri_first + t0) * kTriBytes, bytes, &wb.bar);
+        tma_load_1d(wb.tri, src + ((size_t)a.tri_first + t0) * tri_size(), bytes, &wb.bar);
     };
     auto claim = [&]() { return claim_base + atomicAdd(SCHED(a, 0), 1u); };   // lane 0 only: the next unit
-    if (lane == 0 && unit < a.n_units) issue_load(unit, pair ? 2 * a.unit_tris : a.unit_tris);
     // ref_logf's table for the direct path's opacities -> the warp's slice, as an asynchronous copy that lands while the
     // first unit is set up (waited for before the first shading; a CTA-wide copy would wait at the barrier below: ~1 us
     // more per warp, measured on the H100)
@@ -785,6 +828,10 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
     if (threadIdx.x == 0) { cq.tail = 0; cq.head = 0; cq.active = blockDim.x >> 5; }
     if (threadIdx.x < kCtaQueueCap) { cq.q[threadIdx.x].ready = 0u; cq.q[threadIdx.x].taken = 0u; }
     __syncthreads();  // tables + help queue: the only CTA-wide barrier before the end of the kernel
+    // the first unit's triangles start moving only now: issued before the table copy, the first loads of all the grid's
+    // warps (4.3 MB of slim triangles on the bench) reach HBM at once from a cold L2, and the table loads and this barrier
+    // queue behind them (DESIGN.md section 4)
+    if (lane == 0 && unit < a.n_units) issue_load(unit, pair ? 2 * a.unit_tris : a.unit_tris);
     const OutRange out = out_range(a);   // the direct path's records
     uint32_t phase = 0;
     uint32_t spar = 0;   // the half of this warp's output stage that its next group of direct records goes to
@@ -826,7 +873,11 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         uint32_t cnt = 0;
         TriSetup ts;
         Rec& myrec = wb.rec[lane];
-        if ((uint32_t)lane < ntri) cnt = setup_triangle<RK>(wb.tri + lane * 9, a.tri_first + t0 + lane, a, tabs, ts, myrec);
+        // the staged triangle in the form the set-up reads; the 144-byte route of PACKED56 restages it into the stash, which
+        // is empty between passes (stash_flush) and is not written before the set-up is done
+        const float4* tri4 = wb.tri + lane * (RK == 1 ? 4 : 9);
+        if (RK == 1 && !slim() && (uint32_t)lane < ntri) tri4 = restage_slim(wb.tri + lane * 9, reinterpret_cast<float4*>(wb.pend) + lane * 4);
+        if ((uint32_t)lane < ntri) cnt = setup_triangle<RK>(tri4, a.tri_first + t0 + lane, a, tabs, ts, myrec);
         __syncwarp();
         TR_PHASE(a, kTrSetup);
         next = __shfl_sync(0xffffffffu, next, 0);

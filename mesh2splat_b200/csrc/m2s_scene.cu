@@ -49,6 +49,23 @@ __global__ void __launch_bounds__(256) mip_groups_kernel(uint32_t* __restrict__ 
     }
 }
 
+// ---- the 64-byte position/uv stream of the PACKED56 raster pass (m2s_dscene::d_tris_slim) -----------------------------------
+// One thread per output float4 k of triangle t: k < 3 is {P_k, u_k}, k = 3 is {v0, v1, v2, 0}; the values are copied, not computed.
+__global__ void __launch_bounds__(256) slim_tris_kernel(const float4* __restrict__ tris, float4* __restrict__ slim, uint64_t n4) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n4) return;
+    const float4* q = tris + (i >> 2) * 9;
+    const uint32_t k = (uint32_t)i & 3u;
+    float4 o;
+    if (k < 3) {
+        const float4 p = __ldg(q + 3 * k), uv = __ldg(q + 3 * k + 2);
+        o = make_float4(p.x, p.y, p.z, uv.z);
+    } else {
+        o = make_float4(__ldg(q + 2).w, __ldg(q + 5).w, __ldg(q + 8).w, 0.0f);
+    }
+    slim[i] = o;
+}
+
 // ---- v-range of a triangle range per texture (host pipeline: which texture rows must be uploaded before these triangles
 // can be shaded).  minmax: [ntex] sortable-int minima | [ntex] maxima | 1 flag (non-finite or absurd v seen). -----------
 __device__ __forceinline__ int float_key(float f) { const int i = __float_as_int(f); return i ^ ((i >> 31) & 0x7fffffff); }
@@ -289,6 +306,14 @@ m2s_status m2s::scene_upload_impl(m2s_ctx* ctx, const m2s_scene* sc, m2s_dscene*
                                std::min<uint64_t>(first_tris, sc->triangle_count - tri_offset) * (size_t)kTriBytes, cudaMemcpyHostToDevice, ctx->stream));
     if (sc->triangle_count && tri_offset < sc->triangle_count && first_tris)
         d->h2d_bytes += std::min<uint64_t>(first_tris, sc->triangle_count - tri_offset) * (uint64_t)kTriBytes;
+    // a scene uploaded whole gets the 64-byte stream its PACKED56 conversions stage (+64 B per triangle), built here once
+    // behind the copy; a partial or lazy upload would have to build it per chunk and keeps the 144-byte route
+    if (sc->triangle_count && tri_offset == 0 && first_tris >= sc->triangle_count && !lazy_tex) {
+        UP_TRY(dalloc((void**)&d->d_tris_slim, sc->triangle_count * (size_t)kSlimTriBytes));
+        const uint64_t n4 = sc->triangle_count * 4;
+        slim_tris_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, ctx->stream>>>(d->d_tris, d->d_tris_slim, n4);
+        UP_TRY(cudaGetLastError());
+    }
     d->nranges = (uint32_t)ranges.size();
     UP_TRY(dalloc((void**)&d->d_ranges, ranges.size() * sizeof(DRange)));
     if (!ranges.empty())
@@ -344,6 +369,17 @@ M2S_EXPORT m2s_status m2s_scene_upload(m2s_ctx* ctx, const m2s_scene* sc, m2s_ds
 }
 
 M2S_EXPORT uint64_t m2s_scene_h2d_bytes(const m2s_dscene* s) { return s ? s->h2d_bytes : 0; }
+
+// Test aid (not part of m2s.h): copies the scene's 64-byte position/uv stream (4 float4 per triangle) to host memory `dst`;
+// M2S_E_INVALID when the scene has none (partial and lazy uploads)
+M2S_EXPORT m2s_status m2s_debug_scene_slim_tris(m2s_ctx* ctx, const m2s_dscene* s, void* dst) {
+    if (!ctx || !s || !dst) { set_error("m2s_debug_scene_slim_tris: NULL argument"); return M2S_E_INVALID; }
+    if (!s->d_tris_slim) { set_error("m2s_debug_scene_slim_tris: the scene has no slim triangle stream"); return M2S_E_INVALID; }
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    CUDA_TRY(cudaMemcpyAsync(dst, s->d_tris_slim, s->ntri * (size_t)kSlimTriBytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return M2S_OK;
+}
 
 M2S_EXPORT m2s_status m2s_scene_read_mip(m2s_ctx* ctx, const m2s_dscene* s, uint32_t texture, uint32_t level, uint8_t* dst,
                                          uint32_t* width, uint32_t* height) {
