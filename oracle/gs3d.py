@@ -89,11 +89,22 @@ def decode(records, layout: int, std_dev: float = 1.0):
 
 
 def graphdeco_forward(pos, scale, rot, colour, opacity, world_to_view, view_to_clip, width: int, height: int, near: float,
-                      scale_modifier: float = 1.0, background=(0.0, 0.0, 0.0), model_to_world=None):
+                      scale_modifier: float = 1.0, background=(0.0, 0.0, 0.0), model_to_world=None, power_err=None, mean_err=None,
+                      render: bool = True):
     """preprocessCUDA + renderCUDA in fp64 with an OpenCV camera made from the GL one (the view matrix's y and z rows
     negated, y_ndc negated), row 0 at the top.  Returns (per gaussian: dict of u, v (GL pixel frame), conic, radius,
     depth, alive, rect), and the image (H, W, 4) flipped to row 0 at the bottom, plus per pixel the smallest margin of any
-    alpha to 1/255, 0.99 and the 1e-4 stop, and whether the pixel's set of gaussians depends on the tile rectangles."""
+    alpha to 1/255, 0.99 and the 1e-4 stop, and whether the pixel's set of gaussians depends on the tile rectangles:
+    whether a gaussian that reaches it (power <= 0, alpha >= 1/255) lies outside its rectangle in either convention's
+    rows, OpenCV's (counted from the top, the ones composited here) or GL's (from the bottom, the checker's).
+
+    For error bounds the dict also holds, per gaussian, cov (a, b, c: the dilated 2-D covariance, GL frame) and mag
+    (|T|_F^2 (s_x^2 + s_y^2 + s_z^2) + 0.3: the size of the terms cov is summed from), and per pixel (flipped like the
+    image) blended (the number of terms composited) and dalpha: the sum over those terms of T alpha (power_err |power| +
+    mean_err |grad_mean power|), power_err and mean_err being per-gaussian relative and absolute (pixel) error bounds of
+    the power's quadratic form and of the mean (default 0): to first order, the largest change of any output channel
+    those errors can make, in units of max(colour, background).  render False: the per-gaussian dict alone (then the
+    image, margin and rectangle flags are None and the dict has no per-pixel entries)."""
     V = np.asarray(world_to_view, np.float64).reshape(4, 4).T
     M = np.eye(4) if model_to_world is None else np.asarray(model_to_world, np.float64).reshape(4, 4).T
     P = np.asarray(view_to_clip, np.float64).reshape(4, 4).T
@@ -142,6 +153,11 @@ def graphdeco_forward(pos, scale, rot, colour, opacity, world_to_view, view_to_c
     rect = np.stack([np.clip(((u - radius) / 16).astype(np.int64), 0, gx), np.clip(((vcv - radius) / 16).astype(np.int64), 0, gy),
                      np.clip(((u + radius + 15) / 16).astype(np.int64), 0, gx), np.clip(((vcv + radius + 15) / 16).astype(np.int64), 0, gy)], -1)
     alive &= (rect[:, 2] - rect[:, 0]) * (rect[:, 3] - rect[:, 1]) != 0
+    mag = (T ** 2).sum(axis=(1, 2)) * (s ** 2).sum(axis=1) + 0.3
+    info = {"u": u, "v": height - 1.0 - vcv, "conic": conic * np.array([1.0, -1.0, 1.0]), "radius": radius, "depth": z, "alive": alive,
+            "rect": rect, "cov": np.stack([a, -b, c], -1), "mag": mag}
+    if not render:
+        return info, None, None, None
     order = sorted(np.nonzero(alive)[0], key=lambda i: (z[i], i))
     col = np.maximum(np.asarray(colour, np.float64), 0.0)
     op = np.asarray(opacity, np.float64)
@@ -152,14 +168,24 @@ def graphdeco_forward(pos, scale, rot, colour, opacity, world_to_view, view_to_c
     C_ = np.zeros((height, width, 3))
     done = np.zeros((height, width), bool)
     rect_dep = np.zeros((height, width), bool)
+    blended = np.zeros((height, width), np.int64)
+    dalpha = np.zeros((height, width))
+    perr = np.zeros(n) if power_err is None else np.broadcast_to(np.asarray(power_err, np.float64), (n,))
+    merr = np.zeros(n) if mean_err is None else np.broadcast_to(np.asarray(mean_err, np.float64), (n,))
     tile_x, tile_y = (xs // 16).astype(np.int64), (ys // 16).astype(np.int64)
+    # the rows of the rectangles in the GL frame the checker bins in (rows counted from the bottom)
+    tile_gl = ((height - 1 - ys) // 16).astype(np.int64)
+    vgl = height - 1.0 - vcv
+    rect_gl = np.stack([np.clip(((vgl - radius) / 16).astype(np.int64), 0, gy), np.clip(((vgl + radius + 15) / 16).astype(np.int64), 0, gy)], -1)
     for i in order:
         dx, dy = u[i] - xs, vcv[i] - ys
         power = -0.5 * (conic[i, 0] * dx * dx + conic[i, 2] * dy * dy) - conic[i, 1] * dx * dy
+        grad = np.hypot(conic[i, 0] * dx + conic[i, 1] * dy, conic[i, 1] * dx + conic[i, 2] * dy)
         al = np.minimum(0.99, op[i] * np.exp(power))
         in_rect = (tile_x >= rect[i, 0]) & (tile_x < rect[i, 2]) & (tile_y >= rect[i, 1]) & (tile_y < rect[i, 3])
+        in_gl = (tile_x >= rect[i, 0]) & (tile_x < rect[i, 2]) & (tile_gl >= rect_gl[i, 0]) & (tile_gl < rect_gl[i, 1])
         use = (power <= 0) & (al >= 1.0 / 255.0)
-        rect_dep |= use & ~in_rect & ~done
+        rect_dep |= use & ~(in_rect & in_gl) & ~done
         use &= in_rect & ~done
         tt = T_ * (1 - al)
         stop = use & (tt < 1e-4)
@@ -170,8 +196,10 @@ def graphdeco_forward(pos, scale, rot, colour, opacity, world_to_view, view_to_c
         done |= stop
         add = use & ~stop
         C_ += np.where(add[..., None], col[i] * (al * T_)[..., None], 0.0)
+        blended += add
+        dalpha += np.where(add, T_ * al * (perr[i] * np.abs(power) + merr[i] * grad), 0.0)
         T_ = np.where(add, tt, T_)
     img[..., :3] = C_ + T_[..., None] * np.asarray(background, np.float64)
     img[..., 3] = 1.0 - T_
-    info = {"u": u, "v": height - 1.0 - vcv, "conic": conic * np.array([1.0, -1.0, 1.0]), "radius": radius, "depth": z, "alive": alive}
+    info.update(blended=blended[::-1].copy(), dalpha=dalpha[::-1].copy())
     return info, img[::-1].copy(), margin[::-1].copy(), rect_dep[::-1].copy()
