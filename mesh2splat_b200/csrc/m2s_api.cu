@@ -53,9 +53,7 @@ static m2s_status ctx_init(m2s_ctx* c) {
     uint64_t thresh = UINT64_MAX;  // keep freed blocks cached: uploads in steady state never hit cudaMalloc
     CUDA_TRY(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thresh));
     CUDA_TRY(cudaMalloc(&c->d_sched, 8 * 128));
-    CUDA_TRY(cudaMalloc(&c->d_counter, sizeof(unsigned long long)));
     CUDA_TRY(cudaMalloc(&c->d_total, sizeof(unsigned long long)));
-    CUDA_TRY(cudaMalloc(&c->d_nitems, sizeof(uint32_t)));
     CUDA_TRY(cudaMallocHost(&c->h_total, sizeof(unsigned long long)));
     CUDA_TRY(cudaHostAlloc(&c->h_status, sizeof(uint32_t), cudaHostAllocMapped));
     *c->h_status = 0;
@@ -103,7 +101,7 @@ M2S_EXPORT void m2s_ctx_destroy(m2s_ctx* c) {
     for (Scratch* s : c->all_scratch()) if (s->p) cudaFreeAsync(s->p, c->stream);
     cudaStreamSynchronize(c->stream);
     if (c->d_prepass_valid) cudaFree(c->d_prepass_valid);
-    cudaFree(c->d_sched); cudaFree(c->d_counter); cudaFree(c->d_total); cudaFree(c->d_nitems);
+    cudaFree(c->d_sched); cudaFree(c->d_total);
     if (c->h_total) cudaFreeHost(c->h_total);
     if (c->h_status) cudaFreeHost(c->h_status);
     for (int i = 0; i < 2; ++i) if (c->h_stage[i]) cudaFreeHost(c->h_stage[i]);

@@ -140,9 +140,8 @@ m2s_status m2s::convert_enqueue_impl(m2s_ctx* ctx, const m2s_dscene* s, const m2
     m2s_status st = grow(ctx, ctx->trifrag, std::max<uint64_t>(tr.count, 1) * tri_frag_bytes(klayout), stream);
     if (st == M2S_OK) st = grow(ctx, ctx->items, pl.queue_cap * sizeof(FragItem), stream);
     if (st != M2S_OK) return st;
-    if (ctx->dirty) {
+    if (ctx->dirty) {  // both scheduler sets
         CUDA_TRY(cudaMemsetAsync(ctx->d_sched, 0, 8 * 128, stream));
-        CUDA_TRY(cudaMemsetAsync(ctx->d_counter, 0, sizeof(unsigned long long), stream));
         ctx->dirty = false;
     }
     ConvertArgs a;
@@ -164,11 +163,16 @@ m2s_status m2s::convert_enqueue_impl(m2s_ctx* ctx, const m2s_dscene* s, const m2
     a.queue_cap = (uint32_t)pl.queue_cap;
     a.item_max_frags = (uint32_t)pl.item_max;
     a.flush_frags = (uint32_t)pl.flush_frags;
-    a.n_items_out = ctx->d_nitems;
     a.out = (uint8_t*)d_out;
     a.cap = pl.cap;
     a.keys = (unsigned long long*)d_keys;
-    a.counter = ctx->d_counter;
+    // the scheduler set of this launch, {unit counter, packed counter} at lines {2 s, 2 s + 1} of d_sched, and the next's
+    auto set_claim = [&](uint32_t s) { return ctx->d_sched + 2 * s * kSchedStride; };
+    auto set_counter = [&](uint32_t s) { return reinterpret_cast<unsigned long long*>(ctx->d_sched + (2 * s + 1) * kSchedStride); };
+    a.claim = set_claim(ctx->sched_parity);
+    a.counter = set_counter(ctx->sched_parity);
+    a.next_claim = set_claim(ctx->sched_parity ^ 1u);
+    a.next_counter = set_counter(ctx->sched_parity ^ 1u);
     // fused gather: the raster kernel's count stays local, the global total goes to d_total after the wait
     a.total_out = (peers && peers->world > 1) ? ctx->d_total : (d_total ? (unsigned long long*)d_total : ctx->d_total);
     a.prev_totals = prev_totals;
@@ -192,6 +196,7 @@ m2s_status m2s::convert_enqueue_impl(m2s_ctx* ctx, const m2s_dscene* s, const m2
     const int fgrid = ctx->sm_count * ctx->frag_blocks_per_sm[klayout];
     cudaError_t e = convert_launch(klayout, a, (int)pl.grid, fgrid, stream, mid);
     if (e != cudaSuccess) { ctx->dirty = true; set_error(std::string("convert launch: ") + cudaGetErrorString(e)); return M2S_E_CUDA; }
+    ctx->sched_parity ^= 1u;   // this launch's fragment kernel zeroes the other set
     if (peers && peers->world > 1)
         CUDA_TRY(gather_wait_launch((const unsigned long long*)peers->xch[peers->rank], peers->world, a.epoch, out_capacity,
                                     (unsigned long long*)d_total, ctx->d_status, stream));
@@ -294,7 +299,7 @@ m2s_status cuda_status(const char* what, cudaError_t e) {
 // stream by the reduction of its v-range per texture and an 8-byte-per-texture copy back.  (2) Per chunk, as soon as its
 // v-range is on the host: the texture row groups it samples (not yet resident) go up on the texture stream, and the
 // compute stream (the context's) generates their mip rows and runs the two kernels.  (3) A chunk's records start
-// crossing PCIe on the download stream as soon as its count has arrived (zero-copy, from the raster kernel's last CTA),
+// crossing PCIe on the download stream as soon as its count has arrived (zero-copy, from the fragment kernel as it starts),
 // while later chunks are still being uploaded and converted.  The first records exist after ~1/nchunks of the upload; a
 // shard (first_triangle/triangle_count) never uploads texture rows it does not sample.
 struct HostConvert {

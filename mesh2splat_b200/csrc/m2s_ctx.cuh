@@ -71,10 +71,10 @@ struct m2s_ctx {
     int device = 0;
     int sm_count = 0;
     cudaStream_t stream = nullptr;
-    uint32_t* d_sched = nullptr;             // 8 x 128 B (one scheduler word per cache line)
-    unsigned long long* d_counter = nullptr; // running fragment counter
+    uint32_t* d_sched = nullptr;             // 8 x 128 B (one scheduler word per cache line): the scheduler sets {unit counter,
+                                             // packed fragment | item counter} at lines {0, 1} and {2, 3}, line 6 the fused
+                                             // gather's finished fragment CTAs (ConvertArgs)
     unsigned long long* d_total = nullptr;   // published count
-    uint32_t* d_nitems = nullptr;            // work items queued by the last raster launch
     uint32_t* d_prepass_valid = nullptr;     // counter of the synchronous m2s_prepass
     unsigned long long* h_total = nullptr;   // pinned
     uint32_t* h_status = nullptr;            // pinned + mapped: raised by device-side waits that timed out (fused gather)
@@ -91,6 +91,7 @@ struct m2s_ctx {
     int frag_blocks_per_sm[kLayouts] = {};  // fragment kernel
     unsigned long long epoch = 0;            // pairs up the ranks' calls of the fused gather
     bool dirty = true;                       // scheduler state needs a memset before the next launch
+    uint32_t sched_parity = 0;               // the scheduler set the next launch uses; its fragment kernel zeroes the other
     // scratch owned by the context (grown on demand)
     m2s::Scratch out, keys;                  // convert_host output and keys
     m2s::Scratch trifrag, items;             // between the raster and the fragment kernel: TriRec per triangle, FragItem queue

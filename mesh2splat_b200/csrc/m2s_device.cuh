@@ -18,7 +18,12 @@ constexpr uint32_t kDeferUnitBlocks = 24; // a work unit whose larger triangles 
 constexpr uint32_t kDeferBlocks = 4;      // row blocks per help-queue entry
 constexpr uint32_t kMaxSplit = 64;       // queue slots one oversized row block can take (item_max_frags >= R / 2)
 constexpr unsigned long long kFragMask = (1ull << 40) - 1;  // ConvertArgs::counter: fragments | queue slots << 40
+constexpr int kSchedStride = 32;        // scheduler words live on separate 128-byte lines (m2s_ctx::d_sched)
 constexpr float kGuard = 8192.0f;        // window-coordinate guard band (|xw| beyond -> triangle dropped)
+// M2S_TRACE builds (scripts/trace_raster.py): the trace buffer starts with a header, then the raster warps' slots
+constexpr int kTraceHeader = 32;
+constexpr int kTraceWarpSlots = 32;
+constexpr int kTrFragEndNs = 0;          // header word: globaltimer when the fragment kernel's last CTA ended
 #ifndef M2S_DIRECT_MAX
 #define M2S_DIRECT_MAX 512   // a unit whose small triangles emit at most this many fragments is shaded by the raster kernel itself (<= 1024)
 #endif
@@ -101,26 +106,32 @@ struct ConvertArgs {
     uint32_t queue_cap;
     uint32_t item_max_frags;           // a row block with more fragments is cut into items of this size (multiple of 32)
     uint32_t flush_frags;              // pending row blocks become one item once they hold this many fragments
-    uint32_t* n_items_out;             // items queued by this launch (published by the raster kernel's last CTA)
     uint8_t* out;
     unsigned long long cap;
     unsigned long long* keys;          // optional
     unsigned long long* counter;       // low 40 bits: fragments generated (the reference's atomic counter), high 24 bits:
-                                       // work items queued; context-owned, zero at launch, re-zeroed by the last CTA
-    unsigned long long* total_out;     // receives the final count (last CTA out)
+                                       // work items queued; this launch's scheduler set (below), final when the fragment
+                                       // kernel starts: every CTA reads its item count there
+    unsigned long long* total_out;     // receives the final count (the fragment kernel's CTA 0)
     const unsigned long long* prev_totals;  // appended launches: counts of the earlier chunks (records start after them)
     uint32_t nprev;
-    unsigned long long* host_total;    // optional, mapped pinned host memory: {count, tag} written by the raster kernel's
-    unsigned long long host_tag;       // last CTA so the host can size the download while the fragment kernel still runs
-    // scheduling state (zero at launch, re-armed by the last CTA)
-    uint32_t* sched;                   // words 128 B apart: 0 unit counter, 4 raster CTAs finished, 6 fragment CTAs finished
-                                       // (fused gather)
+    unsigned long long* host_total;    // optional, mapped pinned host memory: {count, tag} written by the fragment kernel's
+    unsigned long long host_tag;       // CTA 0 as it starts, so the host can size the download while the kernel still runs
+    // scheduling state: two sets {unit counter, packed counter} in the context, alternated by launch (m2s_ctx::sched_parity).
+    // This launch's set is zero at launch; its fragment kernel zeroes the other set for the next launch, which starts only
+    // once this launch's fragment kernel has ended (stream order: the raster kernel is launched without PDL)
+    uint32_t* claim;                   // this launch's unit counter (the set of `counter`)
+    uint32_t* next_claim;              // the next launch's set, zeroed by this launch's fragment kernel
+    unsigned long long* next_counter;
+    uint32_t* sched;                   // words 128 B apart (SCHED): 6 fragment CTAs finished (fused gather); SCHED 0-3 are
+                                       // the two sets (m2s_ctx::d_sched)
     uint32_t unit_tris;                // triangles per work unit (<= 32), chosen by the host for balance
     uint32_t n_units;
     uint32_t direct_ok;                // the raster kernel may shade light units itself (ConvertPlan::direct_ok)
     uint32_t claim_late;               // ... and claims its next unit once the current one is done (ConvertPlan::claim_late)
     uint32_t pair_first;               // a warp's first pass sets up units 2g and 2g + 1 on its two half warps (ConvertPlan::pair_first)
-    unsigned long long* trace;         // M2S_TRACE builds only: 16 per-phase sums per raster warp (TraceSlot)
+    unsigned long long* trace;         // M2S_TRACE builds only: kTraceHeader words (kTrFragEndNs), then kTraceWarpSlots
+                                       // per raster warp (TraceSlot, m2s_raster.cu)
     // multi-GPU fused gather (world <= 1: off).  peer_out[p] / peer_xch[p] are rank p's final buffer and
     // exchange block mapped into this process (NVLink peer memory); every rank's fragment kernel stores its
     // records into ALL final buffers at its global offset.  xch block: [kMaxPeers][4] u64 =

@@ -69,6 +69,26 @@ __device__ __noinline__ void micro_item(const ConvertArgs& a, uint32_t it, uint4
     __syncwarp();
 }
 
+// Thread 0 of CTA 0, once the raster grid has ended: the launch's count -> total_out, the host's mapped slot and (fused
+// gather) every peer, before any CTA waits for the peers' counts; then the other scheduler set is zeroed for the next
+// launch (ConvertArgs::next_claim).  Out of line: the kernel's other threads never run it.
+__device__ __noinline__ void publish_counts(const ConvertArgs& a, unsigned long long tot) {
+    *a.total_out = tot;
+    if (a.host_total) {  // zero-copy count for the host (PCIe posted write, ~1 us): the count is ordered before its tag
+        *reinterpret_cast<volatile unsigned long long*>(a.host_total) = tot;
+        __threadfence_system();
+        *reinterpret_cast<volatile unsigned long long*>(a.host_total + 1) = a.host_tag;
+    }
+    if (a.world > 1) {  // fused gather: tell every peer how many records this rank will write
+        const unsigned long long mine = tot < a.cap ? tot : a.cap;
+        for (uint32_t p = 0; p < a.world; ++p) a.peer_xch[p][a.rank * 4 + 0] = mine;
+        __threadfence_system();
+        for (uint32_t p = 0; p < a.world; ++p) st_release_sys(a.peer_xch[p] + a.rank * 4 + 1, a.epoch);
+    }
+    *a.next_claim = 0;
+    *a.next_counter = 0ull;
+}
+
 template <int LAYOUT>
 __global__ void __launch_bounds__(kFragThreads, (LAYOUT == 1 ? M2S_FRAG_THREADS_P56 : 512) / kFragThreads) fragment_kernel(const __grid_constant__ ConvertArgs a) {
     using S = FragSmem<LAYOUT>;
@@ -86,9 +106,28 @@ __global__ void __launch_bounds__(kFragThreads, (LAYOUT == 1 ? M2S_FRAG_THREADS_
         fence_barrier_init();
     }
     __syncthreads();
+    // ---- the item pipeline: header + block list of item i+1 are loaded while item i is processed ----
+    struct Hdr { uint4 h0; uint2 h1; uint2 blk; };
+    auto load_hdr = [&](uint32_t it, uint32_t bound) {
+        Hdr h;
+        h.h0 = make_uint4(0, 0, 0, 0); h.h1 = make_uint2(0, 0); h.blk = make_uint2(0xffffffffu, 0);
+        if (it < bound) {
+            const FragItem* q = a.items + it;
+            h.h0 = __ldg(reinterpret_cast<const uint4*>(q));
+            h.h1 = __ldg(reinterpret_cast<const uint2*>(q) + 2);
+            if (!(h.h0.w & 0x80000000u) && (uint32_t)lane < (h.h0.w & 0xffu)) h.blk = __ldg(reinterpret_cast<const uint2*>(q->blocks + lane));
+        }
+        return h;
+    };
     // launched with programmatic stream serialisation: the CTAs of this grid are placed while the raster
     // kernel drains; everything it wrote is visible after this wait
     asm volatile("griddepcontrol.wait;" ::: "memory");
+    // the first header is loaded together with the packed counter (one global round trip instead of two before the first
+    // TMA): whatever an unused queue slot holds is discarded by the loop condition
+    Hdr cur = load_hdr(blockIdx.x, a.queue_cap);
+    const unsigned long long packed = *reinterpret_cast<const volatile unsigned long long*>(a.counter);
+    const uint32_t nitems = min((uint32_t)(packed >> 40), a.queue_cap);   // work items queued
+    if (blockIdx.x == 0 && threadIdx.x == 0) publish_counts(a, packed & kFragMask);
     const OutRange out = out_range(a);
     const unsigned long long base = out.base, room = out.room;
     // fused gather: wait for every rank's count of this epoch, my records start after the lower ranks'
@@ -107,19 +146,6 @@ __global__ void __launch_bounds__(kFragThreads, (LAYOUT == 1 ? M2S_FRAG_THREADS_
         goff = s_goff;
     }
     const uint32_t* __restrict__ texb = a.tex_base;
-    // ---- the item pipeline: header + block list of item i+1 are loaded while item i is processed ----
-    struct Hdr { uint4 h0; uint2 h1; uint2 blk; };
-    auto load_hdr = [&](uint32_t it, uint32_t bound) {
-        Hdr h;
-        h.h0 = make_uint4(0, 0, 0, 0); h.h1 = make_uint2(0, 0); h.blk = make_uint2(0xffffffffu, 0);
-        if (it < bound) {
-            const FragItem* q = a.items + it;
-            h.h0 = __ldg(reinterpret_cast<const uint4*>(q));
-            h.h1 = __ldg(reinterpret_cast<const uint2*>(q) + 2);
-            if (!(h.h0.w & 0x80000000u) && (uint32_t)lane < (h.h0.w & 0xffu)) h.blk = __ldg(reinterpret_cast<const uint2*>(q->blocks + lane));
-        }
-        return h;
-    };
     auto live = [&](const Hdr& h) {  // uniform over the CTA: does the item emit anything?
         const unsigned long long first = item_first(h.h0.x, h.h0.y);
         return h.h1.y > h.h1.x && first + h.h1.x < room;
@@ -138,10 +164,6 @@ __global__ void __launch_bounds__(kFragThreads, (LAYOUT == 1 ? M2S_FRAG_THREADS_
     constexpr uint32_t buf = 0;
     // one header in flight per CTA: the other resident CTAs of the SM hide the load (a software pipeline over the queue
     // was measured: no gain, 16 more registers in the shading loop)
-    // the first header is loaded together with the item count (one global round trip instead of two before the first
-    // TMA): whatever an unused queue slot holds is discarded by the loop condition
-    Hdr cur = load_hdr(blockIdx.x, a.queue_cap);
-    const uint32_t nitems = min(*reinterpret_cast<const volatile uint32_t*>(a.n_items_out), a.queue_cap);
     for (uint32_t it = blockIdx.x; it < nitems; it += gridDim.x, cur = load_hdr(it, nitems)) {
         if (!live(cur)) continue;
         if (cur.h0.w & kItMicro) {
@@ -262,6 +284,10 @@ __global__ void __launch_bounds__(kFragThreads, (LAYOUT == 1 ? M2S_FRAG_THREADS_
             }
         }
     }
+#ifdef M2S_TRACE
+    __syncthreads();   // the end of the step as scripts/trace_raster.py places it: the last CTA's last record written
+    if (a.trace && threadIdx.x == 0) atomicMax(a.trace + kTrFragEndNs, gtimer_ns());
+#endif
 }
 
 // waits until every rank's records of this epoch have landed in THIS rank's final buffer, publishes the

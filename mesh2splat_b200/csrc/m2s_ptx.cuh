@@ -97,7 +97,6 @@ __device__ __forceinline__ bool wait_epoch(const unsigned long long* flag, unsig
     }
     return true;
 }
-constexpr int kSchedStride = 32;  // scheduler words live on separate 128-byte lines
 #define SCHED(a, i) ((a).sched + (i) * kSchedStride)
 
 }  // namespace m2s

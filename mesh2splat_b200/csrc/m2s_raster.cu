@@ -44,15 +44,18 @@
 
 namespace m2s {
 
-// M2S_TRACE builds: per-warp SUMS over all the warp's units, 16 slots per raster warp (scripts/trace_raster.py).
-// Phases are clock64() deltas (SM cycles: the globaltimer ticks too coarsely for one unit); TR_PHASE adds the cycles
-// since the previous mark to its slot.  Fire-and-forget atomics: the trace adds no wait to the chain it measures.
+// M2S_TRACE builds: per-warp SUMS over all the warp's units, kTraceWarpSlots slots per raster warp after the trace's
+// header (scripts/trace_raster.py).  Phases are clock64() deltas (SM cycles: the globaltimer ticks too coarsely for one
+// unit); TR_PHASE adds the cycles since the previous mark to its slot.  The three *Ns slots are absolute globaltimer
+// stamps (entry, unit-loop exit, exit) that place the warps' work inside the launch.  Fire-and-forget atomics: the
+// trace adds no wait to the chain it measures.
 enum TraceSlot {
     kTrLoadWait, kTrSetup, kTrWalkScan, kTrLarger, kTrReserve, kTrList, kTrShade, kTrUnitEnd, kTrTail,
-    kTrUnits, kTrDirectUnits, kTrGroups, kTrCycles, kTrNanos, kTrEntry
+    kTrUnits, kTrDirectUnits, kTrGroups, kTrCycles, kTrNanos, kTrEntry, kTrEntryNs, kTrLoopExitNs, kTrExitNs
 };
+static_assert(kTrExitNs < kTraceWarpSlots, "trace slots per raster warp");
 #ifdef M2S_TRACE
-#define TR_SLOT(s) (((size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * 16 + (s))
+#define TR_SLOT(s) (kTraceHeader + ((size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * kTraceWarpSlots + (s))
 #define TR_PHASE(a, s) do { const long long n_ = clock64(); if ((a).trace && (threadIdx.x & 31) == 0) atomicAdd((a).trace + TR_SLOT(s), (unsigned long long)(n_ - tr_prev_)); tr_prev_ = n_; } while (0)
 #define TR_ADD(a, s, v) do { if ((a).trace && (threadIdx.x & 31) == 0) atomicAdd((a).trace + TR_SLOT(s), (unsigned long long)(v)); } while (0)
 #else
@@ -736,45 +739,6 @@ __device__ __forceinline__ void help_cta(const ConvertArgs& a, unsigned char* sm
     }
 }
 
-// the last CTA out publishes the counts and re-arms the scheduler for the next launch
-__device__ __forceinline__ void raster_last_cta(const ConvertArgs& a, int warp, int lane) {
-    __syncthreads();
-    if (warp == 0) {
-        uint32_t last = 0;
-        unsigned long long tot = 0;
-        if (lane == 0) {
-            __threadfence();
-            const uint32_t done = atomicAdd(SCHED(a, 4), 1u);
-            if (done == gridDim.x - 1) {
-                __threadfence();
-                last = 1;
-                const unsigned long long packed = *reinterpret_cast<volatile unsigned long long*>(a.counter);
-                tot = packed & kFragMask;                       // fragments generated
-                *a.total_out = tot;
-                *a.n_items_out = (uint32_t)(packed >> 40);      // work items queued
-                *a.counter = 0ull;
-                if (a.host_total) {  // zero-copy count for the host (PCIe posted write, ~1 us)
-                    *reinterpret_cast<volatile unsigned long long*>(a.host_total) = tot;
-                    __threadfence_system();
-                    *reinterpret_cast<volatile unsigned long long*>(a.host_total + 1) = a.host_tag;
-                }
-                *SCHED(a, 0) = 0; *SCHED(a, 4) = 0;
-                __threadfence();
-            }
-        }
-        if (a.world > 1) {  // fused gather: tell every peer how many records this rank will write, one lane per peer
-            last = __shfl_sync(0xffffffffu, last, 0);
-            tot = __shfl_sync(0xffffffffu, tot, 0);
-            if (last && (uint32_t)lane < a.world) {
-                const unsigned long long mine = tot < a.cap ? tot : a.cap;
-                a.peer_xch[lane][a.rank * 4 + 0] = mine;
-                __threadfence_system();
-                st_release_sys(a.peer_xch[lane] + a.rank * 4 + 1, a.epoch);
-            }
-        }
-    }
-}
-
 // ------------------------------------------------------------------------------------------
 // raster_kernel
 // ------------------------------------------------------------------------------------------
@@ -817,7 +781,7 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         mbar_arrive_expect_tx(&wb.bar, bytes);
         tma_load_1d(wb.tri, src + ((size_t)a.tri_first + t0) * tri_size(), bytes, &wb.bar);
     };
-    auto claim = [&]() { return claim_base + atomicAdd(SCHED(a, 0), 1u); };   // lane 0 only: the next unit
+    auto claim = [&]() { return claim_base + atomicAdd(a.claim, 1u); };   // lane 0 only: the next unit
     // ref_logf's table for the direct path's opacities -> the warp's slice, as an asynchronous copy that lands while the
     // first unit is set up (waited for before the first shading; a CTA-wide copy would wait at the barrier below: ~1 us
     // more per warp, measured on the H100)
@@ -1020,14 +984,24 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         pair = false;
         TR_PHASE(a, kTrUnitEnd);
     }
+#ifdef M2S_TRACE
+    const unsigned long long tr_loop_ns_ = gtimer_ns();
+#endif
     help_cta<RK>(a, smem, wb, st, cq, shade, lane);
+    // no CTA barrier and no grid-wide count at the end: each warp exits once its own bulk stores are complete.  A warp
+    // that shades from another warp's slice is done before the help queue lets that slice be rewritten, and shared
+    // memory lives until the CTA ends.  The fragment kernel reads the counts once this grid has ended (griddepcontrol.wait)
+    // and re-arms the scheduler there
     if (lane == 0) tma_store_wait_all();  // record stores are complete (not just read) before the kernel ends
     if constexpr (kDirectOK) cp_async_wait_all();   // a warp without a direct unit never waited for its wb.logtab
-    raster_last_cta(a, warp, lane);
 #ifdef M2S_TRACE
     TR_PHASE(a, kTrTail);
     TR_ADD(a, kTrCycles, clock64() - tr_c0_);   // with kTrNanos: the SM clock the cycles convert at
-    TR_ADD(a, kTrNanos, gtimer_ns() - tr_ns0_);
+    const unsigned long long tr_exit_ns_ = gtimer_ns();
+    TR_ADD(a, kTrNanos, tr_exit_ns_ - tr_ns0_);
+    TR_ADD(a, kTrEntryNs, tr_ns0_);
+    TR_ADD(a, kTrLoopExitNs, tr_loop_ns_);
+    TR_ADD(a, kTrExitNs, tr_exit_ns_);
 #endif
 }
 
