@@ -697,6 +697,42 @@ m2s_status m2s_3dgs_render_enqueue(m2s_ctx* ctx, const void* d_records, uint64_t
 m2s_status m2s_3dgs_render(m2s_ctx* ctx, const void* d_records, uint64_t count, const m2s_3dgs_params* params, const float* d_sh,
                            uint32_t buffer_degree, uint32_t sh_degree, float* d_rgba32f, uint8_t* d_rgba8, uint64_t* pairs);
 
+/* ---- the standard 3DGS render's backward pass (beyond the reference) ---------------------------------------------------
+ * graphdeco's backward pass (diff-gaussian-rasterization's renderCUDA / preprocessCUDA backward) for PACKED56 records, so
+ * that converted gaussians can be refined against images.  A forward pass that keeps its state writes the same image,
+ * pair count and drawn prefix as m2s_3dgs_render_enqueue on the same records, bit for bit, and keeps in the state what the
+ * backward pass needs: the splat records, the depth ranks, the sorted pairs and tile runs, and per pixel the final
+ * transmittance and its last contributing gaussian.  Several states can hold several views' forward passes at once.
+ * DESIGN §2 fixes every fp32 operation and the summation order (no floating-point atomics), so two backward calls on the
+ * same inputs give identical bits.  Conventions (graphdeco's): the 0.99 alpha clamp passes the gradient as if unclamped;
+ * gaussians skipped below 1/255 or past a pixel's stop contribute nothing; the 1.3 tan(fov / 2) clamp of the view x or y
+ * zeroes that component; a colour clamped at 0 gets no gradient; an infinite opacity logit gets 0 (the other fields
+ * still get theirs), and a record whose logit is NaN gets a row of zeros. */
+typedef struct m2s_3dgs_state m2s_3dgs_state;
+/* A state of ctx's device, empty.  Its memory grows stream-ordered on the stream of the forward pass that needs it, so
+ * reusing a state across iterations allocates nothing.  Destroy it before its context. */
+m2s_status m2s_3dgs_state_create(m2s_ctx* ctx, m2s_3dgs_state** out);
+void m2s_3dgs_state_destroy(m2s_3dgs_state* state);
+/* Enqueue-only forward pass keeping its state: d_params count x 14 floats (PACKED56, 16-byte aligned), params->layout
+ * M2S_LAYOUT_PACKED56, one RGBA32F target (16-byte aligned); max_pairs, d_pairs and d_drawn as m2s_3dgs_render_enqueue.
+ * M2S_E_INVALID before any launch, with nothing written, for another layout, a NULL state or target, a misaligned
+ * buffer, a state of another device, or anything m2s_3dgs_render_enqueue rejects.  Replaces the state's last forward. */
+m2s_status m2s_3dgs_render_grad_enqueue(m2s_ctx* ctx, m2s_3dgs_state* state, const float* d_params, uint64_t count,
+                                        const m2s_3dgs_params* params, float* d_rgba32f, uint64_t max_pairs, uint64_t* d_pairs,
+                                        uint32_t* d_drawn, void* stream);
+/* Synchronous form on the context stream: counts the pairs, reads the count back once and draws every survivor. */
+m2s_status m2s_3dgs_render_grad(m2s_ctx* ctx, m2s_3dgs_state* state, const float* d_params, uint64_t count,
+                                const m2s_3dgs_params* params, float* d_rgba32f, uint64_t* pairs);
+/* Enqueue-only backward pass of the state's last forward pass: d_grad_rgba32f dL/d(image), width x height x 4 floats
+ * (16-byte aligned); d_grad_params count x 14 floats (4-byte aligned), written whole: dL/d(xyz, quaternion wxyz, log-scale,
+ * SH0, opacity logit).  Culled records, records past the drawn prefix and records with a NaN logit get rows of zeros.  d_params and params must be
+ * those of the forward pass.  M2S_E_INVALID before any launch, with nothing written, for another layout, a NULL or
+ * misaligned buffer, a state that holds no forward pass, a count or size that differs from the state's forward pass, or
+ * anything m2s_3dgs_render_enqueue rejects.  Scratch (36 B per pair of the budget) is stream-ordered context memory grown
+ * on `stream` (NULL = context stream); nothing is synchronised. */
+m2s_status m2s_3dgs_backward_enqueue(m2s_ctx* ctx, const m2s_3dgs_state* state, const float* d_params, uint64_t count,
+                                     const m2s_3dgs_params* params, const float* d_grad_rgba32f, float* d_grad_params, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

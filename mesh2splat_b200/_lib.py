@@ -27,6 +27,8 @@ SYMBOLS = [
     "m2s_ply_parse_header", "m2s_ply_decode_enqueue", "m2s_ply_read", "m2s_ply_h2d_bytes",
     "m2s_ply_decode_sh_enqueue", "m2s_ply_read_sh", "m2s_prepass_sh", "m2s_prepass_sh_enqueue",
     "m2s_image_compare", "m2s_image_compare_enqueue", "m2s_3dgs_render", "m2s_3dgs_render_enqueue",
+    "m2s_3dgs_state_create", "m2s_3dgs_state_destroy", "m2s_3dgs_render_grad", "m2s_3dgs_render_grad_enqueue",
+    "m2s_3dgs_backward_enqueue",
 ]
 
 
@@ -171,6 +173,16 @@ def lib() -> C.CDLL:
     L.m2s_3dgs_render_enqueue.argtypes = [vp, vp, u64, vp, C.POINTER(_abi.m2s_3dgs_params), vp, u32, u32, vp, vp, u64, vp, vp, vp]
     L.m2s_3dgs_render.restype = i32
     L.m2s_3dgs_render.argtypes = [vp, vp, u64, C.POINTER(_abi.m2s_3dgs_params), vp, u32, u32, vp, vp, C.POINTER(u64)]
+    L.m2s_3dgs_state_create.restype = i32
+    L.m2s_3dgs_state_create.argtypes = [vp, C.POINTER(vp)]
+    L.m2s_3dgs_state_destroy.restype = None
+    L.m2s_3dgs_state_destroy.argtypes = [vp]
+    L.m2s_3dgs_render_grad_enqueue.restype = i32
+    L.m2s_3dgs_render_grad_enqueue.argtypes = [vp, vp, vp, u64, C.POINTER(_abi.m2s_3dgs_params), vp, u64, vp, vp, vp]
+    L.m2s_3dgs_render_grad.restype = i32
+    L.m2s_3dgs_render_grad.argtypes = [vp, vp, vp, u64, C.POINTER(_abi.m2s_3dgs_params), vp, C.POINTER(u64)]
+    L.m2s_3dgs_backward_enqueue.restype = i32
+    L.m2s_3dgs_backward_enqueue.argtypes = [vp, vp, vp, u64, C.POINTER(_abi.m2s_3dgs_params), vp, vp, vp]
     _lib = L
     return L
 

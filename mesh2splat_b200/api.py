@@ -492,6 +492,24 @@ class Context:
                                                           buffer_degree, degree, ptr("rgba32f"), ptr("rgba8"), *budget))
         return images, drawn, npairs
 
+    def gs3d_state(self) -> "Gs3dState":
+        """A state of the 3DGS render's backward pass (m2s_3dgs_state): holds one forward pass of render_3dgs_grad until
+        its backward.  Free it (or use it as a context manager) before the context."""
+        return Gs3dState(self)
+
+    def render_3dgs_grad(self, params, state: "Gs3dState", world_to_view, view_to_clip, model_to_world, width: int, height: int,
+                         near: float = 0.2, scale_modifier: float = 1.0, background=(0.0, 0.0, 0.0), max_pairs: int | None = None):
+        """The standard 3DGS render of PACKED56 gaussians as a differentiable torch operation: params is a (count, 14)
+        float32 CUDA tensor (xyz, quaternion wxyz, log-scale, SH0, opacity logit; e.g. out.data[:n * 56].view(torch.float32)
+        .view(n, 14)).  Returns the (height, width, 4) RGBA32F image (row 0 = the bottom row), bit for bit render_3dgs's.
+        Its backward (m2s_3dgs_backward_enqueue on torch's current stream, no synchronisation) fills params.grad.
+        max_pairs None: m2s_3dgs_render_grad (every survivor drawn; one read-back of the pair count); otherwise
+        m2s_3dgs_render_grad_enqueue on torch's current stream with that pair budget.  The state keeps this forward pass
+        until the next one that uses it; the backward of an older one raises."""
+        p = _abi.make_3dgs_params(world_to_view, view_to_clip, model_to_world, width, height, near, 1.0, scale_modifier, background,
+                                  _abi.LAYOUT_PACKED56)
+        return _Render3dgsGrad.apply(params, self, state, p, max_pairs)
+
     def gs3d_preprocess(self, records, count: int, layout: int, world_to_view, view_to_clip, model_to_world, width: int, height: int,
                         near: float = 0.2, std_dev: float = 1.0, scale_modifier: float = 1.0, sh=None, sh_degree: int | None = None):
         """The 3DGS render's preprocess kernel alone (m2s_debug_3dgs_preprocess, not in m2s.h): (splat records [count, 12]
@@ -656,6 +674,19 @@ def ply_parse_file(path: str) -> _abi.m2s_ply_info:
     return ply_parse_header(head, os.path.getsize(path))
 
 
+def write_3dgs_ply(path: str, params) -> None:
+    """PACKED56 gaussians (an (n, 14) float32 array or tensor: xyz, quaternion wxyz, log-scale, SH0, opacity logit) as a
+    standard 3DGS .ply: the header of m2s_ply_header format 0 (LAYOUT_PLY_STANDARD), the fields as they are, zero normals
+    and f_rest."""
+    a = params.detach().cpu().numpy() if hasattr(params, "detach") else np.asarray(params)
+    a = np.asarray(a, np.float32).reshape(-1, 14)
+    rows = np.zeros(len(a), _abi.record_dtype(_abi.LAYOUT_PLY_STANDARD))
+    rows["xyz"], rows["f_dc"], rows["opacity"], rows["scale"], rows["rot"] = a[:, 0:3], a[:, 10:13], a[:, 13], a[:, 7:10], a[:, 3:7]
+    with open(path, "wb") as f:
+        f.write(ply_header(0, len(a)))
+        f.write(rows.tobytes())
+
+
 def ply_write(path: str, ref96: np.ndarray, fmt: int, scale_multiplier: float) -> None:
     a = np.ascontiguousarray(ref96)
     count = a.nbytes // 96
@@ -665,6 +696,82 @@ def ply_write(path: str, ref96: np.ndarray, fmt: int, scale_multiplier: float) -
 # ---------------------------------------------------------------------------------------------
 # reference-shaped objects
 # ---------------------------------------------------------------------------------------------
+class Gs3dState:
+    """m2s_3dgs_state: what one forward pass of Context.render_3dgs_grad keeps for its backward pass."""
+
+    def __init__(self, ctx: Context):
+        h = C.c_void_p(0)
+        check(lib().m2s_3dgs_state_create(ctx.handle, C.byref(h)))
+        self.handle = h.value
+        self.generation = 0   # counts the forward passes; a backward checks that its own is still the one held
+
+    def free(self):
+        if getattr(self, "handle", 0):
+            lib().m2s_3dgs_state_destroy(self.handle)
+            self.handle = 0
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.free()
+
+
+_CUDA_STREAM_LEGACY = 1   # cudaStreamLegacy: the default stream torch's handle 0 stands for
+
+
+def _render_3dgs_grad_class():
+    torch = _torch()
+
+    class Render3dgsGrad(torch.autograd.Function):
+        @staticmethod
+        def forward(fctx, params, ctx, state, p, max_pairs):
+            assert params.dtype == torch.float32 and params.is_cuda and params.dim() == 2 and params.shape[1] == 14, params.shape
+            params = params.detach().contiguous()
+            dev = params.device
+            count = params.shape[0]
+            img = torch.empty(p.height * p.width * 4, dtype=torch.float32, device=dev)
+            _binned_pass(dev, max_pairs, count,
+                         lambda pairs: lib().m2s_3dgs_render_grad(ctx.handle, state.handle, params.data_ptr(), count, C.byref(p),
+                                                                  img.data_ptr(), pairs),
+                         lambda *budget: lib().m2s_3dgs_render_grad_enqueue(ctx.handle, state.handle, params.data_ptr(), count,
+                                                                            C.byref(p), img.data_ptr(), *budget))
+            state.generation += 1
+            fctx.save_for_backward(params)   # torch's version counter: an in-place change before the backward raises
+            fctx.saved = (ctx, state, p, state.generation)
+            return img.view(p.height, p.width, 4)
+
+        @staticmethod
+        def backward(fctx, grad_img):
+            (params,) = fctx.saved_tensors
+            ctx, state, p, gen = fctx.saved
+            if state.generation != gen:
+                raise RuntimeError("render_3dgs_grad: the state has since held another forward pass; use one state per view")
+            g = grad_img.detach().to(torch.float32).contiguous()
+            grad = torch.empty_like(params)
+            # torch's current stream; its default stream has handle 0, which the C ABI reads as "the context's stream" (not
+            # ordered with torch's work), so that one is named as cudaStreamLegacy (0x1)
+            stream = torch.cuda.current_stream(params.device).cuda_stream or _CUDA_STREAM_LEGACY
+            check(lib().m2s_3dgs_backward_enqueue(ctx.handle, state.handle, params.data_ptr(), params.shape[0], C.byref(p), g.data_ptr(),
+                                                  grad.data_ptr(), stream))
+            return grad, None, None, None, None
+
+    return Render3dgsGrad
+
+
+class _LazyFunction:
+    """The autograd Function, made on first use (torch is imported lazily)."""
+    fn = None
+
+    def apply(self, *args):
+        if _LazyFunction.fn is None:
+            _LazyFunction.fn = _render_3dgs_grad_class()
+        return _LazyFunction.fn.apply(*args)
+
+
+_Render3dgsGrad = _LazyFunction()
+
+
 class RenderContext:
     """The fields of struct RenderContext (RenderContext.hpp:28-124) the conversion path touches."""
 

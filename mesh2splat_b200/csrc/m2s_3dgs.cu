@@ -11,20 +11,18 @@
 //                           prefix that fits the budget, stably sorted by tile, so each tile's run is depth-ordered
 //   gs3d_tile_kernel        one CTA per tile, one thread per pixel: front-to-back compositing in registers, the tile
 //                           stops once every pixel has terminated; one coalesced store per target
+// The forward pass that keeps its state for the backward pass (m2s_3dgs_grad.cu) runs the same steps with
+// gs3d_rank_kernel (the inverse of the depth order) after the sort and gs3d_tile_kernel<true>, which also stores each
+// pixel's final T and last contributor; gs3d_tile_kernel<false> is the render's kernel unchanged.
 // All arithmetic that decides a bit of the image is round-to-nearest fp32 with no contraction (__f*_rn) and rn_exp, so
 // the images equal the checker's (oracle/m2s_3dgs_oracle.c) bit for bit.
 #include "m2s_3dgs.cuh"
+#include "m2s_3dgs_proj.cuh"
 #include "m2s_bin.cuh"
-#include "m2s_gauss.cuh"
 
 namespace m2s {
 
 constexpr int kGs3dThreads = 256;
-
-// row r of the column-major 4 x 4 m applied to (x, y, z, 1): ((m_r0 x + m_r1 y) + m_r2 z) + m_r3
-__device__ __forceinline__ float gs3d_row(const float* m, int r, float x, float y, float z) {
-    return ad(ad(ad(ml(m[r], x), ml(m[4 + r], y)), ml(m[8 + r], z)), m[12 + r]);
-}
 
 // one record -> its splat record and depth key (DESIGN §2, the 3DGS render: per record); false if culled
 __device__ __forceinline__ bool gs3d_splat(const Gs3dArgs& a, unsigned long long gid, Gs3dSplat& out, uint32_t& key) {
@@ -36,51 +34,9 @@ __device__ __forceinline__ bool gs3d_splat(const Gs3dArgs& a, unsigned long long
         const float2* r = reinterpret_cast<const float2*>(a.records + gid * 56ull);
         packed56_fields<true>(__ldg(r), __ldg(r + 1), __ldg(r + 2), __ldg(r + 3), __ldg(r + 4), __ldg(r + 5), __ldg(r + 6), g);
     }
-    // ---- view and cull ----
-    const float tx = gs3d_row(a.MV, 0, g.px, g.py, g.pz), ty = gs3d_row(a.MV, 1, g.px, g.py, g.pz), tz = gs3d_row(a.MV, 2, g.px, g.py, g.pz);
-    const float d = -tz;
-    if (!(d > a.near)) return false;
-    // ---- mean in pixels (ndc2Pix) ----
-    const float c0 = gs3d_row(a.P, 0, tx, ty, tz), c1 = gs3d_row(a.P, 1, tx, ty, tz), c3 = gs3d_row(a.P, 3, tx, ty, tz);
-    const float pw = dv(1.0f, ad(c3, 1e-7f));
-    const float W = (float)a.width, H = (float)a.height;
-    const float u = ml(sb(ml(ad(ml(c0, pw), 1.0f), W), 1.0f), 0.5f), v = ml(sb(ml(ad(ml(c1, pw), 1.0f), H), 1.0f), 0.5f);
-    // ---- 3-D covariance (computeCov3D): scale, normalised rotation, Sigma = (S R^T)^T (S R^T) ----
-    const float s[3] = {ml(ml(g.sx, a.mult), a.scale_modifier), ml(ml(g.sy, a.mult), a.scale_modifier), ml(ml(g.sz, a.mult), a.scale_modifier)};
-    const float qn = fmaxf(__fsqrt_rn(ad(ad(ad(ml(g.qx, g.qx), ml(g.qy, g.qy)), ml(g.qz, g.qz)), ml(g.qw, g.qw))), 1e-12f);
-    const float qr = dv(g.qx, qn), qi = dv(g.qy, qn), qj = dv(g.qz, qn), qk = dv(g.qw, qn);   // (w, x, y, z)
-    const float R[3][3] = {{sb(1.0f, ml(2.0f, ad(ml(qj, qj), ml(qk, qk)))), ml(2.0f, sb(ml(qi, qj), ml(qr, qk))), ml(2.0f, ad(ml(qi, qk), ml(qr, qj)))},
-                           {ml(2.0f, ad(ml(qi, qj), ml(qr, qk))), sb(1.0f, ml(2.0f, ad(ml(qi, qi), ml(qk, qk)))), ml(2.0f, sb(ml(qj, qk), ml(qr, qi)))},
-                           {ml(2.0f, sb(ml(qi, qk), ml(qr, qj))), ml(2.0f, ad(ml(qj, qk), ml(qr, qi))), sb(1.0f, ml(2.0f, ad(ml(qi, qi), ml(qj, qj))))}};
-    float Mk[3][3];   // Mk[k][j] = s_k R[j][k]
-#pragma unroll
-    for (int k = 0; k < 3; ++k)
-#pragma unroll
-        for (int j = 0; j < 3; ++j) Mk[k][j] = ml(s[k], R[j][k]);
-    float S[3][3];
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-        for (int j = 0; j < 3; ++j) S[i][j] = ad(ad(ml(Mk[0][i], Mk[0][j]), ml(Mk[1][i], Mk[1][j])), ml(Mk[2][i], Mk[2][j]));
-    // ---- 2-D covariance (computeCov2D in GL axes): cov = J W Sigma W^T J^T + 0.3 I ----
-    const float fx = ml(ml(a.P[0], W), 0.5f), fy = ml(ml(a.P[5], H), 0.5f);
-    const float limx = dv(1.3f, a.P[0]), limy = dv(1.3f, a.P[5]);
-    const float txc = ml(fminf(limx, fmaxf(-limx, dv(tx, d))), d), tyc = ml(fminf(limy, fmaxf(-limy, dv(ty, d))), d);
-    const float dd = ml(d, d);
-    const float J00 = dv(fx, d), J02 = dv(ml(fx, txc), dd), J11 = dv(fy, d), J12 = dv(ml(fy, tyc), dd);
-    float T[2][3];
-#pragma unroll
-    for (int j = 0; j < 3; ++j) {
-        T[0][j] = ad(ml(J00, a.MV[4 * j + 0]), ml(J02, a.MV[4 * j + 2]));
-        T[1][j] = ad(ml(J11, a.MV[4 * j + 1]), ml(J12, a.MV[4 * j + 2]));
-    }
-    float A[2][3];
-#pragma unroll
-    for (int i = 0; i < 2; ++i)
-#pragma unroll
-        for (int j = 0; j < 3; ++j) A[i][j] = ad(ad(ml(T[i][0], S[0][j]), ml(T[i][1], S[1][j])), ml(T[i][2], S[2][j]));
-    auto cov = [&](int i, int j) { return ad(ad(ml(A[i][0], T[j][0]), ml(A[i][1], T[j][1])), ml(A[i][2], T[j][2])); };
-    const float ca = ad(cov(0, 0), 0.3f), cb = cov(0, 1), cc = ad(cov(1, 1), 0.3f);
+    Gs3dProj pr;
+    if (!gs3d_project(a, g, pr)) return false;
+    const float u = pr.u, v = pr.v, ca = pr.ca, cb = pr.cb, cc = pr.cc, d = pr.d;
     // ---- conic, radius, tile rectangle (getRect) ----
     const float det = sb(ml(ca, cc), ml(cb, cb));
     if (det == 0.0f) return false;
@@ -123,8 +79,9 @@ __global__ void __launch_bounds__(kGs3dThreads) gs3d_preprocess_kernel(const __g
 }
 
 // ---- binning (m2s_bin.cuh): the survivors in depth order, pair value = record index ---------------------------------------
-struct Gs3dBins {
-    Gs3dArgs a;
+template <typename A>
+struct Gs3dBinner {
+    A a;
     __host__ __device__ unsigned long long items() const { return a.count; }
     __host__ __device__ uint64_t tiles() const { return tile_count(a.width, a.height); }
     __device__ __forceinline__ uint32_t n() const { return a.ctrl[1]; }
@@ -139,20 +96,25 @@ struct Gs3dBins {
         return (x1 - x0) * (y1 - y0);
     }
 };
+struct Gs3dBins : Gs3dBinner<Gs3dArgs> {};
+struct Gs3dSaveBins : Gs3dBinner<Gs3dSaveArgs> {};   // the same pairs; the arguments carry the forward state
 
 // ---- tile kernel: front-to-back compositing (renderCUDA) ------------------------------------------------------------------
-constexpr int kGs3dVaryings = 9;   // u, v, conic.xyz, opacity, r, g, b
 struct Gs3dStage {
     float v[kGs3dVaryings][kTileThreads];
 };
 
-__global__ void __launch_bounds__(kTileThreads) gs3d_tile_kernel(Gs3dArgs a, const uint32_t* __restrict__ vals) {
+// kSave: also the per-pixel state of the backward pass (a.final_T, a.n_contrib); kSave = false is the render's kernel
+template <bool kSave>
+__global__ void __launch_bounds__(kTileThreads) gs3d_tile_kernel(std::conditional_t<kSave, Gs3dSaveArgs, Gs3dArgs> a,
+                                                                  const uint32_t* __restrict__ vals) {
     __shared__ Gs3dStage s;
     const TileFrame f = tile_frame(a.scratch, bin_layout(a.count, tile_count(a.width, a.height)), tiles_x(a.width), blockIdx.x);
     const bool inside = f.x < (int)a.width && f.y < (int)a.height;
     const float px = (float)f.x, py = (float)f.y;
     float T = 1.0f, C0 = 0.0f, C1 = 0.0f, C2 = 0.0f;
     bool done = !inside;
+    uint32_t seen = 0, last = 0;   // kSave: the run positions this pixel has visited, 1 + its last blended one
     auto stage = [&](int tid, uint32_t val) {
         const Gs3dSplat sp = a.splats[val];
         s.v[0][tid] = sp.a.x; s.v[1][tid] = sp.a.y; s.v[2][tid] = sp.a.z; s.v[3][tid] = sp.a.w;
@@ -162,6 +124,7 @@ __global__ void __launch_bounds__(kTileThreads) gs3d_tile_kernel(Gs3dArgs a, con
         f, vals, stage,
         [&](uint32_t j) {
             if (done) return;
+            if constexpr (kSave) ++seen;
             const float dx = sb(s.v[0][j], px), dy = sb(s.v[1][j], py);
             const float power = sb(ml(-0.5f, ad(ml(ml(s.v[2][j], dx), dx), ml(ml(s.v[4][j], dy), dy))), ml(ml(s.v[3][j], dx), dy));
             if (power > 0.0f) return;
@@ -173,6 +136,7 @@ __global__ void __launch_bounds__(kTileThreads) gs3d_tile_kernel(Gs3dArgs a, con
             C1 = ad(C1, ml(ml(s.v[7][j], alpha), T));
             C2 = ad(C2, ml(ml(s.v[8][j], alpha), T));
             T = tt;
+            if constexpr (kSave) last = seen;
         },
         [&] { return done; });
     if (!inside) return;
@@ -180,6 +144,17 @@ __global__ void __launch_bounds__(kTileThreads) gs3d_tile_kernel(Gs3dArgs a, con
     const size_t pix = (size_t)f.y * a.width + f.x;
     if (a.rgba32f) a.rgba32f[pix] = o;
     if (a.rgba8) a.rgba8[pix] = unorm8(o.x) | unorm8(o.y) << 8 | unorm8(o.z) << 16 | unorm8(o.w) << 24;
+    if constexpr (kSave) {
+        a.final_T[pix] = T;
+        a.n_contrib[pix] = last;
+    }
+}
+
+// the inverse of the depth order: rank[order[k]] = k
+__global__ void __launch_bounds__(kGs3dThreads) gs3d_rank_kernel(const uint32_t* __restrict__ order, uint32_t* __restrict__ rank,
+                                                                  unsigned long long count) {
+    const unsigned long long k = (unsigned long long)blockIdx.x * kGs3dThreads + threadIdx.x;
+    if (k < count) rank[order[k]] = (uint32_t)k;
 }
 
 // ---- launches ------------------------------------------------------------------------------------------------------------
@@ -195,11 +170,26 @@ cudaError_t gs3d_count_launch(const Gs3dArgs& a, cudaStream_t stream) {
     if (e != cudaSuccess) return e;
     e = sort_order_launch(a.keys, a.count, a.ctrl, a.order, a.sort_scratch, a.sm_count, stream);
     if (e != cudaSuccess) return e;
-    return bin_count_launch(Gs3dBins{a}, stream);
+    return bin_count_launch(Gs3dBins{{a}}, stream);
 }
 
 cudaError_t gs3d_draw_launch(const Gs3dArgs& a, int sm_count, cudaStream_t stream) {
-    return bin_draw_launch(Gs3dBins{a}, gs3d_tile_kernel, sm_count, stream);
+    return bin_draw_launch(Gs3dBins{{a}}, gs3d_tile_kernel<false>, sm_count, stream);
+}
+
+cudaError_t gs3d_count_save_launch(const Gs3dSaveArgs& a, cudaStream_t stream) {
+    cudaError_t e = gs3d_preprocess_launch(a, stream);
+    if (e != cudaSuccess) return e;
+    e = sort_order_launch(a.keys, a.count, a.ctrl, a.order, a.sort_scratch, a.sm_count, stream);
+    if (e != cudaSuccess) return e;
+    e = bin_count_launch(Gs3dSaveBins{{a}}, stream);
+    if (e != cudaSuccess || a.count == 0) return e;
+    gs3d_rank_kernel<<<(unsigned)((a.count + kGs3dThreads - 1) / kGs3dThreads), kGs3dThreads, 0, stream>>>(a.order, a.rank, a.count);
+    return cudaGetLastError();
+}
+
+cudaError_t gs3d_draw_save_launch(const Gs3dSaveArgs& a, int sm_count, cudaStream_t stream) {
+    return bin_draw_launch(Gs3dSaveBins{{a}}, gs3d_tile_kernel<true>, sm_count, stream);
 }
 
 }  // namespace m2s

@@ -103,11 +103,12 @@ struct m2s_ctx {
     m2s::Scratch compare;                    // image comparison: per-tile partial totals, then the synchronous form's result
     m2s::Scratch gs3d, gs3d_sort;            // 3DGS render: splat records, depth keys and order (Gs3dLayout); their depth sort
     m2s::BinScratch gs3d_bins;               // 3DGS render: its binning
+    m2s::Scratch gs3d_grad;                  // 3DGS backward pass: per pair slot partials, per tile run length (Gs3dGradLayout)
     // every Scratch above (m2s_ctx_destroy frees them): a member added above is added here too
     std::vector<m2s::Scratch*> all_scratch() {
         return {&out, &keys, &trifrag, &items, &sort, &light_quads, &ply_rows, &compare, &splat_bins.bins, &splat_bins.pairs,
                 &shadow_bins.bins, &shadow_bins.pairs, &depth_bins.bins, &depth_bins.pairs, &mesh_bins.bins, &mesh_bins.pairs,
-                &gs3d, &gs3d_sort, &gs3d_bins.bins, &gs3d_bins.pairs};
+                &gs3d, &gs3d_sort, &gs3d_bins.bins, &gs3d_bins.pairs, &gs3d_grad};
     }
     uint64_t ply_h2d = 0;                    // row bytes m2s_ply_read copied host -> device
 };

@@ -2,6 +2,7 @@
 // map, deferred lighting (and its split screen), mesh depth pre-pass and mesh G-buffer pass: argument checks, the
 // uniforms built on the host, and the launches.
 #include <cmath>
+#include <new>
 
 #include "m2s_3dgs.cuh"
 #include "m2s_bin.cuh"
@@ -707,13 +708,13 @@ static m2s_status gs3d_args(const char* fn, const m2s_ctx* ctx, const void* d_re
     return M2S_OK;
 }
 
-// the render's own scratch (splat records, keys, order, their sort), grown on stream
-static m2s_status gs3d_scratch(m2s_ctx* ctx, Gs3dArgs& a, cudaStream_t stream) {
+// the render's own scratch (splat records, keys, order in `own`; their sort in the context's), grown on stream
+static m2s_status gs3d_scratch(m2s_ctx* ctx, Scratch& own, Gs3dArgs& a, cudaStream_t stream) {
     const Gs3dLayout l = gs3d_layout(a.count);
-    m2s_status st = grow(ctx, ctx->gs3d, l.total_bytes, stream);
+    m2s_status st = grow(ctx, own, l.total_bytes, stream);
     if (st == M2S_OK && a.count) st = grow(ctx, ctx->gs3d_sort, sort_layout(a.count).total_bytes, stream);
     if (st != M2S_OK) return st;
-    unsigned char* base = static_cast<unsigned char*>(ctx->gs3d.p);
+    unsigned char* base = static_cast<unsigned char*>(own.p);
     a.ctrl = reinterpret_cast<uint32_t*>(base);
     a.splats = reinterpret_cast<Gs3dSplat*>(base + l.splats_off);
     a.keys = reinterpret_cast<uint32_t*>(base + l.keys_off);
@@ -738,7 +739,7 @@ static m2s_status gs3d_pass(m2s_ctx* ctx, const void* d_records, uint64_t count,
     a.rgba8 = reinterpret_cast<uint32_t*>(d_rgba8);
     CUDA_TRY(cudaSetDevice(ctx->device));
     cudaStream_t stream = pick_stream(ctx, stream_);
-    st = gs3d_scratch(ctx, a, stream);
+    st = gs3d_scratch(ctx, ctx->gs3d, a, stream);
     if (st != M2S_OK) return st;
     return bin_pass(ctx, ctx->gs3d_bins, bin_layout(count, tile_count(p->width, p->height)).total_bytes, a, gs3d_count_launch, gs3d_draw_launch,
                     stream, sync, max_pairs, pairs, d_drawn, "m2s_3dgs_render: the gaussians need 2^30 or more (tile, gaussian) pairs");
@@ -780,5 +781,120 @@ M2S_EXPORT m2s_status m2s_debug_3dgs_preprocess(m2s_ctx* ctx, const void* d_reco
     CUDA_TRY(cudaMemcpyAsync(ctrl, a.ctrl, sizeof(ctrl), cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     if (survivors) *survivors = ctrl[1];
+    return M2S_OK;
+}
+
+// ---- the standard 3DGS render's backward pass (beyond the reference): graphdeco's backward, DESIGN §2 ----------------------
+// A state owns what one forward pass keeps for its backward pass: the render's scratch (splat records, keys, order), its
+// binning (ranges, drawn prefix, sorted pairs) and the save buffers (ranks, final T, last contributors), and the
+// arguments that forward pass ran with.
+struct m2s_3dgs_state {
+    int device = 0;
+    Scratch gs3d, save;
+    BinScratch bins;
+    bool valid = false;    // holds a forward pass
+    Gs3dSaveArgs args;     // that forward pass's arguments and scratch pointers (the budget it drew)
+};
+
+M2S_EXPORT m2s_status m2s_3dgs_state_create(m2s_ctx* ctx, m2s_3dgs_state** out) {
+    if (!ctx || !out) return invalid("m2s_3dgs_state_create", "NULL argument");
+    m2s_3dgs_state* s = new (std::nothrow) m2s_3dgs_state();
+    if (!s) return invalid("m2s_3dgs_state_create", "out of host memory");
+    s->device = ctx->device;
+    *out = s;
+    return M2S_OK;
+}
+
+M2S_EXPORT void m2s_3dgs_state_destroy(m2s_3dgs_state* s) {
+    if (!s) return;
+    cudaSetDevice(s->device);
+    for (Scratch* b : {&s->gs3d, &s->save, &s->bins.bins, &s->bins.pairs})
+        if (b->p) cudaFree(b->p);   // synchronising: the passes that use the state are done before its memory goes
+    delete s;
+}
+
+// the checks both calls share: a PACKED56 state call on ctx's device
+static m2s_status gs3d_state_ok(const char* fn, const m2s_ctx* ctx, const m2s_3dgs_state* s, const m2s_3dgs_params* p) {
+    if (!ctx || !s || !p) return invalid(fn, "NULL argument");
+    if (p->layout != M2S_LAYOUT_PACKED56) return invalid(fn, "layout PACKED56 only");
+    if (s->device != ctx->device) return invalid(fn, "the state belongs to another device");
+    return M2S_OK;
+}
+
+// both forms of the forward pass that keeps its state: the render's checks and arguments, the state's scratch, bin_pass
+static m2s_status gs3d_grad_pass(m2s_ctx* ctx, m2s_3dgs_state* s, const float* d_params, uint64_t count, const m2s_3dgs_params* p,
+                                 float* d_rgba32f, void* stream_, bool sync, uint64_t max_pairs, uint64_t* pairs, uint32_t* d_drawn) {
+    const char* fn = "m2s_3dgs_render_grad";
+    m2s_status st = gs3d_state_ok(fn, ctx, s, p);
+    if (st != M2S_OK) return st;
+    Gs3dSaveArgs a;
+    std::memset(&a, 0, sizeof(a));
+    st = gs3d_args(fn, ctx, d_params, count, nullptr, p, nullptr, 0, 0, a);
+    if (st != M2S_OK) return st;
+    if (!d_rgba32f) return invalid(fn, "NULL RGBA32F target");
+    if (!aligned_ok(fn, "the RGBA32F target must be 16-byte aligned", {{d_rgba32f, 16}}) || !pair_budget_ok(fn, max_pairs)) return M2S_E_INVALID;
+    a.rgba32f = reinterpret_cast<float4*>(d_rgba32f);
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    cudaStream_t stream = pick_stream(ctx, stream_);
+    s->valid = false;
+    st = gs3d_scratch(ctx, s->gs3d, a, stream);
+    const Gs3dSaveLayout sl = gs3d_save_layout(count, p->width, p->height);
+    if (st == M2S_OK) st = grow(ctx, s->save, sl.total_bytes, stream);
+    if (st != M2S_OK) return st;
+    unsigned char* base = static_cast<unsigned char*>(s->save.p);
+    a.rank = reinterpret_cast<uint32_t*>(base + sl.rank_off);
+    a.final_T = reinterpret_cast<float*>(base + sl.final_T_off);
+    a.n_contrib = reinterpret_cast<uint32_t*>(base + sl.contrib_off);
+    st = bin_pass(ctx, s->bins, bin_layout(count, tile_count(p->width, p->height)).total_bytes, a, gs3d_count_save_launch,
+                  gs3d_draw_save_launch, stream, sync, max_pairs, pairs, d_drawn,
+                  "m2s_3dgs_render_grad: the gaussians need 2^30 or more (tile, gaussian) pairs");
+    if (st != M2S_OK) return st;
+    s->args = a;
+    s->valid = true;
+    return M2S_OK;
+}
+
+M2S_EXPORT m2s_status m2s_3dgs_render_grad_enqueue(m2s_ctx* ctx, m2s_3dgs_state* state, const float* d_params, uint64_t count,
+                                                   const m2s_3dgs_params* p, float* d_rgba32f, uint64_t max_pairs, uint64_t* d_pairs,
+                                                   uint32_t* d_drawn, void* stream_) {
+    return gs3d_grad_pass(ctx, state, d_params, count, p, d_rgba32f, stream_, false, max_pairs, d_pairs, d_drawn);
+}
+
+M2S_EXPORT m2s_status m2s_3dgs_render_grad(m2s_ctx* ctx, m2s_3dgs_state* state, const float* d_params, uint64_t count,
+                                           const m2s_3dgs_params* p, float* d_rgba32f, uint64_t* pairs) {
+    return gs3d_grad_pass(ctx, state, d_params, count, p, d_rgba32f, nullptr, true, 0, pairs, nullptr);
+}
+
+M2S_EXPORT m2s_status m2s_3dgs_backward_enqueue(m2s_ctx* ctx, const m2s_3dgs_state* s, const float* d_params, uint64_t count,
+                                                const m2s_3dgs_params* p, const float* d_grad_rgba32f, float* d_grad_params, void* stream_) {
+    const char* fn = "m2s_3dgs_backward";
+    m2s_status st = gs3d_state_ok(fn, ctx, s, p);
+    if (st != M2S_OK) return st;
+    if (!s->valid) return invalid(fn, "the state holds no forward pass");
+    Gs3dGradArgs g;
+    std::memset(&g, 0, sizeof(g));
+    st = gs3d_args(fn, ctx, d_params, count, nullptr, p, nullptr, 0, 0, g.a);
+    if (st != M2S_OK) return st;
+    if (count != s->args.count || p->width != s->args.width || p->height != s->args.height)
+        return invalid(fn, "count, width and height must be those of the state's forward pass");
+    if (!d_grad_rgba32f || (count && !d_grad_params)) return invalid(fn, "NULL gradient buffer");
+    if (!aligned_ok(fn, "the image gradient must be 16-byte aligned, the parameter gradient 4-byte aligned",
+                    {{d_grad_rgba32f, 16}, {d_grad_params, 4}}))
+        return M2S_E_INVALID;
+    const Gs3dSaveArgs& f = s->args;
+    g.a.ctrl = f.ctrl; g.a.splats = f.splats; g.a.keys = f.keys; g.a.order = f.order;
+    g.a.max_pairs = f.max_pairs; g.a.scratch = f.scratch; g.a.pairs = f.pairs;
+    g.a.rank = f.rank; g.a.final_T = f.final_T; g.a.n_contrib = f.n_contrib;
+    g.grad_rgba = reinterpret_cast<const float4*>(d_grad_rgba32f);
+    g.grad = d_grad_params;
+    g.vals = f.max_pairs ? sort_pairs16_vals(f.pairs, f.max_pairs) : nullptr;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    cudaStream_t stream = pick_stream(ctx, stream_);
+    const Gs3dGradLayout l = gs3d_grad_layout(f.max_pairs, tile_count(p->width, p->height));
+    st = grow(ctx, ctx->gs3d_grad, l.total_bytes, stream);
+    if (st != M2S_OK) return st;
+    g.part = static_cast<float*>(ctx->gs3d_grad.p);
+    g.tile_last = reinterpret_cast<uint32_t*>(static_cast<unsigned char*>(ctx->gs3d_grad.p) + l.tile_last_off);
+    CUDA_TRY(gs3d_backward_launch(g, stream));
     return M2S_OK;
 }
