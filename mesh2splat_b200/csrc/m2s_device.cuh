@@ -24,6 +24,8 @@ constexpr float kGuard = 8192.0f;        // window-coordinate guard band (|xw| b
 constexpr int kTraceHeader = 32;
 constexpr int kTraceWarpSlots = 32;
 constexpr int kTrFragEndNs = 0;          // header word: globaltimer when the fragment kernel's last CTA ended
+constexpr int kTrFragStartNs = 1;        // ... when its first CTA started, before griddepcontrol.wait (atomicMin: the reader sets it to ~0)
+constexpr int kTrFragWaitNs = 2;         // ... when its first CTA left griddepcontrol.wait (atomicMin: the reader sets it to ~0)
 #ifndef M2S_DIRECT_MAX
 #define M2S_DIRECT_MAX 512   // a unit whose small triangles emit at most this many fragments is shaded by the raster kernel itself (<= 1024)
 #endif
@@ -130,7 +132,7 @@ struct ConvertArgs {
     uint32_t direct_ok;                // the raster kernel may shade light units itself (ConvertPlan::direct_ok)
     uint32_t claim_late;               // ... and claims its next unit once the current one is done (ConvertPlan::claim_late)
     uint32_t pair_first;               // a warp's first pass sets up units 2g and 2g + 1 on its two half warps (ConvertPlan::pair_first)
-    unsigned long long* trace;         // M2S_TRACE builds only: kTraceHeader words (kTrFragEndNs), then kTraceWarpSlots
+    unsigned long long* trace;         // M2S_TRACE builds only: kTraceHeader words (kTrFrag*Ns), then kTraceWarpSlots
                                        // per raster warp (TraceSlot, m2s_raster.cu)
     // multi-GPU fused gather (world <= 1: off).  peer_out[p] / peer_xch[p] are rank p's final buffer and
     // exchange block mapped into this process (NVLink peer memory); every rank's fragment kernel stores its

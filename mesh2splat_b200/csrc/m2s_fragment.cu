@@ -119,13 +119,25 @@ __global__ void __launch_bounds__(kFragThreads, (LAYOUT == 1 ? M2S_FRAG_THREADS_
         }
         return h;
     };
-    // launched with programmatic stream serialisation: the CTAs of this grid are placed while the raster
-    // kernel drains; everything it wrote is visible after this wait
+    // launched with programmatic stream serialisation behind the raster kernel; on its direct path the raster warps trigger
+    // this launch once they are out of units (pdl_launch_dependents), and the CTAs of this grid take the SMs as the raster
+    // CTAs exit.  They wait here until the whole raster grid has completed; everything it wrote is visible after this wait
+#ifdef M2S_TRACE
+    if (a.trace && threadIdx.x == 0) atomicMin(a.trace + kTrFragStartNs, gtimer_ns());
+#endif
     asm volatile("griddepcontrol.wait;" ::: "memory");
+#ifdef M2S_TRACE
+    if (a.trace && threadIdx.x == 0) atomicMin(a.trace + kTrFragWaitNs, gtimer_ns());
+#endif
     // the first header is loaded together with the packed counter (one global round trip instead of two before the first
-    // TMA): whatever an unused queue slot holds is discarded by the loop condition
+    // TMA): whatever an unused queue slot holds is discarded by the loop condition.  One read of the counter per CTA,
+    // shared through shared memory: every warp of the grid reading the same word at once queues ~4 200 requests on one L2
+    // line, and on the direct path this wait is the end of the step (DESIGN.md section 4)
+    __shared__ unsigned long long s_packed;
+    if (threadIdx.x == 0) s_packed = *reinterpret_cast<const volatile unsigned long long*>(a.counter);
     Hdr cur = load_hdr(blockIdx.x, a.queue_cap);
-    const unsigned long long packed = *reinterpret_cast<const volatile unsigned long long*>(a.counter);
+    __syncthreads();
+    const unsigned long long packed = s_packed;
     const uint32_t nitems = min((uint32_t)(packed >> 40), a.queue_cap);   // work items queued
     if (blockIdx.x == 0 && threadIdx.x == 0) publish_counts(a, packed & kFragMask);
     const OutRange out = out_range(a);

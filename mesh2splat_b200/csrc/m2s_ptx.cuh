@@ -1,6 +1,6 @@
 // m2s_ptx.cuh — the PTX the conversion kernels use directly: mbarrier + 1-D bulk async copy (TMA engine; SASS UBLKCP),
-// system-scope release / acquire, and the bounded wait of the fused gather; and the warp scan of the kernels' and the
-// viewer's prefix sums.
+// system-scope release / acquire, the early trigger of programmatic dependent launch, and the bounded wait of the fused
+// gather; and the warp scan of the kernels' and the viewer's prefix sums.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -78,6 +78,9 @@ __device__ __forceinline__ unsigned long long ld_acquire_sys(const unsigned long
     asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
     return v;
 }
+// programmatic dependent launch: the grid launched behind this one may be scheduled once every CTA of this grid has
+// executed this or exited.  Its griddepcontrol.wait still waits for this grid to complete and its memory to be flushed
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ unsigned long long gtimer_ns() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 // Bounded wait for a peer's flag (fused gather): a rank that never launches its kernels must not hang every GPU of the
 // node forever.  After kSpinTimeoutNs the waiter gives up, raises bit `why` in the context's status word (mapped pinned

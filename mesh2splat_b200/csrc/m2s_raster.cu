@@ -987,6 +987,12 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
 #ifdef M2S_TRACE
     const unsigned long long tr_loop_ns_ = gtimer_ns();
 #endif
+    // direct-path launches let the fragment grid launch now: its CTAs take the SMs as the raster CTAs exit and wait there
+    // (griddepcontrol.wait) until this grid has completed, instead of being launched and placed after the last exit.
+    // Every warp triggers once it is out of units, so the launch fires near the end of the slowest CTA's work; triggered at
+    // the kernel's start it made the raster warps slower.  Launches whose fragments the fragment kernel shades (REF96,
+    // the .ply rows, single-round launches) keep the launch at the grid's end: REF96 measured slower with it (DESIGN.md section 4)
+    if (kDirectOK && a.direct_ok) pdl_launch_dependents();
     help_cta<RK>(a, smem, wb, st, cq, shade, lane);
     // no CTA barrier and no grid-wide count at the end: each warp exits once its own bulk stores are complete.  A warp
     // that shades from another warp's slice is done before the help queue lets that slice be rewritten, and shared

@@ -2,8 +2,9 @@
 
 Every raster warp sums the SM cycles (clock64) it spends in each phase over ALL its units; the kernel also records each
 warp's cycles and globaltimer nanoseconds from entry to exit, which give the SM clock the cycles convert at.  Globaltimer
-stamps at each warp's entry, unit-loop exit and exit, and at the fragment kernel's end, place the raster warps' work
-inside the step, whose length comes from the events of the same call.  The trace build shows shape, not timing: its
+stamps at each warp's entry, unit-loop exit and exit, and the fragment kernel's (its first CTA's start and release from
+griddepcontrol.wait, its last CTA's end), place the raster warps' work inside the step, whose length comes from the events
+of the same call.  The trace build shows shape, not timing: its
 atomics and stamps lengthen the step.
 usage: trace_raster.py [packed56|ref96] [density] [helmet|dh|quad]"""
 import os, sys, ctypes as C
@@ -24,10 +25,10 @@ _lib.lib().m2s_debug_set_trace(C.c_void_p(tr.data_ptr()))
 flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
 out = None
 for i in range(5):
-    flush.zero_(); tr.zero_(); torch.cuda.synchronize()   # cold L2, as in bench.py
+    flush.zero_(); tr.zero_(); tr[1:3] = -1; torch.cuda.synchronize()   # cold L2, as in bench.py; ~0 under the atomicMin stamps
     out = ctx.convert(ds, R, layout, flags=_abi.FLAG_UNCAPPED, capacity=6 * R * R, out=out.data if out else None)
 trn = tr.cpu().numpy()
-frag_end = int(trn[0])   # kTrFragEndNs
+frag_end, frag_start, frag_wait = (int(v) for v in trn[:3])   # kTrFragEndNs, kTrFragStartNs, kTrFragWaitNs
 ts = trn[HEADER:].reshape(nw, SLOTS)   # the globaltimer stamps, exact in int64
 t = ts.astype(np.float64)
 _lib.lib().m2s_debug_set_trace(None)
@@ -65,5 +66,8 @@ print(f"spans of the step (globaltimer, us): CTAs {len(cta_exit)}, first entries
       f"exits spread {(cta_exit.max() - cta_exit.min()) / 1e3:.2f}")
 print(f"  launch -> first warp entry            {(first_entry.min() - start) / 1e3:8.2f}")
 print(f"  last unit-loop exit -> last CTA exit  {(cta_exit.max() - ts[:, LOOP_NS].max()) / 1e3:8.2f}")
-print(f"  last CTA exit -> step end             {(frag_end - cta_exit.max()) / 1e3:8.2f}")
+last = cta_exit.max()   # the last raster CTA's exit; < 0 below: before it
+print(f"  last raster CTA exit -> first fragment CTA resident  {(frag_start - last) / 1e3:8.2f}")
+print(f"  last raster CTA exit -> first fragment wait released {(frag_wait - last) / 1e3:8.2f}")
+print(f"  last raster CTA exit -> fragment end (step end)      {(frag_end - last) / 1e3:8.2f}")
 print(f"  step (events)                         {step_ns / 1e3:8.2f}")
