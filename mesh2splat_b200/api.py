@@ -15,6 +15,7 @@ libm2s.so.
 from __future__ import annotations
 
 import ctypes as C
+from contextlib import contextmanager
 from dataclasses import dataclass
 
 import numpy as np
@@ -99,6 +100,14 @@ class DeviceScene:
 
     def h2d_bytes(self) -> int:
         return int(lib().m2s_scene_h2d_bytes(self.handle))
+
+    def r_small_max(self) -> float:
+        """The largest density at which every triangle's candidate box is certainly small (m2s_debug_scene_r_small_max):
+        PACKED56 conversions up to it end in the raster kernel.  0 for scenes uploaded in part (no slim triangle stream)."""
+        fn = lib().m2s_debug_scene_r_small_max
+        fn.restype = C.c_float
+        fn.argtypes = [C.c_void_p]
+        return float(fn(self.handle))
 
     def free(self):
         if self.handle:
@@ -205,6 +214,19 @@ class Context:
                    allow=(_abi.M2S_E_CAPACITY,) if allow_overflow else ())
         return ConvertOutput(out, keys, int(res.total), int(res.written), int(res.cap), float(res.device_ms), layout,
                              st == _abi.M2S_E_CAPACITY)
+
+    @staticmethod
+    @contextmanager
+    def single_launch_off():
+        """Within the block, conversions that could end in the raster kernel launch the fragment kernel as well
+        (m2s_debug_set_single_off): the two-kernel route that the single launch is compared against."""
+        fn = lib().m2s_debug_set_single_off
+        fn.argtypes = [C.c_int]
+        fn(1)
+        try:
+            yield
+        finally:
+            fn(0)
 
     def convert_plan(self, dscene: DeviceScene, resolution: int, layout: int = _abi.LAYOUT_REF96, capacity: int = 0,
                      max_gaussians: int = 0, flags: int = 0, first_triangle: int = 0,

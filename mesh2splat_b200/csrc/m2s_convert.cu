@@ -17,6 +17,10 @@ M2S_EXPORT void m2s_debug_set_direct_off(int off) { g_direct_off = off != 0; }
 // route the slim stream's records are compared against
 static bool g_slim_off = false;
 M2S_EXPORT void m2s_debug_set_slim_off(int off) { g_slim_off = off != 0; }
+// Test aid: conversions that could end in the raster kernel launch the fragment kernel as well, the route the single
+// launch's count and records are compared against
+static bool g_single_off = false;
+M2S_EXPORT void m2s_debug_set_single_off(int off) { g_single_off = off != 0; }
 
 // ---- the hot path -----------------------------------------------------------------------------
 uint64_t m2s::effective_cap(const m2s_dscene* s, const m2s_params* p, uint64_t out_capacity) {
@@ -47,10 +51,13 @@ struct ConvertPlan {
     uint64_t claim_late;              // ... and claims a warp's next unit once its current one is done (< 3 units per warp)
     uint64_t direct_max;              // M2S_DIRECT_MAX: the heaviest unit (small-triangle fragments) the direct path takes
     uint64_t pair_first;              // 16-triangle units; a warp's first pass sets up units 2g and 2g + 1, one per half warp
+    uint64_t single_launch;           // the raster kernel alone: no work item can be queued, the count is its own (DESIGN §4)
 };
 
+// world: GPUs of a fused gather; two_kernels: the caller needs the fragment kernel's work at the end of the step (an
+// appended range, the host's mapped count, the per-kernel timing)
 static void convert_plan(const m2s_ctx* ctx, const m2s_dscene* s, const m2s_params* p, uint64_t out_capacity, uint32_t world,
-                         ConvertPlan* pl) {
+                         bool two_kernels, ConvertPlan* pl) {
     const uint64_t count = tri_range(p->first_triangle, p->triangle_count, s->ntri).count;
     const int klayout = (int)p->layout;
     pl->cap = effective_cap(s, p, out_capacity);
@@ -77,6 +84,10 @@ static void convert_plan(const m2s_ctx* ctx, const m2s_dscene* s, const m2s_para
         pl->unit_tris = kUnitTris / 2;
         pl->n_units = (count + pl->unit_tris - 1) / pl->unit_tris;
     }
+    // a launch on the direct path needs no fragment kernel when nothing can reach the queue: every triangle's candidate
+    // box is small at this density (the scene's bound), and units beyond M2S_DIRECT_MAX are shaded in rounds.  The last
+    // raster CTA then publishes the count
+    pl->single_launch = pl->direct_ok && !two_kernels && !g_single_off && (float)p->resolution <= s->r_small_max;
     // work-item granularity: ~8 items per SM at the expected output (O(2 R^2) fragments) so that small conversions
     // still spread over the GPU, at most 2048 fragments; an oversized row block (<= 32 rows x R pixels) takes at most
     // kMaxSplit queue slots
@@ -100,16 +111,17 @@ M2S_EXPORT m2s_status m2s_debug_convert_plan(m2s_ctx* ctx, const m2s_dscene* s, 
     if (!ctx || !s || !p || !plan) { set_error("m2s_debug_convert_plan: NULL argument"); return M2S_E_INVALID; }
     if (p->resolution < 1 || p->resolution > 4096 || p->layout > M2S_LAYOUT_PLY_COMPRESSED) { set_error("m2s_debug_convert_plan: bad params"); return M2S_E_INVALID; }
     ConvertPlan pl;
-    convert_plan(ctx, s, p, out_capacity, 1u, &pl);
+    convert_plan(ctx, s, p, out_capacity, 1u, false, &pl);
     std::memcpy(plan, &pl, sizeof(pl));
     return M2S_OK;
 }
 
-// The two kernels of one conversion on one stream.  mid != nullptr: recorded between them (measurement of the per-kernel
-// shares); the fragment kernel then launches without programmatic dependent launch, so the kernels do not overlap.
+// The kernels of one conversion on one stream: the raster kernel, then the fragment kernel unless the launch is single.
+// mid != nullptr: recorded between them (measurement of the per-kernel shares); the fragment kernel then launches without
+// programmatic dependent launch, so the kernels do not overlap.
 static cudaError_t convert_launch(int layout, const ConvertArgs& a, int raster_grid, int fragment_grid, cudaStream_t stream, cudaEvent_t mid) {
     cudaError_t e = raster_launch(layout, a, raster_grid, stream);
-    if (e != cudaSuccess) return e;
+    if (e != cudaSuccess || a.single_launch) return e;
     if (mid) { e = cudaEventRecord(mid, stream); if (e != cudaSuccess) return e; }
     return fragment_launch(layout, a, fragment_grid, mid == nullptr, stream);
 }
@@ -135,7 +147,7 @@ m2s_status m2s::convert_enqueue_impl(m2s_ctx* ctx, const m2s_dscene* s, const m2
     const int klayout = (int)p->layout;  // every layout, the .ply rows included, is written by the fragment kernel itself
     if (!aligned_ok("m2s_convert", "the output buffer must be 16-byte aligned", {{d_out, 16}})) return M2S_E_INVALID;
     ConvertPlan pl;
-    convert_plan(ctx, s, p, out_capacity, (peers && peers->world > 1) ? peers->world : 1u, &pl);
+    convert_plan(ctx, s, p, out_capacity, (peers && peers->world > 1) ? peers->world : 1u, nprev != 0 || host_total || mid, &pl);
     // scratch between the two kernels (grown on demand, kept by the context)
     m2s_status st = grow(ctx, ctx->trifrag, std::max<uint64_t>(tr.count, 1) * tri_frag_bytes(klayout), stream);
     if (st == M2S_OK) st = grow(ctx, ctx->items, pl.queue_cap * sizeof(FragItem), stream);
@@ -185,6 +197,7 @@ m2s_status m2s::convert_enqueue_impl(m2s_ctx* ctx, const m2s_dscene* s, const m2
     a.direct_ok = (uint32_t)pl.direct_ok;
     a.claim_late = (uint32_t)pl.claim_late;
     a.pair_first = (uint32_t)pl.pair_first;
+    a.single_launch = (uint32_t)pl.single_launch;
     a.trace = g_trace;
     if (peers && peers->world > 1) {
         a.world = peers->world; a.rank = peers->rank;
@@ -196,7 +209,7 @@ m2s_status m2s::convert_enqueue_impl(m2s_ctx* ctx, const m2s_dscene* s, const m2
     const int fgrid = ctx->sm_count * ctx->frag_blocks_per_sm[klayout];
     cudaError_t e = convert_launch(klayout, a, (int)pl.grid, fgrid, stream, mid);
     if (e != cudaSuccess) { ctx->dirty = true; set_error(std::string("convert launch: ") + cudaGetErrorString(e)); return M2S_E_CUDA; }
-    ctx->sched_parity ^= 1u;   // this launch's fragment kernel zeroes the other set
+    ctx->sched_parity ^= 1u;   // this launch's raster kernel zeroes the other set
     if (peers && peers->world > 1)
         CUDA_TRY(gather_wait_launch((const unsigned long long*)peers->xch[peers->rank], peers->world, a.epoch, out_capacity,
                                     (unsigned long long*)d_total, ctx->d_status, stream));
@@ -236,7 +249,8 @@ M2S_EXPORT m2s_status m2s_convert(m2s_ctx* ctx, const m2s_dscene* s, const m2s_p
 }
 
 // Measurement aid: one conversion with an event between the two kernels (no programmatic dependent launch, so they do
-// not overlap): the per-kernel shares of the step, measured live instead of read from a profile.
+// not overlap): the per-kernel shares of the step, measured live instead of read from a profile.  Always both kernels,
+// also where m2s_convert would end in the raster kernel, so the two shares keep their meaning.
 M2S_EXPORT m2s_status m2s_convert_timed(m2s_ctx* ctx, const m2s_dscene* s, const m2s_params* p, void* d_out, uint64_t out_capacity,
                                         float* raster_ms, float* fragment_ms) {
     if (!ctx) { set_error("m2s_convert_timed: ctx is NULL"); return M2S_E_INVALID; }

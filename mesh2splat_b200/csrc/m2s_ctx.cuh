@@ -91,7 +91,7 @@ struct m2s_ctx {
     int frag_blocks_per_sm[kLayouts] = {};  // fragment kernel
     unsigned long long epoch = 0;            // pairs up the ranks' calls of the fused gather
     bool dirty = true;                       // scheduler state needs a memset before the next launch
-    uint32_t sched_parity = 0;               // the scheduler set the next launch uses; its fragment kernel zeroes the other
+    uint32_t sched_parity = 0;               // the scheduler set the next launch uses; its raster kernel zeroes the other
     // scratch owned by the context (grown on demand)
     m2s::Scratch out, keys;                  // convert_host output and keys
     m2s::Scratch trifrag, items;             // between the raster and the fragment kernel: TriRec per triangle, FragItem queue
@@ -120,6 +120,9 @@ struct m2s_dscene {
     // the mip levels: the raster pass of a PACKED56 conversion reads 64 B per triangle instead of 144.  Only scenes uploaded
     // whole in one call have it; partial and lazy uploads (the host pipeline, m2s_scene_upload_range) leave it null
     float4* d_tris_slim = nullptr;
+    // with the slim stream: the largest density at which every triangle's candidate box is certainly small (slim_tris_kernel,
+    // m2s_scene.cu), so that no conversion up to it queues work for the fragment kernel (ConvertPlan::single_launch)
+    float r_small_max = 0.0f;
     m2s::DRange* d_ranges = nullptr;
     uint32_t nranges = 0;
     m2s::DPrim* d_prims = nullptr;

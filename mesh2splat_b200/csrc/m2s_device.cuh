@@ -114,16 +114,17 @@ struct ConvertArgs {
     unsigned long long* counter;       // low 40 bits: fragments generated (the reference's atomic counter), high 24 bits:
                                        // work items queued; this launch's scheduler set (below), final when the fragment
                                        // kernel starts: every CTA reads its item count there
-    unsigned long long* total_out;     // receives the final count (the fragment kernel's CTA 0)
+    unsigned long long* total_out;     // receives the final count (the fragment kernel's CTA 0; on single launches the
+                                       // raster kernel's last CTA)
     const unsigned long long* prev_totals;  // appended launches: counts of the earlier chunks (records start after them)
     uint32_t nprev;
     unsigned long long* host_total;    // optional, mapped pinned host memory: {count, tag} written by the fragment kernel's
     unsigned long long host_tag;       // CTA 0 as it starts, so the host can size the download while the kernel still runs
     // scheduling state: two sets {unit counter, packed counter} in the context, alternated by launch (m2s_ctx::sched_parity).
-    // This launch's set is zero at launch; its fragment kernel zeroes the other set for the next launch, which starts only
-    // once this launch's fragment kernel has ended (stream order: the raster kernel is launched without PDL)
+    // This launch's set is zero at launch; its raster kernel zeroes the other set for the next launch as it starts: the
+    // launch before, which used that set, has ended by then (stream order: the raster kernel is launched without PDL)
     uint32_t* claim;                   // this launch's unit counter (the set of `counter`)
-    uint32_t* next_claim;              // the next launch's set, zeroed by this launch's fragment kernel
+    uint32_t* next_claim;              // the next launch's set, zeroed by this launch's raster kernel
     unsigned long long* next_counter;
     uint32_t* sched;                   // words 128 B apart (SCHED): 6 fragment CTAs finished (fused gather); SCHED 0-3 are
                                        // the two sets (m2s_ctx::d_sched)
@@ -132,6 +133,8 @@ struct ConvertArgs {
     uint32_t direct_ok;                // the raster kernel may shade light units itself (ConvertPlan::direct_ok)
     uint32_t claim_late;               // ... and claims its next unit once the current one is done (ConvertPlan::claim_late)
     uint32_t pair_first;               // a warp's first pass sets up units 2g and 2g + 1 on its two half warps (ConvertPlan::pair_first)
+    uint32_t single_launch;            // no fragment kernel follows: the raster kernel shades every unit and publishes the
+                                       // count itself (ConvertPlan::single_launch)
     unsigned long long* trace;         // M2S_TRACE builds only: kTraceHeader words (kTrFrag*Ns), then kTraceWarpSlots
                                        // per raster warp (TraceSlot, m2s_raster.cu)
     // multi-GPU fused gather (world <= 1: off).  peer_out[p] / peer_xch[p] are rank p's final buffer and

@@ -70,8 +70,7 @@ __device__ __noinline__ void micro_item(const ConvertArgs& a, uint32_t it, uint4
 }
 
 // Thread 0 of CTA 0, once the raster grid has ended: the launch's count -> total_out, the host's mapped slot and (fused
-// gather) every peer, before any CTA waits for the peers' counts; then the other scheduler set is zeroed for the next
-// launch (ConvertArgs::next_claim).  Out of line: the kernel's other threads never run it.
+// gather) every peer, before any CTA waits for the peers' counts.  Out of line: the kernel's other threads never run it.
 __device__ __noinline__ void publish_counts(const ConvertArgs& a, unsigned long long tot) {
     *a.total_out = tot;
     if (a.host_total) {  // zero-copy count for the host (PCIe posted write, ~1 us): the count is ordered before its tag
@@ -85,8 +84,6 @@ __device__ __noinline__ void publish_counts(const ConvertArgs& a, unsigned long 
         __threadfence_system();
         for (uint32_t p = 0; p < a.world; ++p) st_release_sys(a.peer_xch[p] + a.rank * 4 + 1, a.epoch);
     }
-    *a.next_claim = 0;
-    *a.next_counter = 0ull;
 }
 
 template <int LAYOUT>

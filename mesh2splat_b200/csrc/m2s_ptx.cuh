@@ -80,6 +80,11 @@ __device__ __forceinline__ unsigned long long ld_acquire_sys(const unsigned long
 }
 // programmatic dependent launch: the grid launched behind this one may be scheduled once every CTA of this grid has
 // executed this or exited.  Its griddepcontrol.wait still waits for this grid to complete and its memory to be flushed
+__device__ __forceinline__ unsigned long long atom_add_acq_rel_gpu(unsigned long long* p, unsigned long long v) {
+    unsigned long long old;
+    asm volatile("atom.add.acq_rel.gpu.global.u64 %0, [%1], %2;" : "=l"(old) : "l"(p), "l"(v) : "memory");
+    return old;
+}
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ unsigned long long gtimer_ns() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 // Bounded wait for a peer's flag (fused gather): a rank that never launches its kernels must not hang every GPU of the

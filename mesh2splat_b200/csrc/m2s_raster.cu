@@ -33,12 +33,15 @@
 //   DIRECT path (PACKED56, launches where the warps take several units each): the small triangles of a light unit are
 //     shaded by the warp that rasterised them, straight from the records in its shared-memory slice (direct_run); each
 //     group of 32 records leaves through one bulk async copy
+//   SINGLE launches (ConvertPlan::single_launch: the direct path, no larger triangle possible at the density, nothing
+//     appended): every unit is direct, no fragment kernel follows, and the grid's last CTA publishes the count
 //
 // Bit-exactness: every float operation of the per-triangle stage is written with __f*_rn intrinsics in the
 // operation order of the oracle (and of GLM, which the reference's GLSL-as-C++ build uses): coverage is
 // bit-exact and Scale/Quaternion match converterGS.glsl bit for bit.  Per-fragment values may use FMA
 // contraction / fast reciprocals and are compared with a tolerance.
 #include <type_traits>
+#include "m2s_plane.cuh"
 #include "m2s_ptx.cuh"
 #include "m2s_shade.cuh"
 
@@ -62,24 +65,6 @@ static_assert(kTrExitNs < kTraceWarpSlots, "trace slots per raster warp");
 #define TR_PHASE(a, s) do { } while (0)
 #define TR_ADD(a, s, v) do { } while (0)
 #endif
-
-// ------------------------------------------------------------------------------------------
-// exact fp32 (one rounding per operation, GLM operation order)
-// ------------------------------------------------------------------------------------------
-struct f3 {
-    float x, y, z;
-};
-__device__ __forceinline__ f3 sub3(f3 a, f3 b) { return {__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y), __fsub_rn(a.z, b.z)}; }
-__device__ __forceinline__ f3 scale3(f3 a, float s) { return {__fmul_rn(a.x, s), __fmul_rn(a.y, s), __fmul_rn(a.z, s)}; }
-__device__ __forceinline__ float dot3(f3 a, f3 b) {
-    return __fadd_rn(__fadd_rn(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)), __fmul_rn(a.z, b.z));
-}
-__device__ __forceinline__ float len3(f3 a) { return __fsqrt_rn(dot3(a, a)); }
-__device__ __forceinline__ f3 norm3(f3 a) { return scale3(a, __fdiv_rn(1.0f, __fsqrt_rn(dot3(a, a)))); }
-__device__ __forceinline__ f3 cross3(f3 x, f3 y) {
-    return {__fsub_rn(__fmul_rn(x.y, y.z), __fmul_rn(y.y, x.z)), __fsub_rn(__fmul_rn(x.z, y.x), __fmul_rn(y.z, x.x)),
-            __fsub_rn(__fmul_rn(x.x, y.y), __fmul_rn(y.x, x.y))};
-}
 
 template <int RK>
 struct __align__(128) WarpBlock {
@@ -193,29 +178,10 @@ __device__ __forceinline__ uint32_t setup_triangle(const float4* __restrict__ t4
     const TriVerts tv = tri_verts<RK == 1>(t4);
     const f3 P0 = tv.P[0], P1 = tv.P[1], P2 = tv.P[2];
 
-    // converterGS.glsl:327-347
-    f3 e1 = sub3(P1, P0), e2 = sub3(P2, P0), e3 = sub3(P2, P1);
-    const float l1 = len3(e1), l2 = len3(e2), l3 = len3(e3);
-    if (l2 > l1 && l2 > l3) { f3 tmp = e1; e1 = e2; e2 = tmp; }
-    else if (l3 > l1 && l3 > l2) { e1 = e3; }
-    e1 = norm3(e1);
-    const f3 n = norm3(cross3(e1, e2));
-    const float ax = fabsf(n.x), ay = fabsf(n.y), az = fabsf(n.z);
-    const int axis = (ax > ay && ax > az) ? 0 : ((ay > az) ? 1 : 2);
-
-    // :354-397 orthogonal uv: X -> (y,z), Y -> (x,z), Z -> (x,y), over max(range_a, range_b)
+    // converterGS.glsl:327-397: face frame and orthographic uv (m2s_plane.cuh)
+    f3 e1, n;
     float ou[3], ov[3];
-    {
-        const float mina = axis == 0 ? pr.bmin[1] : pr.bmin[0], maxa = axis == 0 ? pr.bmax[1] : pr.bmax[0];
-        const float minb = axis == 2 ? pr.bmin[1] : pr.bmin[2], maxb = axis == 2 ? pr.bmax[1] : pr.bmax[2];
-        const float ra = __fsub_rn(maxa, mina), rb = __fsub_rn(maxb, minb);
-        const float range = (ra < rb) ? rb : ra;
-        const float pa0 = axis == 0 ? P0.y : P0.x, pa1 = axis == 0 ? P1.y : P1.x, pa2 = axis == 0 ? P2.y : P2.x;
-        const float pb0 = axis == 2 ? P0.y : P0.z, pb1 = axis == 2 ? P1.y : P1.z, pb2 = axis == 2 ? P2.y : P2.z;
-        ou[0] = __fdiv_rn(__fsub_rn(pa0, mina), range); ov[0] = __fdiv_rn(__fsub_rn(pb0, minb), range);
-        ou[1] = __fdiv_rn(__fsub_rn(pa1, mina), range); ov[1] = __fdiv_rn(__fsub_rn(pb1, minb), range);
-        ou[2] = __fdiv_rn(__fsub_rn(pa2, mina), range); ov[2] = __fdiv_rn(__fsub_rn(pb2, minb), range);
-    }
+    ortho_uv(tv.P, pr, e1, n, ou, ov);
 
     // rasteriser set-up first: gl_Position = ouv*2-1 (:439), viewport R x R, 8 sub-pixel bits.  A triangle that
     // cannot emit a fragment leaves here, before the quaternion / Jacobian / sampler arithmetic
@@ -487,6 +453,20 @@ __device__ __forceinline__ void list_pixels(T* list, uint32_t k, unsigned long l
     }
 }
 
+// The full rounds of a direct pass whose list exceeds the slice: this lane's pixels sit at places k.. of the pass's list;
+// only those in the window [lo, lo + n) are listed, at place - lo.
+__device__ __forceinline__ void list_pixels_window(unsigned short* list, uint32_t k, unsigned long long hits, uint32_t w, uint32_t slot,
+                                                   uint32_t lo, uint32_t n) {
+    const uint32_t inv = (65536u + w - 1u) / w;
+    for (; k < lo && hits; ++k) hits &= hits - 1ull;   // the places before the window
+    for (; k < lo + n && hits; ++k) {
+        const uint32_t b = (uint32_t)__ffsll((long long)hits) - 1u;
+        hits &= hits - 1ull;
+        const uint32_t row = (b * inv) >> 16, col = b - row * w;
+        list[k - lo] = (unsigned short)(slot | (col << 5) | (row << 11));
+    }
+}
+
 // the unit's small triangles as one item (blocks implicit: one per triangle, TriRec::first/hits).  A unit with at
 // most 32 such fragments (sub-pixel meshes: most units of a 1 M-triangle scan) lists them in the item instead: the
 // fragment kernel then needs neither the staged unit nor its span table.  hits/w/first/slot: this lane's triangle.
@@ -658,6 +638,11 @@ __device__ __noinline__ uint32_t direct_run(const WarpBlock<1>& src, uint32_t f0
 struct DirectShare {
     uint32_t fit, done;
 };
+// places of a direct pass's list in the slice (the stash area): a pass lists up to this many fragments at once.  It holds
+// two units of M2S_DIRECT_MAX, so a pass of the two-kernel route takes one round; only single launches (every unit direct,
+// ConvertPlan::single_launch) list and shade a longer pass in rounds
+constexpr uint32_t kDirectList = 2 * M2S_DIRECT_MAX;
+static_assert(kDirectList * sizeof(unsigned short) <= sizeof(BlockRef) * kStashItems * kItemBlocks, "a round's list fits the stash");
 template <class Shade>
 __device__ __forceinline__ DirectShare direct_share(CtaQueue& cq, WarpBlock<1>& wb, uint32_t owner, uint32_t dsum, unsigned long long dfirst,
                                                     uint32_t tri0, Shade&& shade, int lane) {
@@ -790,6 +775,9 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
     const Tables tabs = copy_tables(a, smem + (size_t)C::kWarps * sizeof(WarpBlock<RK>));
     CtaQueue& cq = *reinterpret_cast<CtaQueue*>(smem + (size_t)C::kWarps * sizeof(WarpBlock<RK>) + kTableSmemBytes);
     if (threadIdx.x == 0) { cq.tail = 0; cq.head = 0; cq.active = blockDim.x >> 5; }
+    // re-arm the other scheduler set for the next launch: the launch before this one used it and has ended (no launch of
+    // this kernel overlaps the one before it), and the next one starts after this one's last kernel
+    if (blockIdx.x == 0 && threadIdx.x == 0) { *a.next_claim = 0; *a.next_counter = 0ull; }
     if (threadIdx.x < kCtaQueueCap) { cq.q[threadIdx.x].ready = 0u; cq.q[threadIdx.x].taken = 0u; }
     __syncthreads();  // tables + help queue: the only CTA-wide barrier before the end of the kernel
     // the first unit's triangles start moving only now: issued before the table copy, the first loads of all the grid's
@@ -885,9 +873,11 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         // this warp shades them itself, straight from the records in its shared-memory slice — no work item, no record
         // round trip through L2, no second kernel on the critical path.  The triangle staging area (dead since the set-up)
         // is the warp's output stage then, so the next unit's triangles start flying in after the shading instead of now.
+        // A single launch has no fragment kernel behind it: every unit is direct, however heavy
         const bool direct_ok = kDirectOK && a.direct_ok != 0;
-        const bool direct0 = direct_ok && tot0 != 0 && tot0 <= (uint32_t)M2S_DIRECT_MAX;
-        const bool direct1 = nu == 2 && direct_ok && tot1 != 0 && tot1 <= (uint32_t)M2S_DIRECT_MAX;
+        const uint32_t dmax = a.single_launch ? 0xffffffffu : (uint32_t)M2S_DIRECT_MAX;
+        const bool direct0 = direct_ok && tot0 != 0 && tot0 <= dmax;
+        const bool direct1 = nu == 2 && direct_ok && tot1 != 0 && tot1 <= dmax;
         const bool direct = direct0 || direct1;
         const uint32_t hf = (uint32_t)lane / (uint32_t)sw;                 // this lane's unit of the pass
         const unsigned hmask = sw == 32 ? 0xffffffffu : 0xffffu << (hf * 16);   // the lanes of that unit
@@ -950,13 +940,27 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
         if constexpr (kDirectOK) {
             if (direct) {
                 TR_ADD(a, kTrDirectUnits, (direct0 ? 1 : 0) + (direct1 ? 1 : 0));
-                // every lane of a direct unit lists the covered pixels of its triangle at their place in the pass's list
-                list_pixels(reinterpret_cast<unsigned short*>(wb.pend), (hf ? dfr0 : 0u) + incl_scan - nh, my_direct ? hits : 0ull,
-                            (uint32_t)w, (uint32_t)lane);
+                // every lane of a direct unit lists the covered pixels of its triangle at their place in the pass's list.  A
+                // list longer than the slice's kDirectList places (single launches only) goes in rounds: the full rounds first,
+                // each shaded before the next rewrites the list, then the rest as a pass of its own
+                uint32_t my0 = (hf ? dfr0 : 0u) + incl_scan - nh;
+                unsigned long long my_hits = my_direct ? hits : 0ull;
+                uint32_t r0 = 0;
+                if (dsum > kDirectList) {
+                    cp_async_wait_all();
+                    for (; dsum - r0 > kDirectList; r0 += kDirectList) {
+                        list_pixels_window(reinterpret_cast<unsigned short*>(wb.pend), my0, my_hits, (uint32_t)w, (uint32_t)lane, r0, kDirectList);
+                        __syncwarp();
+                        direct_share_wait(wb, direct_share(cq, wb, (uint32_t)warp, kDirectList, dfirst + r0, a.tri_first + t0, shade, lane), lane);
+                    }
+                    for (; my0 < r0 && my_hits; ++my0) my_hits &= my_hits - 1ull;   // the places listed already
+                    my0 = my0 >= r0 ? my0 - r0 : 0u;
+                }
+                list_pixels(reinterpret_cast<unsigned short*>(wb.pend), my0, my_hits, (uint32_t)w, (uint32_t)lane);
                 cp_async_wait_all();   // wb.logtab has landed (a no-op after the first direct unit)
                 __syncwarp();
                 TR_PHASE(a, kTrList);
-                const DirectShare sh = direct_share(cq, wb, (uint32_t)warp, dsum, dfirst, a.tri_first + t0, shade, lane);
+                const DirectShare sh = direct_share(cq, wb, (uint32_t)warp, dsum - r0, dfirst + r0, a.tri_first + t0, shade, lane);
                 TR_PHASE(a, kTrShade);
                 // the stage was written through the generic proxy: every writer fences before the TMA engine writes there again
                 fence_proxy_async();
@@ -994,12 +998,32 @@ __global__ void __launch_bounds__(RCfg<RK>::kWarps * 32, 1) raster_kernel(const 
     // the .ply rows, single-round launches) keep the launch at the grid's end: REF96 measured slower with it (DESIGN.md section 4)
     if (kDirectOK && a.direct_ok) pdl_launch_dependents();
     help_cta<RK>(a, smem, wb, st, cq, shade, lane);
-    // no CTA barrier and no grid-wide count at the end: each warp exits once its own bulk stores are complete.  A warp
-    // that shades from another warp's slice is done before the help queue lets that slice be rewritten, and shared
-    // memory lives until the CTA ends.  The fragment kernel reads the counts once this grid has ended (griddepcontrol.wait)
-    // and re-arms the scheduler there
+    // two-kernel launches: no CTA barrier and no grid-wide count at the end: each warp exits once its own bulk stores are
+    // complete.  A warp that shades from another warp's slice is done before the help queue lets that slice be rewritten,
+    // and shared memory lives until the CTA ends.  The fragment kernel reads the count once this grid has ended
+    // (griddepcontrol.wait)
     if (lane == 0) tma_store_wait_all();  // record stores are complete (not just read) before the kernel ends
     if constexpr (kDirectOK) cp_async_wait_all();   // a warp without a direct unit never waited for its wb.logtab
+    if constexpr (kDirectOK) {
+        if (a.single_launch) {
+            // single launches: the grid's last CTA publishes the count.  The queue half of the packed counter stays 0 on
+            // these launches (no work item), so it counts the CTAs that are done: one acq_rel add of 1 << 40 per CTA.
+            // Every reservation of the CTA precedes its add: the reservations are atomics on the same word, made by the
+            // warps before the CTA barrier below, and the barrier orders them before thread 0's add, whose release is
+            // cumulative; same-word atomics are totally ordered, so the add that finds gridDim.x - 1 CTAs before it comes
+            // after every CTA's every reservation, and the low 40 bits it returns are the final, uncapped count
+            __syncthreads();
+            if (threadIdx.x == 0) {
+                const unsigned long long old = atom_add_acq_rel_gpu(a.counter, 1ull << 40);
+                if ((uint32_t)(old >> 40) == gridDim.x - 1) {
+                    *a.total_out = old & kFragMask;
+#ifdef M2S_TRACE
+                    if (a.trace) atomicMax(a.trace + kTrFragEndNs, gtimer_ns());   // the step's end, as the trace places it
+#endif
+                }
+            }
+        }
+    }
 #ifdef M2S_TRACE
     TR_PHASE(a, kTrTail);
     TR_ADD(a, kTrCycles, clock64() - tr_c0_);   // with kTrNanos: the SM clock the cycles convert at

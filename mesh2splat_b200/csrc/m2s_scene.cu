@@ -1,6 +1,7 @@
 // m2s_scene.cu — C-ABI implementation (include/m2s.h): the device scene.  Eager and lazy upload, texture row groups and
 // their mip rows, the v-range reduction that decides which rows a triangle range samples, and the shard upload.
 #include "m2s_ctx.cuh"
+#include "m2s_plane.cuh"
 
 using namespace m2s;
 
@@ -51,19 +52,46 @@ __global__ void __launch_bounds__(256) mip_groups_kernel(uint32_t* __restrict__ 
 
 // ---- the 64-byte position/uv stream of the PACKED56 raster pass (m2s_dscene::d_tris_slim) -----------------------------------
 // One thread per output float4 k of triangle t: k < 3 is {P_k, u_k}, k = 3 is {v0, v1, v2, 0}; the values are copied, not computed.
-__global__ void __launch_bounds__(256) slim_tris_kernel(const float4* __restrict__ tris, float4* __restrict__ slim, uint64_t n4) {
+// The thread of k = 3 also bounds the density at which the triangle's candidate box is small (small_box_density); the
+// scene's minimum goes to *r_small (float bits, atomicMin: the bounds are >= 0), m2s_dscene::r_small_max.
+__global__ void __launch_bounds__(256) slim_tris_kernel(const float4* __restrict__ tris, float4* __restrict__ slim, uint64_t n4,
+                                                        const DRange* __restrict__ ranges, uint32_t nranges,
+                                                        const DPrim* __restrict__ prims, uint32_t* __restrict__ r_small) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n4) return;
     const float4* q = tris + (i >> 2) * 9;
     const uint32_t k = (uint32_t)i & 3u;
-    float4 o;
-    if (k < 3) {
-        const float4 p = __ldg(q + 3 * k), uv = __ldg(q + 3 * k + 2);
-        o = make_float4(p.x, p.y, p.z, uv.z);
-    } else {
-        o = make_float4(__ldg(q + 2).w, __ldg(q + 5).w, __ldg(q + 8).w, 0.0f);
+    float r = INFINITY;
+    if (i < n4) {
+        float4 o;
+        if (k < 3) {
+            const float4 p = __ldg(q + 3 * k), uv = __ldg(q + 3 * k + 2);
+            o = make_float4(p.x, p.y, p.z, uv.z);
+        } else {
+            o = make_float4(__ldg(q + 2).w, __ldg(q + 5).w, __ldg(q + 8).w, 0.0f);
+            const uint32_t t = (uint32_t)(i >> 2);
+            int lo = 0, hi = (int)nranges - 1, found = -1;   // the set-up's triangle -> primitive search
+            while (lo <= hi) {
+                const int mid = (lo + hi) >> 1;
+                const DRange rg = ranges[mid];
+                if (t < rg.first) hi = mid - 1;
+                else if (t >= rg.end) lo = mid + 1;
+                else { found = (int)rg.prim; break; }
+            }
+            if (found >= 0) {
+                f3 P[3], e1, n;
+                float ou[3], ov[3];
+#pragma unroll
+                for (int v = 0; v < 3; ++v) { const float4 p = __ldg(q + 3 * v); P[v] = {p.x, p.y, p.z}; }
+                ortho_uv(P, prims[found], e1, n, ou, ov);
+                const float eu = fmaxf(ou[0], fmaxf(ou[1], ou[2])) - fminf(ou[0], fminf(ou[1], ou[2]));
+                const float ev = fmaxf(ov[0], fmaxf(ov[1], ov[2])) - fminf(ov[0], fminf(ov[1], ov[2]));
+                r = small_box_density(eu, ev);
+            }
+        }
+        slim[i] = o;
     }
-    slim[i] = o;
+    const uint32_t m = __reduce_min_sync(0xffffffffu, __float_as_uint(r));
+    if ((threadIdx.x & 31u) == 0 && m != __float_as_uint(INFINITY)) atomicMin(r_small, m);
 }
 
 // ---- v-range of a triangle range per texture (host pipeline: which texture rows must be uploaded before these triangles
@@ -306,14 +334,6 @@ m2s_status m2s::scene_upload_impl(m2s_ctx* ctx, const m2s_scene* sc, m2s_dscene*
                                std::min<uint64_t>(first_tris, sc->triangle_count - tri_offset) * (size_t)kTriBytes, cudaMemcpyHostToDevice, ctx->stream));
     if (sc->triangle_count && tri_offset < sc->triangle_count && first_tris)
         d->h2d_bytes += std::min<uint64_t>(first_tris, sc->triangle_count - tri_offset) * (uint64_t)kTriBytes;
-    // a scene uploaded whole gets the 64-byte stream its PACKED56 conversions stage (+64 B per triangle), built here once
-    // behind the copy; a partial or lazy upload would have to build it per chunk and keeps the 144-byte route
-    if (sc->triangle_count && tri_offset == 0 && first_tris >= sc->triangle_count && !lazy_tex) {
-        UP_TRY(dalloc((void**)&d->d_tris_slim, sc->triangle_count * (size_t)kSlimTriBytes));
-        const uint64_t n4 = sc->triangle_count * 4;
-        slim_tris_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, ctx->stream>>>(d->d_tris, d->d_tris_slim, n4);
-        UP_TRY(cudaGetLastError());
-    }
     d->nranges = (uint32_t)ranges.size();
     UP_TRY(dalloc((void**)&d->d_ranges, ranges.size() * sizeof(DRange)));
     if (!ranges.empty())
@@ -322,6 +342,21 @@ m2s_status m2s::scene_upload_impl(m2s_ctx* ctx, const m2s_scene* sc, m2s_dscene*
     UP_TRY(dalloc((void**)&d->d_prims, prims.size() * sizeof(DPrim)));
     if (!prims.empty())
         UP_TRY(cudaMemcpyAsync(d->d_prims, prims.data(), prims.size() * sizeof(DPrim), cudaMemcpyHostToDevice, ctx->stream));
+    // a scene uploaded whole gets the 64-byte stream its PACKED56 conversions stage (+64 B per triangle), built here once
+    // behind the copies, and the density up to which every candidate box is small (r_small_max, read back once: it
+    // decides per launch whether a conversion can end in the raster kernel); a partial or lazy upload would have to build
+    // the stream per chunk and keeps the 144-byte route
+    uint32_t* d_r_small = nullptr;
+    if (sc->triangle_count && tri_offset == 0 && first_tris >= sc->triangle_count && !lazy_tex) {
+        UP_TRY(dalloc((void**)&d->d_tris_slim, sc->triangle_count * (size_t)kSlimTriBytes));
+        UP_TRY(dalloc((void**)&d_r_small, sizeof(uint32_t)));
+        UP_TRY(cudaMemsetAsync(d_r_small, 0x7f, sizeof(uint32_t), ctx->stream));   // 3.4e38: no bound yet
+        const uint64_t n4 = sc->triangle_count * 4;
+        slim_tris_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, ctx->stream>>>(d->d_tris, d->d_tris_slim, n4, d->d_ranges,
+                                                                                d->nranges, d->d_prims, d_r_small);
+        UP_TRY(cudaGetLastError());
+        UP_TRY(cudaMemcpyAsync(&d->r_small_max, d_r_small, sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+    }
     // textures: ONE arena for all mip chains (levels addressed by 32-bit texel offsets); levels 1..
     // are built on the GPU
     d->ntex = sc->texture_count;
@@ -358,7 +393,7 @@ m2s_status m2s::scene_upload_impl(m2s_ctx* ctx, const m2s_scene* sc, m2s_dscene*
     UP_TRY(dalloc((void**)&d->d_texs, d->h_texs.size() * sizeof(DTexture)));
     if (!d->h_texs.empty())
         UP_TRY(cudaMemcpyAsync(d->d_texs, d->h_texs.data(), d->h_texs.size() * sizeof(DTexture), cudaMemcpyHostToDevice, ctx->stream));
-    if (sync) UP_TRY(cudaStreamSynchronize(ctx->stream));
+    if (sync || d_r_small) UP_TRY(cudaStreamSynchronize(ctx->stream));   // r_small_max has landed
 #undef UP_TRY
     *out = d;
     return M2S_OK;
@@ -369,6 +404,9 @@ M2S_EXPORT m2s_status m2s_scene_upload(m2s_ctx* ctx, const m2s_scene* sc, m2s_ds
 }
 
 M2S_EXPORT uint64_t m2s_scene_h2d_bytes(const m2s_dscene* s) { return s ? s->h2d_bytes : 0; }
+
+// Test aid (not part of m2s.h): the scene's r_small_max (m2s_dscene); 0 when it has no slim triangle stream
+M2S_EXPORT float m2s_debug_scene_r_small_max(const m2s_dscene* s) { return s ? s->r_small_max : 0.0f; }
 
 // Test aid (not part of m2s.h): copies the scene's 64-byte position/uv stream (4 float4 per triangle) to host memory `dst`;
 // M2S_E_INVALID when the scene has none (partial and lazy uploads)

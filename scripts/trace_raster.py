@@ -3,10 +3,12 @@
 Every raster warp sums the SM cycles (clock64) it spends in each phase over ALL its units; the kernel also records each
 warp's cycles and globaltimer nanoseconds from entry to exit, which give the SM clock the cycles convert at.  Globaltimer
 stamps at each warp's entry, unit-loop exit and exit, and the fragment kernel's (its first CTA's start and release from
-griddepcontrol.wait, its last CTA's end), place the raster warps' work inside the step, whose length comes from the events
+griddepcontrol.wait, its last CTA's end; on a single launch the raster kernel's last CTA stamps the end), place the raster
+warps' work inside the step, whose length comes from the events
 of the same call.  The trace build shows shape, not timing: its
 atomics and stamps lengthen the step.
-usage: trace_raster.py [packed56|ref96] [density] [helmet|dh|quad]"""
+usage: trace_raster.py [packed56|ref96] [density] [helmet|dh|quad] [single|two]   (two: the fragment kernel is launched
+even where the conversion could end in the raster kernel)"""
 import os, sys, ctypes as C
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
@@ -15,6 +17,7 @@ from mesh2splat_b200.api import Context
 layout = {"ref96": 0, "packed56": 1}[sys.argv[1] if len(sys.argv) > 1 else "packed56"]
 R = int(sys.argv[2]) if len(sys.argv) > 2 else 512
 which = sys.argv[3] if len(sys.argv) > 3 else "helmet"
+_lib.lib().m2s_debug_set_single_off(int(len(sys.argv) > 4 and sys.argv[4] == "two"))
 ctx = Context(0)
 scene = {"helmet": lambda: synth.helmet_standin(2048), "quad": synth.unit_quad, "dh": lambda: synth.damaged_helmet_standin(2048)}[which]()
 ds = ctx.upload(scene)
@@ -67,7 +70,10 @@ print(f"spans of the step (globaltimer, us): CTAs {len(cta_exit)}, first entries
 print(f"  launch -> first warp entry            {(first_entry.min() - start) / 1e3:8.2f}")
 print(f"  last unit-loop exit -> last CTA exit  {(cta_exit.max() - ts[:, LOOP_NS].max()) / 1e3:8.2f}")
 last = cta_exit.max()   # the last raster CTA's exit; < 0 below: before it
-print(f"  last raster CTA exit -> first fragment CTA resident  {(frag_start - last) / 1e3:8.2f}")
-print(f"  last raster CTA exit -> first fragment wait released {(frag_wait - last) / 1e3:8.2f}")
-print(f"  last raster CTA exit -> fragment end (step end)      {(frag_end - last) / 1e3:8.2f}")
+if plan.single_launch:   # no fragment grid: the step ends when the raster kernel's last CTA has published the count
+    print(f"  single launch (no fragment kernel)")
+else:
+    print(f"  last raster CTA exit -> first fragment CTA resident  {(frag_start - last) / 1e3:8.2f}")
+    print(f"  last raster CTA exit -> first fragment wait released {(frag_wait - last) / 1e3:8.2f}")
+print(f"  last raster CTA exit -> step end                     {(frag_end - last) / 1e3:8.2f}")
 print(f"  step (events)                         {step_ns / 1e3:8.2f}")
